@@ -1,7 +1,7 @@
 // mwb.cu -- libmwb.so: the C ABI of include/mwb.h on top of the CUDA kernels.
 //
 //   step_kernel   (K1)  physics.cuh + reset.cuh   one warp per env
-//   render_kernel (K2)  raster.cuh                one block per env, one warp per 8x8 tile
+//   render_kernel (K2)  raster.cuh                one block per env, one warp per 8x4 half-tile
 //   scatter / gather    host <-> SoA state exchange for host-generated worlds
 //
 // Built for sm_90a (H100) only.  The same file can be compiled by g++ with -DMWB_HOSTSIM into the
@@ -86,8 +86,7 @@ struct WorldUpload {   // AoS image of one env's dynamic state (host <-> device 
   mwb_rng_state rng;
 };
 
-#define MWB_MAX_D2H_CHUNKS 32
-#define MWB_DEFAULT_D2H_CHUNKS 16   // device->host copies of a step are split into this many chunks (env MWB_D2H_CHUNKS)
+#define MWB_D2H_CHUNKS 16   // device->host copies of a step are split into this many chunks
 
 struct mwb_handle {
   mwb_config cfg;
@@ -116,8 +115,6 @@ struct mwb_handle {
   bool have_params, have_protos, have_template;
   bool profiling;
   bool frames_copied;
-  int k2_variant;
-  int k2_flags;                   // MWB_K2_* measurement switches (env MWB_K2_FLAGS)
   int obs_peer_hint;              // mwb_set_obs_peer: 1 / 0 = the caller says where observations go, -1 = look it up
   const void* peer_checked;       // last observation pointer whose home device was looked up, and the answer
   bool peer_result;
@@ -128,8 +125,7 @@ struct mwb_handle {
   int k2_parts;                   // blocks per env frame (1 at 80x60, 4 at 160x120)
 #ifndef MWB_HOSTSIM
   cudaStream_t copy_stream;
-  cudaEvent_t chunk_done[MWB_MAX_D2H_CHUNKS], copies_done;
-  int d2h_chunks;                 // pieces a host-destination frame batch is rendered + copied in
+  cudaEvent_t chunk_done[MWB_D2H_CHUNKS], copies_done;
 #endif
 #ifndef MWB_HOSTSIM
   std::vector<cudaEvent_t> ev_k1, ev_k2;   // start/stop pairs
@@ -370,7 +366,6 @@ __global__ void seed_kernel(DevState S, const WorldUpload* u, int n) {
 #else
 // host simulator: sequential stand-in for mesh_setup_kernel + render_kernel built from the
 // same MWB_DEV functions
-static long long g_tile[6];   // half-tiles, bbox hits, after edge rejection, full covers, culled by an occluder, tiles with one
 struct VecTris {
   const TriRec* t;
   const TriRec& operator()(uint32_t slot) const { return t[slot]; }
@@ -429,50 +424,16 @@ static void hostsim_render_t(const DevState& S, const RenderAssets& A, const Vie
       tris.push_back(rec);
       pairable.push_back(0);
     }
-    const bool use_pairs = !getenv("MWB_HS_NOPAIRS");
-    // test-only experiment: visit triangles front to back (MWB_HS_SORT=1); slots keep draw order
+    // like K2, visit the triangles front to back by their nearest possible depth; slots keep draw order
     std::vector<int> order(tris.size());
-    for (size_t j = 0; j < tris.size(); ++j) order[j] = (int)j;
-    if (!getenv("MWB_HS_NOSORT")) {
-      std::vector<float> zmin(tris.size());
-      for (size_t j = 0; j < tris.size(); ++j) {
-        const TriRec& t = tris[j];
-        float x0 = (float)(t.bx & 0xFFFF), x1 = (float)((t.bx >> 16) + 1), y0 = (float)(t.by & 0xFFFF), y1 = (float)((t.by >> 16) + 1);
-        zmin[j] = t.Zc + fminf(t.Za * x0, t.Za * x1) + fminf(t.Zb * y0, t.Zb * y1);
-      }
-      std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return zmin[a] < zmin[b]; });
+    std::vector<float> zmin(tris.size());
+    for (size_t j = 0; j < tris.size(); ++j) {
+      const TriRec& t = tris[j];
+      float x0 = (float)(t.bx & 0xFFFF), x1 = (float)((t.bx >> 16) + 1), y0 = (float)(t.by & 0xFFFF), y1 = (float)((t.by >> 16) + 1);
+      zmin[j] = t.Zc + fminf(t.Za * x0, t.Za * x1) + fminf(t.Zb * y0, t.Zb * y1);
+      order[j] = (int)j;
     }
-    if (getenv("MWB_HS_TILESTATS")) {   // test-only: how the half-tile level tests of K2 would triage this frame
-      for (int ty0 = 0; ty0 < H; ty0 += 4)
-        for (int tx0 = 0; tx0 < W; tx0 += 8) {
-          g_tile[0]++;
-          float occl = 65535.0f;
-          std::vector<float> zn;
-          for (size_t j = 0; j < tris.size(); ++j) {
-            const TriRec& t = tris[j];
-            const int bx0 = t.bx & 0xFFFF, bx1 = t.bx >> 16, by0 = t.by & 0xFFFF, by1 = t.by >> 16;
-            if (!(bx0 <= tx0 + 7 && bx1 >= tx0 && by0 <= ty0 + 3 && by1 >= ty0)) continue;
-            g_tile[1]++;
-            const float fx0 = (float)tx0, fy0 = (float)ty0;
-            bool hit = true, covers = true;
-            for (int k = 0; k < 3; ++k) {
-              const float e = t.A[k] * fx0 + t.B[k] * fy0;
-              if (e + t.K[k] < 0.0f) hit = false;
-              covers = covers && e + t.C[k] - t.R[k] + 8.0f * fminf(t.A[k], 0.0f) + 4.0f * fminf(t.B[k], 0.0f) > 0.0f;
-            }
-            if (!hit) continue;
-            g_tile[2]++;
-            const float zb = t.Za * fx0 + t.Zb * fy0, zmin = zb + t.Kz;
-            const float zmax = zb + t.Zc + t.Zr + 8.0f * fmaxf(t.Za, 0.0f) + 4.0f * fmaxf(t.Zb, 0.0f);
-            const float chi = zmax * 65535.0f + 1.5f;
-            zn.push_back(zmin * 65535.0f - 1.0f);
-            if (covers) g_tile[3]++;
-            if (covers && zmin >= 0.0f && zmax <= 1.0f && chi < 65535.0f) occl = fminf(occl, chi);
-          }
-          if (occl < 65535.0f) g_tile[5]++;
-          for (size_t k = 0; k < zn.size(); ++k) if (zn[k] > occl) g_tile[4]++;
-        }
-    }
+    std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return zmin[a] < zmin[b]; });
     VecTris fetch{tris.data()};
     for (int py = 0; py < H; ++py)
       for (int px = 0; px < W; ++px) {
@@ -482,7 +443,7 @@ static void hostsim_render_t(const DevState& S, const RenderAssets& A, const Vie
           const int j = order[jj];
           const TriRec& t = tris[j];
           if ((t.bx & 0xFFFF) > px || (t.bx >> 16) < px || (t.by & 0xFFFF) > py || (t.by >> 16) < py) continue;
-          const TriRec* partner = use_pairs && pairable[j] ? &tris[j ^ 1] : nullptr;
+          const TriRec* partner = pairable[j] ? &tris[j ^ 1] : nullptr;
           if (classify_pixel<MSAA>(load_class(&t), j, px, py, P, partner, (j & 1) ? 1 : 2) == 0) continue;
           if (P.mode == MWB_PX_LAZY) {     // materialise the lazily held triangle (both halves of a lazily held pair) first
             raster_pixel<MSAA>(load_hot(&tris[P.lazy_slot]), P.lazy_slot, px, py, P.keys, P.kmax);
@@ -564,7 +525,7 @@ static int k2_frame_stage_bytes(const mwb_handle* h) {
   if (h->k2_parts != 1 && (h->obs_format != MWB_OBS_HWC_U8 || (H & 3) != 0)) return 0;
   // Staging pays only when the stores leave the GPU (peer memory of rank 0: full 16-byte address-ordered stores
   // instead of 8-byte row segments, 52 % -> 89 % weak-scaling efficiency on 8 GPUs); for local HBM it costs 6 %.
-  if ((h->k2_flags & MWB_K2_NO_FRAME_STAGE) || !(h->obs_is_peer || (h->k2_flags & MWB_K2_FORCE_FRAME_STAGE))) return 0;
+  if (!h->obs_is_peer) return 0;
   // not at the price of a resident block: three blocks per SM (+ 1 KB each for the system) must still fit in 227 KB
   const size_t per_block = (size_t)k2_list_bytes(h) + bytes + (size_t)h->k2_static_smem + 1024;
   if (3 * per_block > 232448) return 0;
@@ -572,26 +533,27 @@ static int k2_frame_stage_bytes(const mwb_handle* h) {
 }
 static int k2_smem_bytes(const mwb_handle* h) { return k2_list_bytes(h) + k2_frame_stage_bytes(h); }
 
+// K2's instantiations, one per block shape x MSAA count; they share one signature.  Block shape on H100 (DESIGN.md
+// §3): 256 threads x 3 blocks / SM when one block renders a whole frame (K2 0.90 vs 1.04 ms for 4096 FourRooms envs
+// at 80x60), 320 x 3 when frames are split over several blocks (1.56 vs 1.64 ms for 512 PickupObjects envs at 160x120).
+typedef decltype(&render_kernel<1, 256, 3>) K2Kernel;
+static const K2Kernel k2_kernels[8] = {
+    render_kernel<1, 256, 3>, render_kernel<4, 256, 3>, render_kernel<8, 256, 3>, render_kernel<16, 256, 3>,
+    render_kernel<1, 320, 3>, render_kernel<4, 320, 3>, render_kernel<8, 320, 3>, render_kernel<16, 320, 3>};
+static int k2_threads(const mwb_handle* h) { return h->k2_parts == 1 ? 256 : 320; }
+static int k2_index(const mwb_handle* h) {
+  const int m = h->S.msaa;
+  return (h->k2_parts == 1 ? 0 : 4) + (m == 1 ? 0 : m == 4 ? 1 : m == 8 ? 2 : 3);
+}
+
 // The opt-in for large dynamic shared memory is an attribute of the kernel FUNCTION (per device), not of a
 // handle: several handles with different triangle capacities share it, so it is only ever raised.
-static int g_k2_smem[16][3] = {};
+static int g_k2_smem[16][8] = {};
 static int ensure_k2_smem(mwb_handle* h, int smem) {
-  const int dev = h->cfg.device & 15;
-  if (smem <= g_k2_smem[dev][h->k2_variant]) return 0;
-#define MWB_K2_ATTR(T, B, D)                                                                                               \
-  (cudaFuncSetAttribute(render_kernel<1, T, B, D>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess ||    \
-   cudaFuncSetAttribute(render_kernel<4, T, B, D>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess ||    \
-   cudaFuncSetAttribute(render_kernel<8, T, B, D>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess ||    \
-   cudaFuncSetAttribute(render_kernel<16, T, B, D>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess)
-  bool bad;
-  switch (h->k2_variant) {
-    case 0: bad = MWB_K2_ATTR(256, 3, true); break;
-    case 1: bad = MWB_K2_ATTR(320, 3, true); break;
-    default: bad = MWB_K2_ATTR(512, 2, true); break;
-  }
-#undef MWB_K2_ATTR
-  if (bad) return -1;
-  g_k2_smem[dev][h->k2_variant] = smem;
+  int& granted = g_k2_smem[h->cfg.device & 15][k2_index(h)];
+  if (smem <= granted) return 0;
+  if (cudaFuncSetAttribute(k2_kernels[k2_index(h)], cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) return -1;
+  granted = smem;
   return 0;
 }
 #endif
@@ -646,13 +608,7 @@ extern "C" int mwb_create(const mwb_config* cfg, mwb_handle** out) {
     delete h;
     return fail(MWB_ECUDA, "cudaStreamCreate failed");
   }
-  for (int c = 0; c < MWB_MAX_D2H_CHUNKS; ++c) cudaEventCreateWithFlags(&h->chunk_done[c], cudaEventDisableTiming);
-  {
-    const char* v = getenv("MWB_D2H_CHUNKS");   // tuning knob
-    h->d2h_chunks = v ? atoi(v) : MWB_DEFAULT_D2H_CHUNKS;
-    if (h->d2h_chunks < 1) h->d2h_chunks = 1;
-    if (h->d2h_chunks > MWB_MAX_D2H_CHUNKS) h->d2h_chunks = MWB_MAX_D2H_CHUNKS;
-  }
+  for (int c = 0; c < MWB_D2H_CHUNKS; ++c) cudaEventCreateWithFlags(&h->chunk_done[c], cudaEventDisableTiming);
   cudaEventCreateWithFlags(&h->copies_done, cudaEventDisableTiming);
   cudaEventCreateWithFlags(&h->last_done, cudaEventDisableTiming);
   h->last_stream = h->stream;
@@ -753,39 +709,12 @@ extern "C" int mwb_create(const mwb_config* cfg, mwb_handle** out) {
   }
   // static quads are staged in shared memory (TMA bulk copy) when they fit in 16 KB; the
   // quad capacity is kept even so that every env's block starts 16-byte aligned
-  {
-    // block shape of K2 (warps claim half-tiles from a shared counter): 0 = 256 threads x 3 blocks/SM, 1 = 320 x 3,
-    // 2 = 512 x 2; env MWB_K2_VARIANT overrides.  Default on H100: 0 when one block renders a whole frame (K2 0.90 vs
-    // 1.04 ms for 4096 FourRooms envs at 80x60), 1 when frames are split over several blocks (1.56 vs 1.64 ms for 512
-    // PickupObjects envs at 160x120).
-    const int dflt = h->k2_parts == 1 ? 0 : MWB_K2_DEFAULT_VARIANT;
-    const char* v = getenv("MWB_K2_VARIANT");
-    h->k2_variant = v ? atoi(v) : dflt;
-    if (h->k2_variant < 0 || h->k2_variant > 2) h->k2_variant = dflt;
-    const char* f = getenv("MWB_K2_FLAGS");
-    h->k2_flags = f ? atoi(f) : (MWB_K2_LISTS | MWB_K2_PAIRS);
-  }
   h->stage_bytes = (int)(((size_t)cfg->max_quads * sizeof(mwb_quad) + 15) & ~(size_t)15);
   if (h->stage_bytes > MWB_STAGE_QUAD_BYTES_HOST) h->stage_bytes = 0;
 #ifndef MWB_HOSTSIM
   {
     cudaFuncAttributes fa;
-    cudaError_t e;
-    switch (h->k2_variant) {
-      case 0: e = cfg->msaa_samples == 16 ? cudaFuncGetAttributes(&fa, render_kernel<16, 256, 3, true>)
-                : cfg->msaa_samples == 8 ? cudaFuncGetAttributes(&fa, render_kernel<8, 256, 3, true>)
-                : cfg->msaa_samples == 4 ? cudaFuncGetAttributes(&fa, render_kernel<4, 256, 3, true>)
-                                         : cudaFuncGetAttributes(&fa, render_kernel<1, 256, 3, true>); break;
-      case 1: e = cfg->msaa_samples == 16 ? cudaFuncGetAttributes(&fa, render_kernel<16, 320, 3, true>)
-                : cfg->msaa_samples == 8 ? cudaFuncGetAttributes(&fa, render_kernel<8, 320, 3, true>)
-                : cfg->msaa_samples == 4 ? cudaFuncGetAttributes(&fa, render_kernel<4, 320, 3, true>)
-                                         : cudaFuncGetAttributes(&fa, render_kernel<1, 320, 3, true>); break;
-      default: e = cfg->msaa_samples == 16 ? cudaFuncGetAttributes(&fa, render_kernel<16, 512, 2, true>)
-                : cfg->msaa_samples == 8 ? cudaFuncGetAttributes(&fa, render_kernel<8, 512, 2, true>)
-                 : cfg->msaa_samples == 4 ? cudaFuncGetAttributes(&fa, render_kernel<4, 512, 2, true>)
-                                          : cudaFuncGetAttributes(&fa, render_kernel<1, 512, 2, true>); break;
-    }
-    if (e == cudaSuccess) {
+    if (cudaFuncGetAttributes(&fa, k2_kernels[k2_index(h)]) == cudaSuccess) {
       h->k2_static_smem = (int)fa.sharedSizeBytes;
     } else {
       cudaGetLastError();
@@ -799,19 +728,10 @@ extern "C" int mwb_create(const mwb_config* cfg, mwb_handle** out) {
   }
   if (getenv("MWB_DEBUG")) {
     int nb = 0;
-    switch (h->k2_variant) {
-      case 0: cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, render_kernel<8, 256, 3, true>, 320, smem); break;
-      case 1: cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, render_kernel<8, 320, 3, true>, 320, smem); break;
-      default: cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, render_kernel<8, 512, 2, true>, 512, smem); break;
-    }
     const int launch_smem = k2_smem_bytes(h);
-    switch (h->k2_variant) {
-      case 0: cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, render_kernel<8, 256, 3, true>, 256, launch_smem); break;
-      case 1: cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, render_kernel<8, 320, 3, true>, 320, launch_smem); break;
-      default: cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, render_kernel<8, 512, 2, true>, 512, launch_smem); break;
-    }
-    fprintf(stderr, "[mwb] K2 variant %d: dynamic smem %d B (local destination), parts %d, resident blocks/SM (8x MSAA) %d\n",
-            h->k2_variant, launch_smem, h->k2_parts, nb);
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k2_kernels[k2_index(h)], k2_threads(h), launch_smem);
+    fprintf(stderr, "[mwb] K2 %d threads, %dx MSAA: dynamic smem %d B (local destination), parts %d, resident blocks/SM %d\n",
+            k2_threads(h), h->S.msaa, launch_smem, h->k2_parts, nb);
   }
 #endif
   *out = h;
@@ -836,7 +756,7 @@ extern "C" int mwb_destroy(mwb_handle* h) {
   cudaStreamSynchronize(h->copy_stream);
   for (cudaEvent_t e : h->ev_k1) cudaEventDestroy(e);
   for (cudaEvent_t e : h->ev_k2) cudaEventDestroy(e);
-  for (int c = 0; c < MWB_MAX_D2H_CHUNKS; ++c) cudaEventDestroy(h->chunk_done[c]);
+  for (int c = 0; c < MWB_D2H_CHUNKS; ++c) cudaEventDestroy(h->chunk_done[c]);
   cudaEventDestroy(h->copies_done);
   cudaEventDestroy(h->last_done);
   cudaStreamDestroy(h->copy_stream);
@@ -855,14 +775,6 @@ extern "C" int64_t mwb_overflow_count(mwb_handle* h) {
   if (d2h(&v, h->d_overflow, sizeof(int), h->stream) != 0 || sync_stream(h->stream) != 0) return -1;
   return v;
 }
-#ifdef MWB_HOSTSIM
-extern "C" void hs_counters(long long* out, int reset) {
-  for (int k = 0; k < 6; ++k) { out[k] = g_cnt[k]; if (reset) g_cnt[k] = 0; }
-}
-extern "C" void hs_tile_counters(long long* out, int reset) {
-  for (int k = 0; k < 6; ++k) { out[k] = g_tile[k]; if (reset) g_tile[k] = 0; }
-}
-#endif
 
 extern "C" int mwb_abi_sizes(int32_t* out, int cap) {
   const int32_t sz[] = {(int32_t)sizeof(mwb_config), (int32_t)sizeof(mwb_params), (int32_t)sizeof(mwb_tex_desc),
@@ -942,98 +854,95 @@ extern "C" int mwb_upload_textures(mwb_handle* h, const mwb_tex_desc* descs, int
   release_texture_objects(h);
   h->A.atlas = 0ull;
   {
-    const char* tm = getenv("MWB_K2_TMU");
-    if (!tm || atoi(tm) != 0) {
-      uint64_t hash = 1469598103934665603ull;
-      auto mix = [&hash](uint64_t v) { hash = (hash ^ v) * 1099511628211ull; };
-      mix((uint64_t)n);
-      for (int t = 0; t < n; ++t) { mix((uint64_t)td[t].w << 32 | (uint32_t)td[t].h); mix((uint64_t)td[t].nlev); }
-      for (size_t k = 0; k + 1 < pool.size(); k += 2) mix((uint64_t)pool[k] << 32 | pool[k + 1]);
-      AtlasEntry* e = nullptr;
-      for (AtlasEntry* c : g_atlases)
-        if (c->device == h->cfg.device && c->hash == hash && c->texels == pool.size()) e = c;
-      if (!e) {
-        struct Item { int t, l, w, hgt; };
-        std::vector<Item> items;
-        for (int t = 0; t < n; ++t)
-          for (int l = 0; l < td[t].nlev; ++l) items.push_back({t, l, td[t].lw[l] + 2, td[t].lh[l] + 2});
-        std::stable_sort(items.begin(), items.end(), [](const Item& a, const Item& b) { return a.hgt > b.hgt; });
-        const int AW = 4096;
-        int cx = 0, cy = 0, shelf = 0;
-        std::vector<std::pair<int, int>> at(items.size());
+    uint64_t hash = 1469598103934665603ull;
+    auto mix = [&hash](uint64_t v) { hash = (hash ^ v) * 1099511628211ull; };
+    mix((uint64_t)n);
+    for (int t = 0; t < n; ++t) { mix((uint64_t)td[t].w << 32 | (uint32_t)td[t].h); mix((uint64_t)td[t].nlev); }
+    for (size_t k = 0; k + 1 < pool.size(); k += 2) mix((uint64_t)pool[k] << 32 | pool[k + 1]);
+    AtlasEntry* e = nullptr;
+    for (AtlasEntry* c : g_atlases)
+      if (c->device == h->cfg.device && c->hash == hash && c->texels == pool.size()) e = c;
+    if (!e) {
+      struct Item { int t, l, w, hgt; };
+      std::vector<Item> items;
+      for (int t = 0; t < n; ++t)
+        for (int l = 0; l < td[t].nlev; ++l) items.push_back({t, l, td[t].lw[l] + 2, td[t].lh[l] + 2});
+      std::stable_sort(items.begin(), items.end(), [](const Item& a, const Item& b) { return a.hgt > b.hgt; });
+      const int AW = 4096;
+      int cx = 0, cy = 0, shelf = 0;
+      std::vector<std::pair<int, int>> at(items.size());
+      for (size_t k = 0; k < items.size(); ++k) {
+        if (cx + items[k].w > AW) { cx = 0; cy += shelf; shelf = 0; }
+        at[k] = {cx, cy};
+        cx += items[k].w;
+        shelf = std::max(shelf, items[k].hgt);
+      }
+      int AH = 1;
+      while (AH < cy + shelf) AH <<= 1;
+      if (AH <= 32768) {
+        e = new AtlasEntry();
+        e->device = h->cfg.device;
+        e->hash = hash;
+        e->texels = pool.size();
+        e->refs = 0;
+        e->arr = nullptr;
+        e->obj = 0;
+        e->ax.assign((size_t)n * MWB_MAX_LEVELS, 0.0f);
+        e->ay.assign((size_t)n * MWB_MAX_LEVELS, 0.0f);
+        std::vector<uint32_t> atlas((size_t)AW * AH, 0u);
         for (size_t k = 0; k < items.size(); ++k) {
-          if (cx + items[k].w > AW) { cx = 0; cy += shelf; shelf = 0; }
-          at[k] = {cx, cy};
-          cx += items[k].w;
-          shelf = std::max(shelf, items[k].hgt);
+          const Item& it = items[k];
+          const int lw = it.w - 2, lh = it.hgt - 2;
+          const uint32_t* src = pool.data() + td[it.t].off[it.l];
+          for (int y = -1; y <= lh; ++y) {
+            uint32_t* dst = &atlas[(size_t)(at[k].second + 1 + y) * AW + at[k].first];
+            const uint32_t* row = src + (size_t)((y + lh) % lh) * lw;
+            dst[0] = row[lw - 1];
+            memcpy(dst + 1, row, (size_t)lw * 4);
+            dst[lw + 1] = row[0];
+          }
+          e->ax[(size_t)it.t * MWB_MAX_LEVELS + it.l] = (float)(at[k].first + 1);
+          e->ay[(size_t)it.t * MWB_MAX_LEVELS + it.l] = (float)(at[k].second + 1);
         }
-        int AH = 1;
-        while (AH < cy + shelf) AH <<= 1;
-        if (AH <= 32768) {
-          e = new AtlasEntry();
-          e->device = h->cfg.device;
-          e->hash = hash;
-          e->texels = pool.size();
-          e->refs = 0;
-          e->arr = nullptr;
-          e->obj = 0;
-          e->ax.assign((size_t)n * MWB_MAX_LEVELS, 0.0f);
-          e->ay.assign((size_t)n * MWB_MAX_LEVELS, 0.0f);
-          std::vector<uint32_t> atlas((size_t)AW * AH, 0u);
-          for (size_t k = 0; k < items.size(); ++k) {
-            const Item& it = items[k];
-            const int lw = it.w - 2, lh = it.hgt - 2;
-            const uint32_t* src = pool.data() + td[it.t].off[it.l];
-            for (int y = -1; y <= lh; ++y) {
-              uint32_t* dst = &atlas[(size_t)(at[k].second + 1 + y) * AW + at[k].first];
-              const uint32_t* row = src + (size_t)((y + lh) % lh) * lw;
-              dst[0] = row[lw - 1];
-              memcpy(dst + 1, row, (size_t)lw * 4);
-              dst[lw + 1] = row[0];
-            }
-            e->ax[(size_t)it.t * MWB_MAX_LEVELS + it.l] = (float)(at[k].first + 1);
-            e->ay[(size_t)it.t * MWB_MAX_LEVELS + it.l] = (float)(at[k].second + 1);
-          }
-          const cudaChannelFormatDesc fmt = cudaCreateChannelDesc<uchar4>();
-          bool ok = cudaMallocArray(&e->arr, &fmt, AW, AH, cudaArrayTextureGather) == cudaSuccess;
-          if (ok) ok = cudaMemcpy2DToArray(e->arr, 0, 0, atlas.data(), (size_t)AW * 4, (size_t)AW * 4, AH, cudaMemcpyHostToDevice) == cudaSuccess;
-          if (ok) {
-            cudaResourceDesc rd;
-            memset(&rd, 0, sizeof(rd));
-            rd.resType = cudaResourceTypeArray;
-            rd.res.array.array = e->arr;
-            cudaTextureDesc tdesc;
-            memset(&tdesc, 0, sizeof(tdesc));
-            tdesc.addressMode[0] = tdesc.addressMode[1] = cudaAddressModeClamp;
-            tdesc.filterMode = cudaFilterModePoint;
-            tdesc.readMode = cudaReadModeNormalizedFloat;
-            tdesc.normalizedCoords = 1;
-            ok = cudaCreateTextureObject(&e->obj, &rd, &tdesc, nullptr) == cudaSuccess;
-          }
-          if (ok) {
-            e->iw = 1.0f / (float)AW;
-            e->ih = 1.0f / (float)AH;
-            g_atlases.push_back(e);
-          } else {
-            cudaGetLastError();
-            if (e->arr) cudaFreeArray(e->arr);
-            delete e;
-            e = nullptr;                     // the pool path stays in use
-          }
+        const cudaChannelFormatDesc fmt = cudaCreateChannelDesc<uchar4>();
+        bool ok = cudaMallocArray(&e->arr, &fmt, AW, AH, cudaArrayTextureGather) == cudaSuccess;
+        if (ok) ok = cudaMemcpy2DToArray(e->arr, 0, 0, atlas.data(), (size_t)AW * 4, (size_t)AW * 4, AH, cudaMemcpyHostToDevice) == cudaSuccess;
+        if (ok) {
+          cudaResourceDesc rd;
+          memset(&rd, 0, sizeof(rd));
+          rd.resType = cudaResourceTypeArray;
+          rd.res.array.array = e->arr;
+          cudaTextureDesc tdesc;
+          memset(&tdesc, 0, sizeof(tdesc));
+          tdesc.addressMode[0] = tdesc.addressMode[1] = cudaAddressModeClamp;
+          tdesc.filterMode = cudaFilterModePoint;
+          tdesc.readMode = cudaReadModeNormalizedFloat;
+          tdesc.normalizedCoords = 1;
+          ok = cudaCreateTextureObject(&e->obj, &rd, &tdesc, nullptr) == cudaSuccess;
+        }
+        if (ok) {
+          e->iw = 1.0f / (float)AW;
+          e->ih = 1.0f / (float)AH;
+          g_atlases.push_back(e);
+        } else {
+          cudaGetLastError();
+          if (e->arr) cudaFreeArray(e->arr);
+          delete e;
+          e = nullptr;                     // the pool path stays in use
         }
       }
-      if (e) {
-        e->refs++;
-        h->atlas = e;
-        for (int t = 0; t < n; ++t)
-          for (int l = 0; l < td[t].nlev; ++l) {
-            td[t].ax[l] = e->ax[(size_t)t * MWB_MAX_LEVELS + l];
-            td[t].ay[l] = e->ay[(size_t)t * MWB_MAX_LEVELS + l];
-          }
-        h->A.atlas = (unsigned long long)e->obj;
-        h->A.atlas_iw = e->iw;
-        h->A.atlas_ih = e->ih;
-      }
+    }
+    if (e) {
+      e->refs++;
+      h->atlas = e;
+      for (int t = 0; t < n; ++t)
+        for (int l = 0; l < td[t].nlev; ++l) {
+          td[t].ax[l] = e->ax[(size_t)t * MWB_MAX_LEVELS + l];
+          td[t].ay[l] = e->ay[(size_t)t * MWB_MAX_LEVELS + l];
+        }
+      h->A.atlas = (unsigned long long)e->obj;
+      h->A.atlas_iw = e->iw;
+      h->A.atlas_ih = e->ih;
     }
   }
 #endif
@@ -1503,19 +1412,9 @@ static int launch_k2(mwb_handle* h, uint8_t* obs, float* depth, int env0, int co
   const K2Layout lay = k2_layout(h->smem_tris, h->tri_cap, h->stage_bytes, k2_halves_per_part(h->S.obs_w, h->S.obs_h, h->k2_parts), fstage);
   if (ensure_k2_smem(h, smem)) return fail(MWB_ECUDA, "cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed");
   prof_mark(h, h->ev_k2, s);
-#define MWB_LAUNCH_K2(M, T, B, D) render_kernel<M, T, B, D><<<count * h->k2_parts, T, smem, s>>>(h->S, h->A, h->view, h->obs_format, obs, depth, env0, h->k2_parts, h->tri_cap, h->stage_bytes, fstage, h->k2_flags, lay, h->d_overflow)
-#define MWB_LAUNCH_K2_MSAA(T, B, D)                 \
-  switch (h->S.msaa) {                              \
-    case 1: MWB_LAUNCH_K2(1, T, B, D); break;       \
-    case 4: MWB_LAUNCH_K2(4, T, B, D); break;       \
-    case 16: MWB_LAUNCH_K2(16, T, B, D); break;     \
-    default: MWB_LAUNCH_K2(8, T, B, D); break;      \
-  }
-  switch (h->k2_variant) {
-    case 0: MWB_LAUNCH_K2_MSAA(256, 3, true); break;
-    case 1: MWB_LAUNCH_K2_MSAA(320, 3, true); break;
-    default: MWB_LAUNCH_K2_MSAA(512, 2, true); break;
-  }
+  k2_kernels[k2_index(h)]<<<count * h->k2_parts, k2_threads(h), smem, s>>>(h->S, h->A, h->view, h->obs_format, obs, depth, env0,
+                                                                          h->k2_parts, h->tri_cap, h->stage_bytes, fstage, lay,
+                                                                          h->d_overflow);
   prof_mark(h, h->ev_k2, s);
   h->launches++;
   CK(cudaGetLastError());
@@ -1544,7 +1443,7 @@ static int launch_render(mwb_handle* h, uint8_t* obs, float* depth, stream_t s, 
   const int N = h->S.N;
   const size_t px = (size_t)h->S.obs_w * h->S.obs_h;
   const bool pipelined = (host_obs || host_depth) && N >= 256;
-  int chunks = pipelined ? h->d2h_chunks : 1;
+  int chunks = pipelined ? MWB_D2H_CHUNKS : 1;
   while (chunks > 1 && N / chunks < 256) --chunks;   // keep every launch a few hundred blocks wide
   for (int c = 0; c < chunks; ++c) {
     const int e0 = (int)((long long)N * c / chunks), e1 = (int)((long long)N * (c + 1) / chunks);

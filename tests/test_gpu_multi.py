@@ -79,8 +79,6 @@ def _worker_one_gpu(rank, world, port, total, steps, q, flag_mode, level="MiniWo
     """Two processes on cuda:0: the peer buffer crosses a process boundary (CUDA IPC), not a GPU boundary."""
     sys.path.insert(0, ROOT)
     os.environ["MWB_FLAG_MODE"] = flag_mode
-    if staged:
-        os.environ["MWB_K2_FLAGS"] = "11"       # lists | pairs | force the frame stage although the destination is local
     import torch
     import torch.distributed as dist
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
@@ -92,6 +90,8 @@ def _worker_one_gpu(rank, world, port, total, steps, q, flag_mode, level="MiniWo
     acts_all = np.random.default_rng(5).integers(0, env.local.action_space.n, size=(steps, total), dtype=np.int32)
     env.reset(1000)
     ok = env.enable_peer_obs()
+    if ok and staged:
+        env.local.engine.set_obs_peer(True)    # stage the frame as for another GPU although the destination is local
     frames = []
     if ok:
         for t in range(steps):              # no synchronisation between the ranks inside the loop: the flags order it
