@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define MWB_ABI_VERSION 6
+#define MWB_ABI_VERSION 7
 
 /* error codes */
 #define MWB_OK 0
@@ -43,6 +43,7 @@ extern "C" {
 /* fixed capacities of the flat records */
 #define MWB_MAX_EDGES 8   /* outline vertices per room (rect rooms and connectors: 4) */
 #define MWB_MAX_OPS 64    /* reset-program length */
+#define MWB_LEVEL_CAP 32  /* levels one handle can run side by side (mwb_set_levels) */
 
 /* entity kinds (reference miniworld/entity.py: Box :386, MeshEnt :124, Agent :455) */
 #define MWB_KIND_NONE 0
@@ -274,6 +275,26 @@ int mwb_set_protos(mwb_handle* h, const mwb_proto* protos, int n);         /* en
 int mwb_set_template(mwb_handle* h, const mwb_geometry* g);                /* shared static rooms */
 int mwb_set_program(mwb_handle* h, const mwb_op* ops, int n);              /* lowered _gen_world  */
 
+/* Several levels in one batch (the reference's vector env built from a list of env constructors, each with its own
+ * level id and kwargs).  A handle holds a table of levels; mwb_create's rule fields, mwb_set_params, mwb_set_template
+ * and mwb_set_program fill level 0 of it, so a handle that never calls mwb_set_levels runs one level.
+ * mwb_set_levels replaces the whole table: level l gets templates[l] as its static rooms and the reset program
+ * ops[op_first, op_first + num_ops).  env_level[i] names the level of env i; the proto table (mwb_set_protos) is
+ * shared, so each level's ops address it with absolute indices.  Only for shared_geometry = 1 handles (MWB_EINVAL
+ * otherwise); MWB_ECAPACITY for more than MWB_LEVEL_CAP levels, a program longer than MWB_MAX_OPS or a template
+ * above the handle's max_rooms / max_quads / max_segs; MWB_EINVAL for an env_level entry outside [0, n_levels).
+ * Per-handle settings (observation size, MSAA, domain_rand, autoreset, action noise) apply to every level. */
+typedef struct mwb_level {
+  int32_t rule_kind;         /* MWB_RULE_*                                                       */
+  int32_t rule_arg;
+  int32_t max_episode_steps;
+  int32_t op_first, num_ops; /* this level's slice of the shared op array                        */
+  int32_t reserved;
+  mwb_params params;
+} mwb_level;
+int mwb_set_levels(mwb_handle* h, int n_levels, const mwb_level* levels, const mwb_geometry* templates /*[n_levels]*/,
+                   const mwb_op* ops, int n_ops, const int32_t* env_level /*[num_envs]*/);
+
 /* Maze level (reference envs/maze.py): every episode's world is a translate-and-select of these
  * templates -- one grid cell and one connector room per neighbour direction, in the order of
  * maze.py:110 `orders = [(0, 1), (0, -1), (-1, 0), (1, 0)]` as (dj, di).  All records are for
@@ -352,7 +373,9 @@ int mwb_get_state(mwb_handle* h, const mwb_state_view* out);
 /* ---- checkpointing: the complete restorable state of all N envs (entity lists, counters, camera and
  * lighting parameters, numpy streams, pending auto-resets, geometry on the device) as one host blob.
  * Restoring into a handle created with the same configuration and level definition resumes every env
- * bit for bit.  (The reference has no equivalent: its state lives in Python objects.) */
+ * bit for bit.  (The reference has no equivalent: its state lives in Python objects.)  The blob of a handle with
+ * several levels also carries env_level; restoring it into a handle with another level count or assignment fails
+ * with MWB_ESTATE. */
 int mwb_snapshot_size(mwb_handle* h, size_t* bytes);
 int mwb_snapshot(mwb_handle* h, void* blob, size_t bytes);
 int mwb_restore(mwb_handle* h, const void* blob, size_t bytes);
@@ -414,7 +437,7 @@ int mwb_flag_wait_geq(void* cuda_stream, const uint32_t* dev_ptr, uint32_t value
 int mwb_flag_mode(void);
 
 /* sizeof() of every ABI struct, in declaration order (config, params, tex_desc, mesh_desc,
- * room, quad, seg, proto, entity, op, geometry, world, rng_state, state_view, maze_desc): lets a
+ * room, quad, seg, proto, entity, op, geometry, world, rng_state, state_view, maze_desc, level): lets a
  * binding verify its mirror of this header.  Returns the number of entries written. */
 int mwb_abi_sizes(int32_t* out, int cap);
 

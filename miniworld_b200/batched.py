@@ -20,9 +20,14 @@ performs the same step with pinned host buffers for callers that want numpy.
 import numpy as np
 
 from . import pack
-from .engine import Engine, RULE_GOAL, RULE_NONE, RULE_HEALTH, RULE_PICKUP, RULE_PUTNEXT, RULE_SIDEWALK, RULE_SIGN, generator_from_state, rng_state_of, RNG_DTYPE
+from .engine import (Engine, LEVEL_CAP, OP_PLACE, OP_PUT, PROTO_DTYPE, RULE_GOAL, RULE_NONE, RULE_HEALTH, RULE_PICKUP,
+                     RULE_PUTNEXT, RULE_SIDEWALK, RULE_SIGN, generator_from_state, rng_state_of, RNG_DTYPE)
 from .envs import LEVELS
 from .program import ResetProgram
+
+
+_RULES = {"goal": RULE_GOAL, "pickup": RULE_PICKUP, "sidewalk": RULE_SIDEWALK, "sign": RULE_SIGN, "health": RULE_HEALTH,
+          "putnext": RULE_PUTNEXT, "none": RULE_NONE}
 
 
 def _resolve_level(level):
@@ -40,16 +45,48 @@ def _torch_stream(torch, device):
     return torch.cuda.current_stream(device).cuda_stream or 1
 
 
+def default_env_level(num_envs, n_levels):
+    """Level of each env when none is given: contiguous, near-equal blocks in the order the levels were listed (the
+    first num_envs % n_levels levels get one env more)."""
+    base, extra = divmod(int(num_envs), int(n_levels))
+    return np.repeat(np.arange(n_levels, dtype=np.int32), [base + (1 if k < extra else 0) for k in range(n_levels)])
+
+
 class BatchedMiniWorld:
+    """`level`: a level id or class, or a sequence of them to run several levels side by side in one batch (multi-task
+    or curriculum training; env i runs level `env_level[i]`).  With a sequence, `level_kwargs` may be a sequence
+    aligned with it, and the observation size, MSAA, domain randomisation, auto-reset and action noise are per batch.
+    Maze-family levels (per-env geometry) and Sign (dict observation) cannot share a batch with other levels."""
+
     def __init__(self, level, num_envs, obs_width=80, obs_height=60, domain_rand=False, autoreset=True,
-                 msaa_samples=8, device=0, want_depth=False, level_kwargs=None, obs_format="hwc"):
-        self.level_cls = _resolve_level(level)
-        self.level_kwargs = dict(level_kwargs or {})
+                 msaa_samples=8, device=0, want_depth=False, level_kwargs=None, obs_format="hwc", env_level=None):
         self.num_envs = int(num_envs)
         self.obs_width, self.obs_height = int(obs_width), int(obs_height)
         self.domain_rand = bool(domain_rand)
         self.want_depth = bool(want_depth)
         self.device = int(device)
+        if isinstance(level, (list, tuple)):
+            self._init_levels(list(level), level_kwargs, env_level, msaa_samples, autoreset)
+        else:
+            if env_level is not None:
+                raise ValueError("env_level assigns envs to levels: pass `level` as a sequence of levels")
+            self._init_level(level, level_kwargs, msaa_samples, autoreset)
+        # observation layout written by the render kernel: the reference's PyTorchObsWrapper ("cwh") and
+        # GreyscaleWrapper ("grey") are fused into its epilogue instead of running as separate passes
+        self.obs_format = obs_format
+        N, H, W = self.num_envs, self.obs_height, self.obs_width
+        self.obs_shape = {"hwc": (N, H, W, 3), "cwh": (N, 3, W, H), "grey": (N, H, W, 1)}[obs_format]
+        self.obs_dtype = np.float64 if obs_format == "grey" else np.uint8
+        if obs_format != "hwc":
+            self.engine.set_obs_format(obs_format)
+        self._seeded = False
+        self._torch = None
+        self._bufs = None
+
+    def _init_level(self, level, level_kwargs, msaa_samples, autoreset):
+        obs_width, obs_height, device = self.obs_width, self.obs_height, self.device
+        self.level_cls = _resolve_level(level)
+        self.level_kwargs = dict(level_kwargs or {})
 
         # a definition-only instance of the level: layout, params, rule, action space
         dr = {"domain_rand": True} if self.domain_rand else {}     # (Sign fixes domain_rand itself, like the reference)
@@ -64,7 +101,7 @@ class BatchedMiniWorld:
         if rule is None:
             raise TypeError("%s has no `device_rule`; use world.MiniWorldEnv (single env) for levels whose "
                             "step() rule is not lowered" % self.level_cls.__name__)
-        rule = {"goal": RULE_GOAL, "pickup": RULE_PICKUP, "sidewalk": RULE_SIDEWALK, "sign": RULE_SIGN, "health": RULE_HEALTH, "putnext": RULE_PUTNEXT, "none": RULE_NONE}[rule[0]], rule[1]
+        rule = _RULES[rule[0]], rule[1]
         self.device_reset = getattr(pe, "device_program", None) is not None
 
         rooms, quads, segs = pack.pack_geometry(pe)
@@ -115,17 +152,80 @@ class BatchedMiniWorld:
             # host-reset levels: one worker env per slot keeps that env's RNG stream
             self._workers = [None] * self.num_envs
             self._host_done = np.zeros(self.num_envs, bool)
-        # observation layout written by the render kernel: the reference's PyTorchObsWrapper ("cwh") and
-        # GreyscaleWrapper ("grey") are fused into its epilogue instead of running as separate passes
-        self.obs_format = obs_format
-        N, H, W = self.num_envs, self.obs_height, self.obs_width
-        self.obs_shape = {"hwc": (N, H, W, 3), "cwh": (N, 3, W, H), "grey": (N, H, W, 1)}[obs_format]
-        self.obs_dtype = np.float64 if obs_format == "grey" else np.uint8
-        if obs_format != "hwc":
-            eng.set_obs_format(obs_format)
-        self._seeded = False
-        self._torch = None
-        self._bufs = None
+        self.level_ids = [level]
+        self.proto_envs = [pe]
+        self.env_level = np.zeros(self.num_envs, np.int32)
+        self._device_info = dict(getattr(pe, "device_info", None) or {})
+        self._device_obs_extra = dict(getattr(pe, "device_obs_extra", None) or {})
+
+    def _init_levels(self, levels, level_kwargs, env_level, msaa_samples, autoreset):
+        """Several levels in one handle: each level's program is built, the proto tables are concatenated (each
+        program's proto indices moved by its level's offset), capacities are the maxima over the levels, and the
+        level table goes to the engine in one mwb_set_levels call."""
+        n = len(levels)
+        if n == 0:
+            raise ValueError("empty level list")
+        if level_kwargs is None or isinstance(level_kwargs, dict):
+            kwargs = [dict(level_kwargs or {}) for _ in range(n)]
+        else:
+            kwargs = [dict(k or {}) for k in level_kwargs]
+            if len(kwargs) != n:
+                raise ValueError("level_kwargs has %d entries for %d levels" % (len(kwargs), n))
+        if n > LEVEL_CAP:
+            raise ValueError("at most %d levels per batch, got %d" % (LEVEL_CAP, n))
+        if env_level is None:
+            env_level = default_env_level(self.num_envs, n)
+        env_level = np.asarray(env_level)
+        if env_level.shape != (self.num_envs,) or not np.issubdtype(env_level.dtype, np.integer):
+            raise ValueError("env_level must be an int array of shape (%d,), got %s %s" % (self.num_envs, env_level.dtype,
+                                                                                     env_level.shape))
+        if env_level.size and (env_level.min() < 0 or env_level.max() >= n):
+            raise ValueError("env_level entries must lie in [0, %d)" % n)
+        dr = {"domain_rand": True} if self.domain_rand else {}
+        classes = [_resolve_level(lv) for lv in levels]
+        names = [lv if isinstance(lv, str) else lv.__name__ for lv in levels]
+        pes, table, protos = [], [], []
+        caps, max_placed = [0, 0, 0], 2
+        for name, cls, kw in zip(names, classes, kwargs):
+            pe = cls(device=None, obs_width=self.obs_width, obs_height=self.obs_height, **dr, **kw)
+            rule = getattr(pe, "device_rule", None)
+            if rule is None or getattr(pe, "device_program", None) is None:
+                raise ValueError("%s resets on the host only; a batch of several levels needs device reset programs" % name)
+            if rule[0] == "sign":
+                raise ValueError("%s cannot share a batch with other levels: its observation is a dict" % name)
+            prog = ResetProgram()
+            pe.device_program(prog)
+            if prog.uses_maze:
+                raise ValueError("%s (Maze family) cannot share a batch with other levels: its geometry is per env" % name)
+            ops = prog.op_array()
+            moved = (ops["op"] == OP_PLACE) | (ops["op"] == OP_PUT)     # the ops whose `a` is a proto index
+            ops["a"][moved] += len(protos)
+            protos.extend(prog.protos)
+            geom = pack.pack_geometry(pe)
+            caps = [max(c, len(g)) for c, g in zip(caps, geom)]
+            max_placed = max(max_placed, prog.num_placed)
+            table.append(dict(rule=(_RULES[rule[0]], rule[1]), max_episode_steps=int(min(pe.max_episode_steps, 2 ** 31 - 1)),
+                              params=pe.params, geometry=geom, ops=ops))
+            pes.append(pe)
+        self.level_ids, self.proto_envs, self.env_level = names, pes, env_level.astype(np.int32)
+        self.level_cls, self.level_kwargs, self.proto_env = None, kwargs, None
+        largest = max(pes, key=lambda pe: pe.action_space.n)
+        self.action_space = self.single_action_space = largest.action_space
+        self.single_observation_space = pes[0].observation_space
+        self.max_episode_steps = [pe.max_episode_steps for pe in pes]     # per level
+        self.device_reset, self.maze_template, self.program = True, None, None
+        self.autoreset = bool(autoreset)
+        self.engine = Engine(self.num_envs, self.obs_width, self.obs_height, msaa_samples, shared_geometry=True,
+                             max_rooms=caps[0], max_quads=caps[1], max_segs=caps[2], max_ents=max_placed,
+                             rule=table[0]["rule"], domain_rand=self.domain_rand,
+                             max_episode_steps=table[0]["max_episode_steps"], autoreset=self.autoreset, device=self.device)
+        self.engine.sync_assets()
+        self.engine.set_protos(np.array(protos, PROTO_DTYPE))
+        self.engine.set_levels(table, self.env_level)
+        # a level's `info` key is returned only when every level defines it the same way
+        infos = [dict(getattr(pe, "device_info", None) or {}) for pe in pes]
+        self._device_info = {k: v for k, v in infos[0].items() if all(i.get(k) == v for i in infos[1:])}
+        self._device_obs_extra = {}
 
     # ------------------------------------------------------------------ buffers
     def _ensure_torch(self):
@@ -149,13 +249,13 @@ class BatchedMiniWorld:
             # what the level's step() puts into `info` / the observation, read in place from the device state
             eng = self.engine
             self._info_views = {}
-            for key, spec in (getattr(self.proto_env, "device_info", None) or {}).items():
+            for key, spec in self._device_info.items():
                 if spec[0] == "counter":                   # CollectHealth: info["health"] (collecthealth.py:100)
                     self._info[key] = torch.as_tensor(eng.state_array("counter"), device=dev)
                 elif spec[0] == "entity_pos":              # TMaze: info["goal_pos"] = self.box.pos (tmaze.py:89)
                     self._info_views[key] = (int(spec[1]), [torch.as_tensor(eng.state_array(n), device=dev)
                                                             for n in ("ent_x", "ent_y", "ent_z")])
-            self._obs_dict = dict(getattr(self.proto_env, "device_obs_extra", None) or {})
+            self._obs_dict = dict(self._device_obs_extra)
         return self._torch
 
     def _wrap(self, obs):
@@ -292,9 +392,12 @@ class BatchedMiniWorld:
     def render_top_view(self, render_agent=True, out=None):
         """Map view of every env in the observation layout -- uint8 [N, H, W, 3] by default (reference
         render_top_view, miniworld.py:1088-1175).
-        Extents come from the level definition (all envs of a level share them).  `out`: optional numpy
-        array / CUDA tensor to fill; default a fresh CUDA tensor."""
-        ext = self.proto_env.top_view_extents(self.obs_width, self.obs_height)
+        Extents come from the level definition (all envs of a level share them; a batch of several levels needs
+        levels with equal extents).  `out`: optional numpy array / CUDA tensor to fill; default a fresh CUDA tensor."""
+        exts = [tuple(pe.top_view_extents(self.obs_width, self.obs_height)) for pe in self.proto_envs]
+        if any(e != exts[0] for e in exts[1:]):
+            raise ValueError("render_top_view needs one map extent for the whole batch; its levels' extents differ")
+        ext = exts[0]
         if out is None:
             torch = self._ensure_torch()
             out = torch.zeros(self.obs_shape, dtype=torch.float64 if self.obs_format == "grey" else torch.uint8,

@@ -64,7 +64,11 @@ static int h2d(void* d, const void* h, size_t n, stream_t s) {
 static int d2h(void* h, const void* d, size_t n, stream_t s) {
   return cudaMemcpyAsync(h, d, n, cudaMemcpyDeviceToHost, s) == cudaSuccess ? 0 : -1;
 }
-static int dev_memset(void* d, int v, size_t n) { return cudaMemset(d, v, n) == cudaSuccess ? 0 : -1; }
+// cudaMemset runs on the legacy default stream, which the handle's non-blocking streams do not wait for: finish it
+// before anything else can touch the memory (set-up only)
+static int dev_memset(void* d, int v, size_t n) {
+  return cudaMemset(d, v, n) == cudaSuccess && cudaStreamSynchronize(cudaStreamLegacy) == cudaSuccess ? 0 : -1;
+}
 static int sync_stream(stream_t s) { return cudaStreamSynchronize(s) == cudaSuccess ? 0 : -1; }
 static bool is_device_ptr(const void* p) {
   if (!p) return false;
@@ -113,6 +117,11 @@ struct mwb_handle {
   bool smem_tris;
   int stage_bytes;
   bool have_params, have_protos, have_template;
+  // level table (host copies of S.levels / S.env_level / S.ops); a handle that never calls mwb_set_levels has one level
+  std::vector<LevelDev> levels;
+  std::vector<int32_t> env_level;
+  std::vector<mwb_op> ops_h;
+  int geom_blocks;                // blocks the geometry arrays hold: N (per-env worlds) or at least levels.size()
   bool profiling;
   bool frames_copied;
   int obs_peer_hint;              // mwb_set_obs_peer: 1 / 0 = the caller says where observations go, -1 = look it up
@@ -234,22 +243,23 @@ MWB_DEV void step_one(const DevState& S, int i, const int32_t* actions, const do
       MWB_WARP_SYNC();
     }
     double fs, fd, ts;
+    const mwb_params& P = env_level_of(S, i).params;
     if (step_params) {
       fs = step_params[i * 3 + 0];
       fd = step_params[i * 3 + 1];
       ts = step_params[i * 3 + 2];
     } else if (S.domain_rand) {   // params.sample(rand, ...) x3, always, before the action is read
       NpRng r = load_rng(S, i);
-      fs = rng_uniform(r, S.params.forward_step_lo, S.params.forward_step_rng);
-      fd = rng_uniform(r, S.params.forward_drift_lo, S.params.forward_drift_rng);
-      ts = rng_uniform(r, S.params.turn_step_lo, S.params.turn_step_rng);
+      fs = rng_uniform(r, P.forward_step_lo, P.forward_step_rng);
+      fd = rng_uniform(r, P.forward_drift_lo, P.forward_drift_rng);
+      ts = rng_uniform(r, P.turn_step_lo, P.turn_step_rng);
       MWB_WARP_SYNC();
       store_rng(S, i, r);
       MWB_WARP_SYNC();
     } else {
-      fs = S.params.forward_step;
-      fd = S.params.forward_drift;
-      ts = S.params.turn_step;
+      fs = P.forward_step;
+      fd = P.forward_drift;
+      ts = P.turn_step;
     }
     o = physics_step(S, i, action, fs, fd, ts);
     if (o.terminated || o.truncated) {
@@ -295,8 +305,9 @@ MWB_DEV void scatter_one(const DevState& S, const WorldUpload& u) {
     for (int r = 0; r < S.num_rooms[i]; ++r)
       for (int k = 0; k < 3; ++k) S.room_tex[((size_t)i * S.R + r) * 3 + k] = rooms[r].tex_id[k];
   } else {
-    for (int r = 0; r < S.num_rooms[0]; ++r)
-      for (int k = 0; k < 3; ++k) S.room_tex[((size_t)i * S.R + r) * 3 + k] = S.rooms[r].tex_id[k];
+    const int g = geom_index(S, i);
+    for (int r = 0; r < S.num_rooms[g]; ++r)
+      for (int k = 0; k < 3; ++k) S.room_tex[((size_t)i * S.R + r) * 3 + k] = S.rooms[(size_t)g * S.R + r].tex_id[k];
   }
 }
 
@@ -332,7 +343,10 @@ MWB_DEV void gather_one(const DevState& S, int i, WorldUpload& u) {
 }
 
 #ifndef MWB_HOSTSIM
-__global__ void step_kernel(DevState S, const int32_t* actions, const double* step_params, double* reward,
+// 6 blocks of 128 threads per SM: K1 keeps the 80-register budget it had while the level data came from kernel
+// parameters (the per-env level table is read through global loads, which the compiler would otherwise hoist into
+// 128 registers)
+__global__ void __launch_bounds__(128, 6) step_kernel(DevState S, const int32_t* actions, const double* step_params, double* reward,
                             uint8_t* term, uint8_t* trunc) {
   int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;   // one warp per env (physics.cuh: circle_hits_walls)
   if (i < S.N) step_one(S, i, actions, step_params, reward, term, trunc);
@@ -627,12 +641,19 @@ extern "C" int mwb_create(const mwb_config* cfg, mwb_handle** out) {
   S.obs_w = cfg->obs_width;
   S.obs_h = cfg->obs_height;
   S.msaa = cfg->msaa_samples;
-  S.rule_kind = cfg->rule_kind;
-  S.rule_arg = cfg->rule_arg;
   S.domain_rand = cfg->domain_rand;
-  S.max_episode_steps = cfg->max_episode_steps;
   S.autoreset = cfg->autoreset;
+  {
+    LevelDev L0;
+    memset(&L0, 0, sizeof(L0));
+    L0.rule_kind = cfg->rule_kind;
+    L0.rule_arg = cfg->rule_arg;
+    L0.max_episode_steps = cfg->max_episode_steps;
+    h->levels.assign(1, L0);
+    h->env_level.assign(N, 0);
+  }
   const size_t G = cfg->shared_geometry ? 1 : N;
+  h->geom_blocks = (int)G;
   int rc = 0;
 #define AL(field, count) if (!rc) rc = alloc_arr(h, &S.field, (count))
   AL(ent_proto, E * N); AL(ent_px, E * N); AL(ent_py, E * N); AL(ent_pz, E * N); AL(ent_dir, E * N);
@@ -644,6 +665,12 @@ extern "C" int mwb_create(const mwb_config* cfg, mwb_handle** out) {
   AL(rooms, G * S.R); AL(quads, G * S.Q + 2); AL(segs, G * S.S); AL(room_tex, N * S.R * 3);
   AL(mesh_seg, N * E); AL(cam_trig, 6 * N); AL(ent_cs, E * 2 * N);
 #undef AL
+  LevelDev* d_levels = nullptr;
+  int32_t* d_env_level = nullptr;
+  if (!rc) rc = alloc_arr(h, &d_levels, MWB_LEVEL_CAP);
+  if (!rc) rc = alloc_arr(h, &d_env_level, N);      // zeros: every env runs level 0
+  S.levels = d_levels;
+  S.env_level = d_env_level;
   if (!rc) rc = alloc_arr(h, &h->d_actions, N);
   if (!rc) rc = alloc_arr(h, &h->d_step_params, 3 * N);
   if (!rc) rc = alloc_arr(h, &h->d_reward, N);
@@ -781,7 +808,8 @@ extern "C" int mwb_abi_sizes(int32_t* out, int cap) {
                         (int32_t)sizeof(mwb_mesh_desc), (int32_t)sizeof(mwb_room), (int32_t)sizeof(mwb_quad),
                         (int32_t)sizeof(mwb_seg), (int32_t)sizeof(mwb_proto), (int32_t)sizeof(mwb_entity),
                         (int32_t)sizeof(mwb_op), (int32_t)sizeof(mwb_geometry), (int32_t)sizeof(mwb_world),
-                        (int32_t)sizeof(mwb_rng_state), (int32_t)sizeof(mwb_state_view), (int32_t)sizeof(mwb_maze_desc)};
+                        (int32_t)sizeof(mwb_rng_state), (int32_t)sizeof(mwb_state_view), (int32_t)sizeof(mwb_maze_desc),
+                        (int32_t)sizeof(mwb_level)};
   const int n = (int)(sizeof(sz) / sizeof(sz[0]));
   for (int k = 0; k < n && k < cap; ++k) out[k] = sz[k];
   return n;
@@ -991,10 +1019,42 @@ extern "C" int mwb_upload_meshes(mwb_handle* h, const mwb_mesh_desc* descs, int 
 }
 
 // ------------------------------------------------------------------ ABI: level definition
+// Work enqueued on a caller stream may still read the buffers a set-up call is about to replace.
+static int drain(mwb_handle* h) {
+#ifndef MWB_HOSTSIM
+  if (h->last_valid && cudaStreamSynchronize(h->last_stream) != cudaSuccess) return fail(MWB_ECUDA, "sync failed");
+#endif
+  return sync_stream(h->stream) == 0 ? MWB_OK : fail(MWB_ECUDA, "sync failed");
+}
+
+// the host copies of the level table and of env_level -> S.levels / S.env_level
+static int upload_levels(mwb_handle* h) {
+  int rc = drain(h);
+  if (rc) return rc;
+  rc |= h2d((void*)h->S.levels, h->levels.data(), h->levels.size() * sizeof(LevelDev), h->stream);
+  rc |= h2d((void*)h->S.env_level, h->env_level.data(), h->env_level.size() * sizeof(int32_t), h->stream);
+  rc |= sync_stream(h->stream);
+  return rc ? fail(MWB_ECUDA, "level table upload failed") : MWB_OK;
+}
+
+static int upload_ops(mwb_handle* h) {
+  int rc = drain(h);
+  if (!rc) rc = replace_buf(&h->ops, h->ops_h.data(), h->ops_h.size() * sizeof(mwb_op), h->stream);
+  if (rc) return rc;
+  h->S.ops = (const mwb_op*)h->ops;
+  return MWB_OK;
+}
+
+static void set_level_params(LevelDev& L, const mwb_params& p) {
+  L.params = p;
+  L.near_extra = 1.1 * p.max_forward_step;
+}
+
 extern "C" int mwb_set_params(mwb_handle* h, const mwb_params* p) {
   if (!h || !p) return fail(MWB_EINVAL, "null argument");
-  h->S.params = *p;
-  h->S.near_extra = 1.1 * p->max_forward_step;
+  set_level_params(h->levels[0], *p);
+  int rc = upload_levels(h);
+  if (rc) return rc;
   h->have_params = true;
   return MWB_OK;
 }
@@ -1062,12 +1122,93 @@ extern "C" int mwb_set_template(mwb_handle* h, const mwb_geometry* g) {
   return rc;
 }
 
+// Level 0's program.  On a one-level handle it is the whole op array; with several levels it is appended, so that
+// the other levels' slices stay valid.
 extern "C" int mwb_set_program(mwb_handle* h, const mwb_op* ops, int n) {
   if (!h || !ops || n <= 0 || n > MWB_MAX_OPS) return fail(MWB_EINVAL, "bad program");
-  int rc = replace_buf(&h->ops, ops, (size_t)n * sizeof(mwb_op), h->stream);
+  if (h->levels.size() == 1) h->ops_h.clear();
+  h->levels[0].op_first = (int32_t)h->ops_h.size();
+  h->levels[0].num_ops = n;
+  h->ops_h.insert(h->ops_h.end(), ops, ops + n);
+  int rc = upload_ops(h);
+  if (!rc) rc = upload_levels(h);
+  return rc;
+}
+
+// Geometry arrays with room for G blocks (set-up only: the old contents are dropped)
+static int grow_geometry(mwb_handle* h, int G) {
+  DevState& S = h->S;
+  int rc = drain(h);
   if (rc) return rc;
-  h->S.ops = (const mwb_op*)h->ops;
-  h->S.num_ops = n;
+  void* old[] = {S.num_rooms, S.num_quads, S.num_segs, S.rooms, S.quads, S.segs};
+  int32_t *nr = nullptr, *nq = nullptr, *ns = nullptr;
+  mwb_room* rooms = nullptr;
+  mwb_quad* quads = nullptr;
+  mwb_seg* segs = nullptr;
+  if (alloc_arr(h, &nr, G) || alloc_arr(h, &nq, G) || alloc_arr(h, &ns, G) || alloc_arr(h, &rooms, (size_t)G * S.R) ||
+      alloc_arr(h, &quads, (size_t)G * S.Q + 2) || alloc_arr(h, &segs, (size_t)G * S.S))
+    return fail(MWB_ECUDA, "geometry allocation failed");
+  for (void* p : old) {
+    auto it = std::find(h->allocs.begin(), h->allocs.end(), p);
+    if (it != h->allocs.end()) {
+      dev_free(p);
+      h->allocs.erase(it);
+    }
+  }
+  S.num_rooms = nr;
+  S.num_quads = nq;
+  S.num_segs = ns;
+  S.rooms = rooms;
+  S.quads = quads;
+  S.segs = segs;
+  h->geom_blocks = G;
+  return MWB_OK;
+}
+
+extern "C" int mwb_set_levels(mwb_handle* h, int n_levels, const mwb_level* levels, const mwb_geometry* templates,
+                              const mwb_op* ops, int n_ops, const int32_t* env_level) {
+  if (!h || !levels || !templates || !ops || !env_level) return fail(MWB_EINVAL, "null argument");
+  if (!h->S.shared_geom) return fail(MWB_EINVAL, "a level table needs shared_geometry = 1 (per-env worlds have no templates)");
+  if (n_levels <= 0) return fail(MWB_EINVAL, "n_levels must be positive");
+  if (n_levels > MWB_LEVEL_CAP) return fail(MWB_ECAPACITY, "more than MWB_LEVEL_CAP levels");
+  if (n_ops <= 0) return fail(MWB_EINVAL, "empty op array");
+  const DevState& S = h->S;
+  for (int l = 0; l < n_levels; ++l) {
+    const mwb_level& L = levels[l];
+    if (L.num_ops > MWB_MAX_OPS) return fail(MWB_ECAPACITY, "level " + std::to_string(l) + ": program longer than MWB_MAX_OPS");
+    if (L.num_ops <= 0 || L.op_first < 0 || L.op_first + L.num_ops > n_ops)
+      return fail(MWB_EINVAL, "level " + std::to_string(l) + ": program slice outside the op array");
+    const mwb_geometry& g = templates[l];
+    if (g.num_rooms < 0 || g.num_quads < 0 || g.num_segs < 0 || g.num_rooms > S.R || g.num_quads > h->cfg.max_quads ||
+        g.num_segs > S.S)
+      return fail(MWB_ECAPACITY, "level " + std::to_string(l) + ": template exceeds max_rooms / max_quads / max_segs");
+    for (int r = 0; r < g.num_rooms; ++r)
+      if (g.rooms[r].num_edges > MWB_MAX_EDGES) return fail(MWB_ECAPACITY, "room outline too long");
+  }
+  for (int i = 0; i < S.N; ++i)
+    if (env_level[i] < 0 || env_level[i] >= n_levels)
+      return fail(MWB_EINVAL, "env_level[" + std::to_string(i) + "] = " + std::to_string(env_level[i]) + " is not a level");
+  int rc = 0;
+  if (n_levels > h->geom_blocks) rc = grow_geometry(h, n_levels);
+  for (int l = 0; l < n_levels && !rc; ++l) rc = upload_geometry(h, (size_t)l, &templates[l]);
+  if (rc) return rc;
+  h->levels.resize(n_levels);
+  for (int l = 0; l < n_levels; ++l) {
+    LevelDev& D = h->levels[l];
+    memset(&D, 0, sizeof(D));
+    set_level_params(D, levels[l].params);
+    D.rule_kind = levels[l].rule_kind;
+    D.rule_arg = levels[l].rule_arg;
+    D.max_episode_steps = levels[l].max_episode_steps;
+    D.op_first = levels[l].op_first;
+    D.num_ops = levels[l].num_ops;
+  }
+  h->env_level.assign(env_level, env_level + S.N);
+  h->ops_h.assign(ops, ops + n_ops);
+  rc = upload_ops(h);
+  if (!rc) rc = upload_levels(h);
+  if (rc) return rc;
+  h->have_params = h->have_template = true;
   return MWB_OK;
 }
 
@@ -1101,7 +1242,7 @@ extern "C" int mwb_set_maze(mwb_handle* h, const mwb_maze_desc* mz) {
 extern "C" int mwb_get_geometry(mwb_handle* h, int env, int32_t counts[3], mwb_room* rooms, mwb_quad* quads, mwb_seg* segs) {
   if (!h || !counts) return fail(MWB_EINVAL, "null argument");
   if (env < 0 || env >= h->S.N) return fail(MWB_EINVAL, "env out of range");
-  const size_t g = h->S.shared_geom ? 0 : (size_t)env;
+  const size_t g = h->S.shared_geom ? (size_t)h->env_level[env] : (size_t)env;
   int rc = 0;
   rc |= stream_enter(h, h->stream);
   rc |= d2h(&counts[0], h->S.num_rooms + g, sizeof(int32_t), h->stream);
@@ -1665,9 +1806,15 @@ struct SnapHeader {
   uint64_t bytes;
 };
 
+// geometry blocks a snapshot carries: one template per level, or one world per env
+static size_t snapshot_blocks(const mwb_handle* h) { return h->S.shared_geom ? h->levels.size() : (size_t)h->S.N; }
+
+// a handle with several levels appends its env_level [N] to the blob (checked on restore, never overwritten)
+static size_t snapshot_level_bytes(const mwb_handle* h) { return h->levels.size() > 1 ? h->env_level.size() * sizeof(int32_t) : 0; }
+
 static void snapshot_arrays(mwb_handle* h, std::vector<std::pair<void*, size_t>>& v) {
   const DevState& S = h->S;
-  const size_t N = S.N, E = S.E, G = S.shared_geom ? 1 : N;
+  const size_t N = S.N, E = S.E, G = snapshot_blocks(h);
 #define SA(field, count) v.push_back(std::make_pair((void*)S.field, (size_t)(count) * sizeof(*S.field)))
   SA(ent_proto, E * N); SA(ent_px, E * N); SA(ent_py, E * N); SA(ent_pz, E * N); SA(ent_dir, E * N);
   SA(ent_col, E * 3 * N); SA(ent_size, E * N); SA(num_slots, N); SA(agent_slot, N); SA(carrying, N); SA(step_count, N);
@@ -1686,8 +1833,8 @@ static SnapHeader snapshot_header(mwb_handle* h) {
   hd.magic = 0x5342574du;   // "MWBS"
   hd.abi = MWB_ABI_VERSION;
   hd.N = h->S.N; hd.E = h->S.E; hd.R = h->S.R; hd.Q = h->S.Q; hd.S = h->S.S;
-  hd.G = h->S.shared_geom ? 1 : h->S.N;
-  hd.bytes = sizeof(SnapHeader);
+  hd.G = (int32_t)snapshot_blocks(h);
+  hd.bytes = sizeof(SnapHeader) + snapshot_level_bytes(h);
   for (size_t k = 0; k < v.size(); ++k) hd.bytes += v[k].second;
   return hd;
 }
@@ -1713,6 +1860,7 @@ extern "C" int mwb_snapshot(mwb_handle* h, void* blob, size_t bytes) {
     p += v[k].second;
   }
   if (sync_stream(h->stream) != 0) return fail(MWB_ECUDA, "sync failed");
+  if (snapshot_level_bytes(h)) memcpy(p, h->env_level.data(), snapshot_level_bytes(h));
   return MWB_OK;
 }
 
@@ -1723,11 +1871,17 @@ extern "C" int mwb_restore(mwb_handle* h, const void* blob, size_t bytes) {
   if (bytes < sizeof(hd)) return fail(MWB_EINVAL, "not a snapshot");
   memcpy(&hd, blob, sizeof(hd));
   if (hd.magic != want.magic || hd.abi != want.abi) return fail(MWB_EABI, "snapshot from another ABI version");
-  if (hd.N != want.N || hd.E != want.E || hd.R != want.R || hd.Q != want.Q || hd.S != want.S || hd.G != want.G ||
-      hd.bytes != want.bytes || bytes < hd.bytes)
+  if (hd.N != want.N || hd.E != want.E || hd.R != want.R || hd.Q != want.Q || hd.S != want.S)
     return fail(MWB_EINVAL, "snapshot does not match this handle's configuration");
+  if (hd.G != want.G || hd.bytes != want.bytes)
+    return fail(h->S.shared_geom ? MWB_ESTATE : MWB_EINVAL, h->S.shared_geom ? "snapshot of a handle with another number of levels"
+                                                                            : "snapshot does not match this handle's configuration");
+  if (bytes < hd.bytes) return fail(MWB_EINVAL, "snapshot truncated");
   std::vector<std::pair<void*, size_t>> v;
   snapshot_arrays(h, v);
+  const size_t lb = snapshot_level_bytes(h);
+  if (lb && memcmp((const unsigned char*)blob + hd.bytes - lb, h->env_level.data(), lb) != 0)
+    return fail(MWB_ESTATE, "snapshot assigns envs to other levels than this handle");
   const unsigned char* p = (const unsigned char*)blob + sizeof(hd);
   if (stream_enter(h, h->stream)) return MWB_ECUDA;
   for (size_t k = 0; k < v.size(); ++k) {

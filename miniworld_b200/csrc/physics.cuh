@@ -108,11 +108,12 @@ struct CarryPos {
 // _get_carry_pos(agent_pos, ent): agent_pos + dir_vec * 1.05 * dist, lifted to stay visible
 MWB_DEV CarryPos carry_pos(const DevState& S, int i, double apx, double apz, double c, double s, int slot, double ar) {
   const EntDims pr = ent_dims(S, i, slot, S.protos[S.ent_proto[(size_t)slot * S.N + i]]);
+  const double mfs = env_level_of(S, i).params.max_forward_step;
   double dist;   // agent.radius + ent.radius + max_forward_step, float32 as soon as ent.radius is
   if (pr.f32)
-    dist = (double)f_add(f_add((float)ar, (float)pr.radius), (float)S.params.max_forward_step);
+    dist = (double)f_add(f_add((float)ar, (float)pr.radius), (float)mfs);
   else
-    dist = d_add(d_add(ar, pr.radius), S.params.max_forward_step);
+    dist = d_add(d_add(ar, pr.radius), mfs);
   CarryPos o;
   o.x = d_add(apx, d_mul(d_mul(c, 1.05), dist));
   o.z = d_add(apz, d_mul(d_mul(-s, 1.05), dist));
@@ -180,7 +181,7 @@ MWB_DEV bool near_agent(const DevState& S, int i, int b, int as, double ar) {
   const double dz = d_sub(S.ent_pz[b * N + i], S.ent_pz[as * N + i]);
   const double d = d_sqrt(d_fma(dz, dz, d_fma(dy, dy, d_mul(dx, dx))));
   const EntDims pr = ent_dims(S, i, b, S.protos[bp]);
-  return d < near_threshold(pr.radius, pr.f32, ar, false, S.near_extra);
+  return d < near_threshold(pr.radius, pr.f32, ar, false, env_level_of(S, i).near_extra);
 }
 
 // MiniWorldEnv.near(ent0, ent1) between two entities of the list
@@ -193,7 +194,7 @@ MWB_DEV bool near_pair(const DevState& S, int i, int a, int b) {
   const double dz = d_sub(S.ent_pz[a * N + i], S.ent_pz[b * N + i]);
   const double d = d_sqrt(d_fma(dz, dz, d_fma(dy, dy, d_mul(dx, dx))));
   const EntDims da = ent_dims(S, i, a, S.protos[pa]), db = ent_dims(S, i, b, S.protos[pb]);
-  return d < near_threshold(da.radius, da.f32, db.radius, db.f32, S.near_extra);
+  return d < near_threshold(da.radius, da.f32, db.radius, db.f32, env_level_of(S, i).near_extra);
 }
 
 struct StepOut {
@@ -282,41 +283,44 @@ MWB_DEV StepOut physics_step(const DevState& S, int i, int action, double fwd_st
     S.ent_dir[carrying * N + i] = dir;
   }
 
+  // the env's level: its rule, rule argument and truncation length
+  const LevelDev& L = env_level_of(S, i);
+  const int rule_kind = L.rule_kind, rule_arg = L.rule_arg, max_steps = L.max_episode_steps;
   StepOut o;
   o.reward = 0.0;
   o.terminated = 0;
-  o.truncated = sc >= S.max_episode_steps ? 1 : 0;
+  o.truncated = sc >= max_steps ? 1 : 0;
 
-  if (S.rule_kind == MWB_RULE_SIDEWALK) {
+  if (rule_kind == MWB_RULE_SIDEWALK) {
     // sidewalk.py:96-99: stepping into the street ends the episode with reward 0, before the goal test
-    const mwb_room& street = S.rooms[(size_t)geom_index(S, i) * S.R + (S.rule_arg >> 8)];
+    const mwb_room& street = S.rooms[(size_t)geom_index(S, i) * S.R + (rule_arg >> 8)];
     if (room_contains(street, px, pz)) {
       o.reward = 0.0;
       o.terminated = 1;
     }
   }
-  if (S.rule_kind == MWB_RULE_GOAL || S.rule_kind == MWB_RULE_SIDEWALK) {
-    if (near_agent(S, i, S.rule_arg & 0xFF, as, ar)) {
-      o.reward = d_add(o.reward, d_sub(1.0, d_mul(0.2, d_div((double)sc, (double)S.max_episode_steps))));
+  if (rule_kind == MWB_RULE_GOAL || rule_kind == MWB_RULE_SIDEWALK) {
+    if (near_agent(S, i, rule_arg & 0xFF, as, ar)) {
+      o.reward = d_add(o.reward, d_sub(1.0, d_mul(0.2, d_div((double)sc, (double)max_steps))));
       o.terminated = 1;
     }
-  } else if (S.rule_kind == MWB_RULE_SIGN) {
+  } else if (rule_kind == MWB_RULE_SIGN) {
     // sign.py:158-173: the extra action ends the episode; touching any of the six objects ends it with
     // reward +1 for the object the sign names (colour index, kind = goal) and -1 otherwise (the last hit wins)
     if (action == 3) o.terminated = 1;
-    const int colour = S.rule_arg & 0xFF, goal = (S.rule_arg >> 8) & 0xFF;
+    const int colour = rule_arg & 0xFF, goal = (rule_arg >> 8) & 0xFF;
     for (int b = 0; b < 6; ++b)
       if (near_agent(S, i, b, as, ar)) {
         o.terminated = 1;
         o.reward = (b % 3 == colour && b / 3 == goal) ? 1.0 : -1.0;
       }
-  } else if (S.rule_kind == MWB_RULE_PUTNEXT) {
+  } else if (rule_kind == MWB_RULE_PUTNEXT) {
     // putnext.py:61-66: done once the two boxes are next to each other and the agent has let go
-    if (carrying < 0 && near_pair(S, i, S.rule_arg & 0xFF, (S.rule_arg >> 8) & 0xFF)) {
-      o.reward = d_add(o.reward, d_sub(1.0, d_mul(0.2, d_div((double)sc, (double)S.max_episode_steps))));
+    if (carrying < 0 && near_pair(S, i, rule_arg & 0xFF, (rule_arg >> 8) & 0xFF)) {
+      o.reward = d_add(o.reward, d_sub(1.0, d_mul(0.2, d_div((double)sc, (double)max_steps))));
       o.terminated = 1;
     }
-  } else if (S.rule_kind == MWB_RULE_HEALTH) {
+  } else if (rule_kind == MWB_RULE_HEALTH) {
     // collecthealth.py:62-86.  The level counter (num_picked) holds the agent's health.
     int health = S.num_picked[i] - 2;
     if (action == 4 && carrying >= 0) {
@@ -367,7 +371,7 @@ MWB_DEV StepOut physics_step(const DevState& S, int i, int action, double fwd_st
       o.reward = -100.0;
       o.terminated = 1;
     }
-  } else if (S.rule_kind == MWB_RULE_PICKUP) {
+  } else if (rule_kind == MWB_RULE_PICKUP) {
     if (carrying >= 0) {
       // the observation of this step still shows the object at its carry position
       S.ghost_slot[i] = carrying;
@@ -382,7 +386,7 @@ MWB_DEV StepOut physics_step(const DevState& S, int i, int action, double fwd_st
       int np_ = S.num_picked[i] + 1;
       S.num_picked[i] = np_;
       o.reward = 1.0;
-      if (np_ == S.rule_arg) o.terminated = 1;
+      if (np_ == rule_arg) o.terminated = 1;
     }
   }
   S.carrying[i] = carrying;

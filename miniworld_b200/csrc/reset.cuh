@@ -7,7 +7,7 @@
 // GPU lands on the same poses, colours and camera parameters as `env.reset()` in Python.
 // The level's `_gen_world()` is lowered on the host into a short program of
 // CHOICE / UNIFORM / PLACE / PUT / IFEQ ops (miniworld_b200/program.py); room layout comes from the
-// shared static template.  Levels whose topology is random per episode (Maze) reset on the
+// static template of the env's level, and the program is that level's slice of the op array.  Levels whose topology is random per episode (Maze) reset on the
 // host and arrive through mwb_set_world instead.
 #pragma once
 #include "maze.cuh"
@@ -27,14 +27,17 @@ MWB_DEV void draw_room_textures(const DevState& S, int i, const mwb_room* rooms,
 MWB_DEV void device_reset(const DevState& S, int i) {
   const size_t N = S.N;
   NpRng rng = load_rng(S, i);
-  const mwb_params& P = S.params;
+  const LevelDev& L = env_level_of(S, i);
+  const mwb_params& P = L.params;
+  const mwb_op* ops = S.ops + L.op_first;
+  const int num_ops = L.num_ops;
   const int g = geom_index(S, i);
   const mwb_room* rooms = S.rooms + (size_t)g * S.R;
   int n_rooms = S.num_rooms[g];
 
   S.step_count[i] = 0;
   S.carrying[i] = -1;
-  S.num_picked[i] = S.rule_kind == MWB_RULE_HEALTH ? 100 : 0;   // CollectHealth: self.health = 100
+  S.num_picked[i] = L.rule_kind == MWB_RULE_HEALTH ? 100 : 0;   // CollectHealth: self.health = 100
   S.ghost_slot[i] = -1;
   S.num_slots[i] = 0;
   for (int e = 0; e < S.E; ++e) {
@@ -52,8 +55,8 @@ MWB_DEV void device_reset(const DevState& S, int i) {
   bool static_done = false;
   int slots = 0;
 
-  for (int pc = 0; pc < S.num_ops; ++pc) {
-    const mwb_op& op = S.ops[pc];
+  for (int pc = 0; pc < num_ops; ++pc) {
+    const mwb_op& op = ops[pc];
     if (op.op == MWB_OP_END) break;
     if (op.op == MWB_OP_MAZE) {          // per-episode topology: regenerate this env's rooms
       if (S.maze != nullptr && !S.shared_geom && maze_generate(S, *S.maze, S.maze_cdf, i, rng)) {

@@ -2,8 +2,8 @@
 //
 // Layout rule: every per-env scalar is an array [N] (env index fastest) so that the
 // one-thread-per-env physics kernel reads and writes fully coalesced; per-entity fields are
-// [max_ents][N].  Static room geometry is either one shared template (all envs of a level
-// without per-episode topology) or [N][capacity] blocks (Maze).  Nothing here is ever
+// [max_ents][N].  Static room geometry is either one shared template per level (levels
+// without per-episode topology; env_level picks the block) or [N][capacity] blocks (Maze).  Nothing here is ever
 // re-laid-out between kernels: the physics kernel and the rasteriser read the same arrays.
 #pragma once
 #include "../../include/mwb.h"
@@ -15,6 +15,16 @@
 struct TriRec;
 struct MeshSegInfo;
 struct MazeDev;
+
+// One row of the level table (mwb_set_levels): what K1 reads per env instead of per handle.
+struct LevelDev {
+  mwb_params params;
+  double near_extra;            // 1.1 * max_forward_step
+  int32_t rule_kind, rule_arg;
+  int32_t max_episode_steps;
+  int32_t op_first, num_ops;    // slice of DevState::ops
+  int32_t reserved;
+};
 
 struct DevState {
   int32_t N, E, R, Q, S;        // envs, entity slots, room / quad / segment capacity
@@ -53,8 +63,8 @@ struct DevState {
   int32_t* rng_has32;
   uint32_t* rng_cache;
 
-  // ---- geometry: [1 or N][capacity] ----
-  int32_t* num_rooms;           // [1 or N]
+  // ---- geometry: [levels][capacity] (shared templates) or [N][capacity] (per-env worlds) ----
+  int32_t* num_rooms;           // [levels or N]
   int32_t* num_quads;
   int32_t* num_segs;
   mwb_room* rooms;
@@ -80,26 +90,25 @@ struct DevState {
   TriRec* room_tris;            // [N][tri_cap] room + box triangle lists in HBM for levels whose lists do
                                 //   not fit shared memory (Maze); null = lists live in shared memory
 
-  // ---- level definition (shared) ----
+  // ---- level definition ----
   const MazeDev* maze;          // Maze templates (mwb_set_maze) or null
   const double* maze_cdf;
-  const mwb_proto* protos;
+  const mwb_proto* protos;      // shared by all levels
   int32_t num_protos;
-  const mwb_op* ops;
-  int32_t num_ops;
-  mwb_params params;
-  int32_t rule_kind, rule_arg;
+  const mwb_op* ops;            // every level's reset program, one after another
+  const LevelDev* levels;       // [levels] rule, truncation, params, program slice
+  const int32_t* env_level;     // [N] level of each env (all 0 on a one-level handle)
   int32_t domain_rand;
-  int32_t max_episode_steps;
   int32_t autoreset;
-  double near_extra;            // 1.1 * max_forward_step
   // StochasticActionWrapper on the device (reference wrappers.py:49-71): per step one uniform() draw from
   // the env's own stream; below act_prob the chosen action stands, else act_random (< 0: integers(0, 6))
   int32_t act_noise, act_random;
   double act_prob;
 };
 
-MWB_DEV int geom_index(const DevState& S, int i) { return S.shared_geom ? 0 : i; }
+// Block of the geometry arrays env i reads: its level's template, or its own world
+MWB_DEV int geom_index(const DevState& S, int i) { return S.shared_geom ? S.env_level[i] : i; }
+MWB_DEV const LevelDev& env_level_of(const DevState& S, int i) { return S.levels[S.env_level[i]]; }
 
 MWB_DEV NpRng load_rng(const DevState& S, int i) {
   NpRng r;

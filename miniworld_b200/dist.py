@@ -21,14 +21,25 @@ def shard_range(total, world_size, rank):
 class ShardedMiniWorld:
     """This rank's slice of a `total_envs`-wide BatchedMiniWorld plus the per-step exchange."""
 
-    def __init__(self, level, total_envs, dist=None, device=0, **kwargs):
-        from .batched import BatchedMiniWorld
+    def __init__(self, level, total_envs, dist=None, device=0, env_level=None, **kwargs):
+        """`level` may be a sequence of levels as for BatchedMiniWorld; `env_level` is then the assignment of all
+        `total_envs` envs (default: contiguous near-equal blocks), and this rank runs its slice of it."""
+        from .batched import BatchedMiniWorld, default_env_level
         self.dist = dist
         self.rank = dist.get_rank() if dist is not None else 0
         self.world = dist.get_world_size() if dist is not None else 1
         self.total = int(total_envs)
         self.start, self.count = shard_range(self.total, self.world, self.rank)
         self.counts = [shard_range(self.total, self.world, r)[1] for r in range(self.world)]
+        if isinstance(level, (list, tuple)):
+            if env_level is None:
+                env_level = default_env_level(self.total, len(level))
+            env_level = np.asarray(env_level)
+            if env_level.shape != (self.total,):
+                raise ValueError("env_level must have one entry per env (%d), got shape %s" % (self.total, env_level.shape))
+            kwargs["env_level"] = env_level[self.start:self.start + self.count]
+        elif env_level is not None:
+            raise ValueError("env_level assigns envs to levels: pass `level` as a sequence of levels")
         self.local = BatchedMiniWorld(level, self.count, device=device, **kwargs)
 
     def reset(self, seed):

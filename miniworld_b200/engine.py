@@ -10,12 +10,14 @@ import os
 
 import numpy as np
 
-ABI_VERSION = 6
+ABI_VERSION = 7
 RULE_NONE, RULE_GOAL, RULE_PICKUP, RULE_SIDEWALK, RULE_SIGN, RULE_HEALTH, RULE_PUTNEXT = 0, 1, 2, 3, 4, 5, 6
 SURF_WALL, SURF_FLOOR, SURF_CEIL = 0, 1, 2
 OP_END, OP_CHOICE, OP_UNIFORM, OP_PLACE, OP_MAZE, OP_IFEQ, OP_PUT = 0, 1, 2, 3, 4, 5, 6
 MAX_EDGES = 8
 MAX_ENTS_CAP = 32
+LEVEL_CAP = 32
+MAX_OPS = 64
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 DEFAULT_LIB = os.path.join(_HERE, "libmwb.so")
@@ -105,12 +107,16 @@ class StateView(C.Structure):
         "cam", "env_params", "rng", "room_tex", "num_picked_up", "episodes_done")]
 
 
+class Level(C.Structure):
+    _fields_ = [("rule_kind", C.c_int32), ("rule_arg", C.c_int32), ("max_episode_steps", C.c_int32),
+                ("op_first", C.c_int32), ("num_ops", C.c_int32), ("reserved", C.c_int32), ("params", Params)]
+
 
 def _expected_sizes():
     return [C.sizeof(Config), C.sizeof(Params), C.sizeof(TexDesc), C.sizeof(MeshDesc),
             ROOM_DTYPE.itemsize, QUAD_DTYPE.itemsize, SEG_DTYPE.itemsize, PROTO_DTYPE.itemsize,
             ENTITY_DTYPE.itemsize, OP_DTYPE.itemsize, C.sizeof(Geometry), C.sizeof(World),
-            RNG_DTYPE.itemsize, C.sizeof(StateView), C.sizeof(MazeDesc)]
+            RNG_DTYPE.itemsize, C.sizeof(StateView), C.sizeof(MazeDesc), C.sizeof(Level)]
 
 
 EXPORTS = (
@@ -122,6 +128,7 @@ EXPORTS = (
     "mwb_render_top_view", "mwb_visible_ents", "mwb_set_action_noise",
     "mwb_snapshot_size", "mwb_snapshot", "mwb_restore", "mwb_set_obs_format",
     "mwb_flag_write", "mwb_flag_wait_geq", "mwb_flag_mode", "mwb_state_array", "mwb_debug_camera", "mwb_set_obs_peer",
+    "mwb_set_levels",
 )
 OBS_FORMATS = {"hwc": 0, "cwh": 1, "grey": 2}
 
@@ -158,6 +165,7 @@ def load_library():
     lib.mwb_set_protos.argtypes = [vp, vp, C.c_int]
     lib.mwb_set_template.argtypes = [vp, C.POINTER(Geometry)]
     lib.mwb_set_program.argtypes = [vp, vp, C.c_int]
+    lib.mwb_set_levels.argtypes = [vp, C.c_int, vp, vp, vp, C.c_int, vp]
     lib.mwb_seed.argtypes = [vp, vp, C.c_int, vp]
     lib.mwb_reset.argtypes = [vp, vp, C.c_int, vp]
     lib.mwb_set_world.argtypes = [vp, vp, C.c_int, vp]
@@ -415,6 +423,28 @@ class Engine:
     def set_program(self, ops):
         ops = np.ascontiguousarray(ops, OP_DTYPE)
         self._check(self.lib.mwb_set_program(self.h, _ptr(ops), len(ops)))
+
+    def set_levels(self, levels, env_level):
+        """Several levels in one handle (mwb_set_levels).  levels: list of dicts with "rule" (kind, arg),
+        "max_episode_steps", "params" (DomainParams), "geometry" (rooms, quads, segs) and "ops" (this level's
+        program, proto indices already absolute); env_level: int [num_envs] level of each env."""
+        n = len(levels)
+        table = (Level * n)()
+        geoms = (Geometry * n)()
+        first = 0
+        for k, lv in enumerate(levels):
+            rec = table[k]
+            rec.rule_kind, rec.rule_arg = int(lv["rule"][0]), int(lv["rule"][1])
+            rec.max_episode_steps = int(lv["max_episode_steps"])
+            rec.op_first, rec.num_ops = first, len(lv["ops"])
+            rec.params = lower_params(lv["params"])
+            geoms[k] = self._geometry(*lv["geometry"])
+            first += len(lv["ops"])
+        ops = np.ascontiguousarray(np.concatenate([lv["ops"] for lv in levels]), OP_DTYPE)
+        env_level = np.ascontiguousarray(env_level, np.int32)
+        self._keep = [lv["geometry"] for lv in levels]
+        self._check(self.lib.mwb_set_levels(self.h, n, C.cast(table, C.c_void_p), C.cast(geoms, C.c_void_p),
+                                            _ptr(ops), len(ops), _ptr(env_level)))
 
     # ---- reset
     def seed(self, env_ids, states):
