@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define MWB_ABI_VERSION 7
+#define MWB_ABI_VERSION 8
 
 /* error codes */
 #define MWB_OK 0
@@ -295,6 +295,34 @@ typedef struct mwb_level {
 int mwb_set_levels(mwb_handle* h, int n_levels, const mwb_level* levels, const mwb_geometry* templates /*[n_levels]*/,
                    const mwb_op* ops, int n_ops, const int32_t* env_level /*[num_envs]*/);
 
+/* Level changes at episode boundaries (curricula: promote an env once it succeeds, re-weight levels by success rate).
+ * Valid after mwb_set_levels (MWB_ESTATE before it, or when already on; the level table is fixed from then on).  It
+ * allocates next_level [N] (all -1), level_draws [N] (all 0) and level_weights [L] (all 0: no draws), and makes the
+ * device's env_level authoritative: the resets rewrite it, and the caller reads and writes these arrays in place
+ * through mwb_state_array (MWB_ARRAY_ENV_LEVEL / NEXT_LEVEL / LEVEL_WEIGHTS), stream-ordered, without a sync.
+ *
+ * A level changes only at a reset: mwb_reset, and the next-step auto-reset inside mwb_step.  An env never changes
+ * level mid-episode.  At every reset of env i, before the level is read:
+ *   1. if next_level[i] is in [0, L): the env takes that level, and next_level[i] is cleared to -1;
+ *   2. otherwise, if the level weights sum to more than 0: the next level is drawn from them;
+ *   3. otherwise the env keeps its level.
+ * A next_level entry outside [-1, L) counts as -1 and is cleared.
+ * The draw does not touch the env's numpy stream, so after a switch env i equals, bit for bit, a fresh env of the new
+ * level whose stream was set to the state env i carried into that reset.  It is defined exactly:
+ *   k      = (uint64)(env_offset + i) << 32 | level_draws[i]     (the env's global index; sharded = single process)
+ *   h      = splitmix64 output at position k for `seed`:
+ *            z = seed + (k + 1) * 0x9E3779B97F4A7C15;  z = (z ^ z >> 30) * 0xBF58476D1CE4E5B9;
+ *            z = (z ^ z >> 27) * 0x94D049BB133111EB;  h = z ^ z >> 31              (all mod 2^64)
+ *   w_l    = level_weights[l] if it is > 0, else 0 (NaN and negative weights count as 0)
+ *   total  = w_0 + w_1 + ... in level order, float32;  target = float32(h >> 40) * 2^-24 * total, float32
+ *   level  = the first l with w_l > 0 whose running float32 sum w_0 + ... + w_l exceeds target (the last such l
+ *            if none does, which only an infinite weight can cause); level_draws[i] += 1.
+ * Handles that never call this behave exactly as before it existed.  Snapshots of a handle with level changes on
+ * carry env_level, next_level, level_draws, level_weights, seed and env_offset; restoring one needs a handle with
+ * the same level count and level changes on, and adopts all of them.  Restoring a blob into a handle whose level
+ * changes are on / off while the blob's were off / on fails with MWB_ESTATE. */
+int mwb_enable_level_changes(mwb_handle* h, uint64_t seed, int32_t env_offset /* global index of env 0, >= 0 */);
+
 /* Maze level (reference envs/maze.py): every episode's world is a translate-and-select of these
  * templates -- one grid cell and one connector room per neighbour direction, in the order of
  * maze.py:110 `orders = [(0, 1), (0, -1), (-1, 0), (1, 0)]` as (dj, di).  All records are for
@@ -375,7 +403,9 @@ int mwb_get_state(mwb_handle* h, const mwb_state_view* out);
  * Restoring into a handle created with the same configuration and level definition resumes every env
  * bit for bit.  (The reference has no equivalent: its state lives in Python objects.)  The blob of a handle with
  * several levels also carries env_level; restoring it into a handle with another level count or assignment fails
- * with MWB_ESTATE. */
+ * with MWB_ESTATE (handles with level changes on: see mwb_enable_level_changes; their blobs are marked as such in the
+ * header, and a blob whose mark differs from the handle's mode is refused with MWB_ESTATE before anything else is
+ * compared). */
 int mwb_snapshot_size(mwb_handle* h, size_t* bytes);
 int mwb_snapshot(mwb_handle* h, void* blob, size_t bytes);
 int mwb_restore(mwb_handle* h, const void* blob, size_t bytes);
@@ -423,7 +453,14 @@ int mwb_debug_camera(mwb_handle* h, float* out /* host [num_envs][16] */);
 #define MWB_ARRAY_ENT_Y 3
 #define MWB_ARRAY_ENT_Z 4
 #define MWB_ARRAY_ENT_DIR 5
+/* with level changes on (mwb_enable_level_changes; MWB_ESTATE otherwise): */
+#define MWB_ARRAY_ENV_LEVEL 6       /* int32   [num_envs]  level of each env's current episode                   */
+#define MWB_ARRAY_NEXT_LEVEL 7      /* int32   [num_envs]  pending assignment for the next reset, -1 = none      */
+#define MWB_ARRAY_LEVEL_WEIGHTS 8   /* float32 [n_levels]  sampling weights of the next resets                   */
 int mwb_state_array(mwb_handle* h, int which, void** dev_ptr, int64_t* count);
+/* 1 when this library keeps the handle's state arrays (mwb_state_array) in host memory -- the CPU build of the kernels
+ * used by the test suite -- and 0 for libmwb.so, whose arrays are device memory. */
+int mwb_state_in_host_memory(void);
 
 /* ---- one-way completion flags for the multi-GPU observation path (SURVEY 8e) --------------
  * The reference has no counterpart (it has no multi-device path at all, README.md:34); these replace the per-step

@@ -12,7 +12,9 @@ Per-environment semantics are exactly those of the reference's `MiniWorldEnv.res
   * levels whose topology is random per episode (Maze) generate worlds with the level's
     Python `_gen_world()` on the host (same numpy stream) and upload them (`mwb_set_world`);
   * `autoreset=True` gives Gymnasium "next-step" auto-reset: the step after a
-    terminated|truncated step resets that env (action ignored, reward 0).
+    terminated|truncated step resets that env (action ignored, reward 0);
+  * with several levels and `dynamic_levels=True`, an env's level can change at its resets:
+    pending assignments (`set_env_level`) and device-side draws from `level_weights`.
 
 Outputs are torch CUDA tensors by default (zero-copy from the kernels); `step_host`
 performs the same step with pinned host buffers for callers that want numpy.
@@ -45,6 +47,42 @@ def _torch_stream(torch, device):
     return torch.cuda.current_stream(device).cuda_stream or 1
 
 
+_SPLITMIX_GAMMA = 0x9E3779B97F4A7C15
+_M64 = (1 << 64) - 1
+
+
+def _splitmix64_at(seed, k):
+    z = (int(seed) + (int(k) + 1) * _SPLITMIX_GAMMA) & _M64
+    z = ((z ^ (z >> 30)) * 0xBF58476D1CE4E5B9) & _M64
+    z = ((z ^ (z >> 27)) * 0x94D049BB133111EB) & _M64
+    return z ^ (z >> 31)
+
+
+def sample_level(seed, global_env, draw, weights):
+    """The level draw a reset makes (include/mwb.h, mwb_enable_level_changes), restated in numpy: the level env
+    `global_env` draws for the `draw`-th time (0-based) under float32 `weights` [n_levels] and handle seed `seed`.
+    Returns None when the weights do not sum to more than 0 (the env keeps its level, and no draw is counted)."""
+    w = np.asarray(weights, np.float32)
+    w = np.where(w > 0, w, np.float32(0))               # NaN and negative weights count as 0
+    total = np.float32(0)
+    for x in w:
+        total = np.float32(total + x)
+    if not total > 0:
+        return None
+    k = ((int(global_env) & 0xFFFFFFFF) << 32) | (int(draw) & 0xFFFFFFFF)
+    u24 = _splitmix64_at(int(seed) & _M64, k) >> 40
+    target = np.float32(np.float32(u24) * np.float32(2.0 ** -24)) * total
+    cdf, pick = np.float32(0), None
+    for l, x in enumerate(w):
+        if not x > 0:
+            continue
+        cdf = np.float32(cdf + x)
+        pick = l
+        if cdf > target:
+            break
+    return pick
+
+
 def default_env_level(num_envs, n_levels):
     """Level of each env when none is given: contiguous, near-equal blocks in the order the levels were listed (the
     first num_envs % n_levels levels get one env more)."""
@@ -56,21 +94,34 @@ class BatchedMiniWorld:
     """`level`: a level id or class, or a sequence of them to run several levels side by side in one batch (multi-task
     or curriculum training; env i runs level `env_level[i]`).  With a sequence, `level_kwargs` may be a sequence
     aligned with it, and the observation size, MSAA, domain randomisation, auto-reset and action noise are per batch.
-    Maze-family levels (per-env geometry) and Sign (dict observation) cannot share a batch with other levels."""
+    Maze-family levels (per-env geometry) and Sign (dict observation) cannot share a batch with other levels.
+
+    `dynamic_levels=True` (with a sequence of levels) lets envs move between levels at their resets, never
+    mid-episode: a pending assignment from `set_env_level` wins, otherwise the next level is drawn on the device from
+    `level_weights` (all zero, the default, keeps every env on its level).  The draws are keyed by `level_seed` and
+    the env's global index `env_offset + i` (ShardedMiniWorld sets the offset), not by the env's own numpy stream."""
 
     def __init__(self, level, num_envs, obs_width=80, obs_height=60, domain_rand=False, autoreset=True,
-                 msaa_samples=8, device=0, want_depth=False, level_kwargs=None, obs_format="hwc", env_level=None):
+                 msaa_samples=8, device=0, want_depth=False, level_kwargs=None, obs_format="hwc", env_level=None,
+                 dynamic_levels=False, level_seed=0, env_offset=0):
         self.num_envs = int(num_envs)
         self.obs_width, self.obs_height = int(obs_width), int(obs_height)
         self.domain_rand = bool(domain_rand)
         self.want_depth = bool(want_depth)
         self.device = int(device)
+        self.dynamic_levels = bool(dynamic_levels)
         if isinstance(level, (list, tuple)):
             self._init_levels(list(level), level_kwargs, env_level, msaa_samples, autoreset)
         else:
             if env_level is not None:
                 raise ValueError("env_level assigns envs to levels: pass `level` as a sequence of levels")
+            if self.dynamic_levels:
+                raise ValueError("dynamic_levels moves envs between levels: pass `level` as a sequence of levels")
             self._init_level(level, level_kwargs, msaa_samples, autoreset)
+        self._level_views = None
+        if self.dynamic_levels:
+            self.level_seed, self.env_offset = int(level_seed), int(env_offset)
+            self.engine.enable_level_changes(self.level_seed, self.env_offset)
         # observation layout written by the render kernel: the reference's PyTorchObsWrapper ("cwh") and
         # GreyscaleWrapper ("grey") are fused into its epilogue instead of running as separate passes
         self.obs_format = obs_format
@@ -154,7 +205,7 @@ class BatchedMiniWorld:
             self._host_done = np.zeros(self.num_envs, bool)
         self.level_ids = [level]
         self.proto_envs = [pe]
-        self.env_level = np.zeros(self.num_envs, np.int32)
+        self._env_level = np.zeros(self.num_envs, np.int32)
         self._device_info = dict(getattr(pe, "device_info", None) or {})
         self._device_obs_extra = dict(getattr(pe, "device_obs_extra", None) or {})
 
@@ -207,7 +258,7 @@ class BatchedMiniWorld:
             table.append(dict(rule=(_RULES[rule[0]], rule[1]), max_episode_steps=int(min(pe.max_episode_steps, 2 ** 31 - 1)),
                               params=pe.params, geometry=geom, ops=ops))
             pes.append(pe)
-        self.level_ids, self.proto_envs, self.env_level = names, pes, env_level.astype(np.int32)
+        self.level_ids, self.proto_envs, self._env_level = names, pes, env_level.astype(np.int32)
         self.level_cls, self.level_kwargs, self.proto_env = None, kwargs, None
         largest = max(pes, key=lambda pe: pe.action_space.n)
         self.action_space = self.single_action_space = largest.action_space
@@ -221,7 +272,7 @@ class BatchedMiniWorld:
                              max_episode_steps=table[0]["max_episode_steps"], autoreset=self.autoreset, device=self.device)
         self.engine.sync_assets()
         self.engine.set_protos(np.array(protos, PROTO_DTYPE))
-        self.engine.set_levels(table, self.env_level)
+        self.engine.set_levels(table, self._env_level)
         # a level's `info` key is returned only when every level defines it the same way
         infos = [dict(getattr(pe, "device_info", None) or {}) for pe in pes]
         self._device_info = {k: v for k, v in infos[0].items() if all(i.get(k) == v for i in infos[1:])}
@@ -256,7 +307,83 @@ class BatchedMiniWorld:
                     self._info_views[key] = (int(spec[1]), [torch.as_tensor(eng.state_array(n), device=dev)
                                                             for n in ("ent_x", "ent_y", "ent_z")])
             self._obs_dict = dict(self._device_obs_extra)
+            if self.dynamic_levels:
+                # the level of each env's current episode (after a terminating step still the one that just ended)
+                self._info["level"] = self.level_tensor
         return self._torch
+
+    # ------------------------------------------------------------------ level changes (dynamic_levels=True)
+    def _views(self):
+        """env_level / next_level / level_weights in place: torch CUDA tensors, or numpy arrays on the kernels' host
+        build (whose state lives in host memory)."""
+        if not self.dynamic_levels:
+            raise RuntimeError("levels are fixed in this batch: construct it with dynamic_levels=True")
+        if self._level_views is None:
+            names = ("env_level", "next_level", "level_weights")
+            if self.engine.host_memory:
+                self._level_views = {n: self.engine.state_array(n) for n in names}
+            else:
+                import torch
+                dev = torch.device("cuda", self.device)
+                self._level_views = {n: torch.as_tensor(self.engine.state_array(n), device=dev) for n in names}
+        return self._level_views
+
+    @property
+    def level_tensor(self):
+        """int32 [N] view of each env's current level (changes only at the env's resets)."""
+        return self._views()["env_level"]
+
+    @property
+    def level_weights(self):
+        """float32 [n_levels] view of the level-sampling weights; update it in place (stream-ordered, no sync).
+        Weights that are not > 0 count as 0; all zero keeps every env on its level at its resets."""
+        return self._views()["level_weights"]
+
+    def set_level_weights(self, weights):
+        """Copy `weights` (sequence, numpy array or tensor of n_levels values) into `level_weights`."""
+        view = self.level_weights
+        n = len(self.level_ids)
+        if tuple(np.shape(weights)) != (n,):
+            raise ValueError("level weights must have shape (%d,), got %s" % (n, tuple(np.shape(weights))))
+        if isinstance(view, np.ndarray):
+            view[:] = np.asarray(weights.cpu() if hasattr(weights, "cpu") else weights, np.float32)
+        else:
+            torch = self._ensure_torch()
+            view.copy_(torch.as_tensor(weights, dtype=torch.float32).to(view.device), non_blocking=False)
+
+    def set_env_level(self, env_ids, levels):
+        """Move the listed envs to `levels` (one level, or one per env) at their next reset; envs in mid-episode finish
+        it on their current level.  An env listed more than once takes its last entry."""
+        ids = np.atleast_1d(np.asarray(env_ids))
+        lv = np.broadcast_to(np.asarray(levels), ids.shape) if np.ndim(levels) == 0 else np.asarray(levels)
+        if lv.shape != ids.shape:
+            raise ValueError("set_env_level: %d env ids but %d levels" % (ids.size, lv.size))
+        if ids.size == 0:
+            return
+        if not (np.issubdtype(ids.dtype, np.integer) and np.issubdtype(lv.dtype, np.integer)):
+            raise ValueError("set_env_level takes integer env ids and levels")
+        if ids.min() < 0 or ids.max() >= self.num_envs:
+            raise ValueError("env ids must lie in [0, %d)" % self.num_envs)
+        if lv.min() < 0 or lv.max() >= len(self.level_ids):
+            raise ValueError("levels must lie in [0, %d)" % len(self.level_ids))
+        last = ids.size - 1 - np.unique(ids[::-1], return_index=True)[1]    # an env listed twice: its last entry wins
+        ids, lv = ids[last], lv[last]
+        view = self._views()["next_level"]
+        if isinstance(view, np.ndarray):
+            view[ids] = lv.astype(np.int32)
+        else:
+            import torch
+            view[torch.as_tensor(ids.astype(np.int64), device=view.device)] = torch.as_tensor(
+                lv.astype(np.int32), device=view.device)
+
+    @property
+    def env_level(self):
+        """numpy int32 [N]: the level of each env.  With dynamic_levels it is a host copy of `level_tensor` and
+        synchronises with the device (the current torch stream) to read it."""
+        if not self.dynamic_levels:
+            return self._env_level
+        view = self.level_tensor
+        return np.array(view) if isinstance(view, np.ndarray) else view.cpu().numpy()
 
     def _wrap(self, obs):
         """Observation / info as the level's own step() shapes them (Sign: {"obs", "goal"}, sign.py:176)."""
@@ -284,7 +411,7 @@ class BatchedMiniWorld:
             if seeds is not None:
                 states = np.array([rng_state_of(s) for s in seeds], RNG_DTYPE)
                 self.engine.seed(ids, states)
-            self.engine.reset(None if env_ids is None else ids)
+            self.engine.reset(None if env_ids is None else ids, stream=self._level_stream())
         else:
             self._host_reset(ids, seeds)
         self._seeded = True
@@ -353,7 +480,8 @@ class BatchedMiniWorld:
             self._host_reset(np.nonzero(self._host_done)[0].astype(np.int32), None, hold=True)
             self._host_done[:] = False
         self.engine.step(acts, obs=out["obs"] if render else None, depth=out.get("depth") if render else None,
-                         reward=out["reward"], terminated=out["terminated"], truncated=out["truncated"])
+                         reward=out["reward"], terminated=out["terminated"], truncated=out["truncated"],
+                         stream=self._level_stream())
         if not self.device_reset and self.autoreset:
             self._host_done = (out["terminated"] | out["truncated"]).astype(bool)
         return out
@@ -376,11 +504,26 @@ class BatchedMiniWorld:
         """Checkpoint of all envs (numpy uint8 blob); `restore` resumes them bit for bit."""
         if not self.device_reset:
             raise TypeError("snapshot covers the device-resident state; host-reset levels keep RNG streams in Python")
+        self._sync_level_writes()
         return self.engine.snapshot()
 
     def restore(self, blob):
+        self._sync_level_writes()
         self.engine.restore(blob)
         self._seeded = True
+
+    def _level_stream(self):
+        """Stream for a call whose resets read next_level / level_weights: with level changes on, torch's current
+        stream, so that the resets run behind the torch work that wrote those arrays (set_env_level, set_level_weights,
+        in-place writes); otherwise None, the handle's own stream.  Calls with host outputs still return finished."""
+        if self.dynamic_levels and not self.engine.host_memory:
+            return _torch_stream(self._ensure_torch(), self.device)
+        return None
+
+    def _sync_level_writes(self):
+        """Finish torch writes to next_level / level_weights before the handle's own stream reads or replaces them."""
+        if self.dynamic_levels and not self.engine.host_memory:
+            self._ensure_torch().cuda.current_stream(self.device).synchronize()
 
     def set_action_noise(self, prob=0.9, random_action=None):
         """Device-side StochasticActionWrapper (reference wrappers.py:49-71) for every env: the replacement draws

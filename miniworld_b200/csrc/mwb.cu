@@ -117,6 +117,7 @@ struct mwb_handle {
   bool smem_tris;
   int stage_bytes;
   bool have_params, have_protos, have_template;
+  bool have_level_table;          // mwb_set_levels succeeded (mwb_enable_level_changes needs it)
   // level table (host copies of S.levels / S.env_level / S.ops); a handle that never calls mwb_set_levels has one level
   std::vector<LevelDev> levels;
   std::vector<int32_t> env_level;
@@ -211,14 +212,8 @@ static int stream_leave(mwb_handle*, stream_t) { return 0; }
 #endif
 
 // ------------------------------------------------------------------ kernels / loops
-// K1 runs an env's scalar logic on all 32 lanes of a warp with identical values (every store writes the same value).
-// The read-modify-write sequences on per-env state (step counter, RNG stream, entity list edits) rely on the lanes
-// not drifting apart between the loads and the stores: explicit warp barriers pin that down.
-#ifdef __CUDA_ARCH__
-#define MWB_WARP_SYNC() __syncwarp()
-#else
-#define MWB_WARP_SYNC()
-#endif
+// K1 runs an env's scalar logic on all 32 lanes of a warp with identical values (every store writes the same value);
+// MWB_WARP_SYNC (state.h) keeps the lanes together across its read-modify-write sequences.
 
 MWB_DEV void step_one(const DevState& S, int i, const int32_t* actions, const double* step_params, double* reward,
                       uint8_t* term, uint8_t* trunc) {
@@ -598,6 +593,7 @@ extern "C" int mwb_create(const mwb_config* cfg, mwb_handle** out) {
   h->profiling = false;
   h->frames_copied = false;
   h->have_params = h->have_protos = h->have_template = false;
+  h->have_level_table = false;
 #ifndef MWB_HOSTSIM
   h->atlas = nullptr;
 #endif
@@ -651,6 +647,7 @@ extern "C" int mwb_create(const mwb_config* cfg, mwb_handle** out) {
     L0.max_episode_steps = cfg->max_episode_steps;
     h->levels.assign(1, L0);
     h->env_level.assign(N, 0);
+    S.num_levels = 1;
   }
   const size_t G = cfg->shared_geometry ? 1 : N;
   h->geom_blocks = (int)G;
@@ -1027,12 +1024,14 @@ static int drain(mwb_handle* h) {
   return sync_stream(h->stream) == 0 ? MWB_OK : fail(MWB_ECUDA, "sync failed");
 }
 
-// the host copies of the level table and of env_level -> S.levels / S.env_level
+// the host copies of the level table and of env_level -> S.levels / S.env_level (once level changes are on, the
+// device's env_level is the authoritative one and is left alone)
 static int upload_levels(mwb_handle* h) {
   int rc = drain(h);
   if (rc) return rc;
   rc |= h2d((void*)h->S.levels, h->levels.data(), h->levels.size() * sizeof(LevelDev), h->stream);
-  rc |= h2d((void*)h->S.env_level, h->env_level.data(), h->env_level.size() * sizeof(int32_t), h->stream);
+  if (!h->S.next_level)
+    rc |= h2d((void*)h->S.env_level, h->env_level.data(), h->env_level.size() * sizeof(int32_t), h->stream);
   rc |= sync_stream(h->stream);
   return rc ? fail(MWB_ECUDA, "level table upload failed") : MWB_OK;
 }
@@ -1169,6 +1168,7 @@ extern "C" int mwb_set_levels(mwb_handle* h, int n_levels, const mwb_level* leve
                               const mwb_op* ops, int n_ops, const int32_t* env_level) {
   if (!h || !levels || !templates || !ops || !env_level) return fail(MWB_EINVAL, "null argument");
   if (!h->S.shared_geom) return fail(MWB_EINVAL, "a level table needs shared_geometry = 1 (per-env worlds have no templates)");
+  if (h->S.next_level) return fail(MWB_ESTATE, "the level table is fixed once level changes are on");
   if (n_levels <= 0) return fail(MWB_EINVAL, "n_levels must be positive");
   if (n_levels > MWB_LEVEL_CAP) return fail(MWB_ECAPACITY, "more than MWB_LEVEL_CAP levels");
   if (n_ops <= 0) return fail(MWB_EINVAL, "empty op array");
@@ -1208,8 +1208,44 @@ extern "C" int mwb_set_levels(mwb_handle* h, int n_levels, const mwb_level* leve
   rc = upload_ops(h);
   if (!rc) rc = upload_levels(h);
   if (rc) return rc;
+  h->S.num_levels = n_levels;
   h->have_params = h->have_template = true;
+  h->have_level_table = true;
   return MWB_OK;
+}
+
+extern "C" int mwb_enable_level_changes(mwb_handle* h, uint64_t seed, int32_t env_offset) {
+  if (!h) return fail(MWB_EINVAL, "null handle");
+  if (!h->have_level_table) return fail(MWB_ESTATE, "level changes need a level table (mwb_set_levels first)");
+  if (h->S.next_level) return fail(MWB_ESTATE, "level changes are already on");
+  if (env_offset < 0) return fail(MWB_EINVAL, "env_offset must not be negative");
+  DevState& S = h->S;
+  int rc = drain(h);
+  if (rc) return rc;
+  int32_t* next = nullptr;
+  uint32_t* draws = nullptr;
+  float* weights = nullptr;
+  if (alloc_arr(h, &next, S.N) || alloc_arr(h, &draws, S.N) || alloc_arr(h, &weights, (size_t)S.num_levels))
+    return fail(MWB_ECUDA, "level-change state allocation failed");
+  if (dev_memset(next, 0xFF, (size_t)S.N * sizeof(int32_t)) != 0) return fail(MWB_ECUDA, "memset failed");   // all -1
+  S.next_level = next;
+  S.level_draws = draws;
+  S.level_weights = weights;       // zeros: no draws until weights are set
+  S.level_seed = seed;
+  S.level_env_offset = env_offset;
+  return MWB_OK;
+}
+
+// env_level[env] as the kernels see it: the host copy, or the device array once level changes are on
+static int current_level(mwb_handle* h, int env, int32_t* out) {
+  if (!h->S.next_level) {
+    *out = h->env_level[env];
+    return MWB_OK;
+  }
+  int rc = stream_enter(h, h->stream);
+  rc |= d2h(out, h->S.env_level + env, sizeof(int32_t), h->stream);
+  rc |= sync_stream(h->stream);
+  return rc ? fail(MWB_ECUDA, "readback failed") : MWB_OK;
 }
 
 extern "C" int mwb_set_maze(mwb_handle* h, const mwb_maze_desc* mz) {
@@ -1242,7 +1278,9 @@ extern "C" int mwb_set_maze(mwb_handle* h, const mwb_maze_desc* mz) {
 extern "C" int mwb_get_geometry(mwb_handle* h, int env, int32_t counts[3], mwb_room* rooms, mwb_quad* quads, mwb_seg* segs) {
   if (!h || !counts) return fail(MWB_EINVAL, "null argument");
   if (env < 0 || env >= h->S.N) return fail(MWB_EINVAL, "env out of range");
-  const size_t g = h->S.shared_geom ? (size_t)h->env_level[env] : (size_t)env;
+  int32_t lvl = 0;
+  if (h->S.shared_geom && current_level(h, env, &lvl) != MWB_OK) return MWB_ECUDA;
+  const size_t g = h->S.shared_geom ? (size_t)lvl : (size_t)env;
   int rc = 0;
   rc |= stream_enter(h, h->stream);
   rc |= d2h(&counts[0], h->S.num_rooms + g, sizeof(int32_t), h->stream);
@@ -1800,6 +1838,10 @@ extern "C" int mwb_visible_ents(mwb_handle* h, uint32_t* mask, void* stream) {
 // ------------------------------------------------------------------ ABI: snapshot / restore
 // Every array that changes while episodes run (entity lists, counters, camera / lighting parameters, RNG
 // streams, pending-reset flags) plus the geometry currently on the device, in one fixed order.
+// the magic names the blob's mode: a handle with level changes on writes (and needs) the level-change section
+static const uint32_t kSnapMagic = 0x5342574du;               // "MWBS"
+static const uint32_t kSnapMagicLevelChanges = 0x4c42574du;   // "MWBL"
+
 struct SnapHeader {
   uint32_t magic, abi;
   int32_t N, E, R, Q, S, G;
@@ -1809,8 +1851,22 @@ struct SnapHeader {
 // geometry blocks a snapshot carries: one template per level, or one world per env
 static size_t snapshot_blocks(const mwb_handle* h) { return h->S.shared_geom ? h->levels.size() : (size_t)h->S.N; }
 
-// a handle with several levels appends its env_level [N] to the blob (checked on restore, never overwritten)
-static size_t snapshot_level_bytes(const mwb_handle* h) { return h->levels.size() > 1 ? h->env_level.size() * sizeof(int32_t) : 0; }
+// the level-change section of a snapshot: next_level [N], level_draws [N], level_weights [L], then this
+struct LevelChangeTail {
+  uint64_t seed;
+  int32_t env_offset, reserved;
+};
+
+// a handle with several levels appends its env_level [N] to the blob (checked on restore, never overwritten); one with
+// level changes on always does, followed by the level-change section (adopted on restore: the assignment is state)
+static size_t level_change_bytes(const mwb_handle* h) {
+  return (size_t)h->S.N * (sizeof(int32_t) + sizeof(uint32_t)) + (size_t)h->S.num_levels * sizeof(float) + sizeof(LevelChangeTail);
+}
+static size_t snapshot_level_bytes(const mwb_handle* h) {
+  const bool level_changes = h->S.next_level != nullptr;
+  const size_t assignment = h->levels.size() > 1 || level_changes ? h->env_level.size() * sizeof(int32_t) : 0;
+  return assignment + (level_changes ? level_change_bytes(h) : 0);
+}
 
 static void snapshot_arrays(mwb_handle* h, std::vector<std::pair<void*, size_t>>& v) {
   const DevState& S = h->S;
@@ -1830,7 +1886,7 @@ static SnapHeader snapshot_header(mwb_handle* h) {
   std::vector<std::pair<void*, size_t>> v;
   snapshot_arrays(h, v);
   SnapHeader hd;
-  hd.magic = 0x5342574du;   // "MWBS"
+  hd.magic = h->S.next_level ? kSnapMagicLevelChanges : kSnapMagic;
   hd.abi = MWB_ABI_VERSION;
   hd.N = h->S.N; hd.E = h->S.E; hd.R = h->S.R; hd.Q = h->S.Q; hd.S = h->S.S;
   hd.G = (int32_t)snapshot_blocks(h);
@@ -1859,8 +1915,25 @@ extern "C" int mwb_snapshot(mwb_handle* h, void* blob, size_t bytes) {
     if (d2h(p, v[k].first, v[k].second, h->stream) != 0) return fail(MWB_ECUDA, "readback failed");
     p += v[k].second;
   }
+  if (h->S.next_level) {
+    const DevState& S = h->S;
+    int rc = d2h(p, S.env_level, (size_t)S.N * sizeof(int32_t), h->stream);
+    p += (size_t)S.N * sizeof(int32_t);
+    rc |= d2h(p, S.next_level, (size_t)S.N * sizeof(int32_t), h->stream);
+    p += (size_t)S.N * sizeof(int32_t);
+    rc |= d2h(p, S.level_draws, (size_t)S.N * sizeof(uint32_t), h->stream);
+    p += (size_t)S.N * sizeof(uint32_t);
+    rc |= d2h(p, S.level_weights, (size_t)S.num_levels * sizeof(float), h->stream);
+    p += (size_t)S.num_levels * sizeof(float);
+    LevelChangeTail tail;
+    memset(&tail, 0, sizeof(tail));
+    tail.seed = S.level_seed;
+    tail.env_offset = S.level_env_offset;
+    memcpy(p, &tail, sizeof(tail));
+    if (rc) return fail(MWB_ECUDA, "readback failed");
+  }
   if (sync_stream(h->stream) != 0) return fail(MWB_ECUDA, "sync failed");
-  if (snapshot_level_bytes(h)) memcpy(p, h->env_level.data(), snapshot_level_bytes(h));
+  if (!h->S.next_level && snapshot_level_bytes(h)) memcpy(p, h->env_level.data(), snapshot_level_bytes(h));
   return MWB_OK;
 }
 
@@ -1870,7 +1943,12 @@ extern "C" int mwb_restore(mwb_handle* h, const void* blob, size_t bytes) {
   SnapHeader hd;
   if (bytes < sizeof(hd)) return fail(MWB_EINVAL, "not a snapshot");
   memcpy(&hd, blob, sizeof(hd));
-  if (hd.magic != want.magic || hd.abi != want.abi) return fail(MWB_EABI, "snapshot from another ABI version");
+  if ((hd.magic != kSnapMagic && hd.magic != kSnapMagicLevelChanges) || hd.abi != want.abi)
+    return fail(MWB_EABI, "snapshot from another ABI version");
+  const bool dynamic = h->S.next_level != nullptr;
+  if (hd.magic != want.magic)
+    return fail(MWB_ESTATE, dynamic ? "snapshot of a handle without level changes (this one has them on)"
+                                    : "snapshot of a handle with level changes on (this one has them off)");
   if (hd.N != want.N || hd.E != want.E || hd.R != want.R || hd.Q != want.Q || hd.S != want.S)
     return fail(MWB_EINVAL, "snapshot does not match this handle's configuration");
   if (hd.G != want.G || hd.bytes != want.bytes)
@@ -1880,13 +1958,39 @@ extern "C" int mwb_restore(mwb_handle* h, const void* blob, size_t bytes) {
   std::vector<std::pair<void*, size_t>> v;
   snapshot_arrays(h, v);
   const size_t lb = snapshot_level_bytes(h);
-  if (lb && memcmp((const unsigned char*)blob + hd.bytes - lb, h->env_level.data(), lb) != 0)
+  if (!dynamic && lb && memcmp((const unsigned char*)blob + hd.bytes - lb, h->env_level.data(), lb) != 0)
     return fail(MWB_ESTATE, "snapshot assigns envs to other levels than this handle");
   const unsigned char* p = (const unsigned char*)blob + sizeof(hd);
+  LevelChangeTail tail;
+  if (dynamic) {
+    // the kernels index the level table with the blob's assignment (pending entries outside [-1, L) are ignored anyway)
+    const DevState& S = h->S;
+    const unsigned char* q = p;
+    for (size_t k = 0; k < v.size(); ++k) q += v[k].second;
+    std::vector<int32_t> lv((size_t)S.N);
+    memcpy(lv.data(), q, lv.size() * sizeof(int32_t));
+    for (size_t k = 0; k < lv.size(); ++k)
+      if (lv[k] < 0 || lv[k] >= S.num_levels) return fail(MWB_EINVAL, "snapshot assigns an env to a level this handle does not have");
+    memcpy(&tail, (const unsigned char*)blob + hd.bytes - sizeof(tail), sizeof(tail));
+    if (tail.env_offset < 0) return fail(MWB_EINVAL, "snapshot has a negative env offset");
+  }
   if (stream_enter(h, h->stream)) return MWB_ECUDA;
   for (size_t k = 0; k < v.size(); ++k) {
     if (h2d(v[k].first, p, v[k].second, h->stream) != 0) return fail(MWB_ECUDA, "upload failed");
     p += v[k].second;
+  }
+  if (dynamic) {
+    DevState& S = h->S;
+    int rc = h2d(S.env_level, p, (size_t)S.N * sizeof(int32_t), h->stream);
+    p += (size_t)S.N * sizeof(int32_t);
+    rc |= h2d(S.next_level, p, (size_t)S.N * sizeof(int32_t), h->stream);
+    p += (size_t)S.N * sizeof(int32_t);
+    rc |= h2d(S.level_draws, p, (size_t)S.N * sizeof(uint32_t), h->stream);
+    p += (size_t)S.N * sizeof(uint32_t);
+    rc |= h2d((void*)S.level_weights, p, (size_t)S.num_levels * sizeof(float), h->stream);
+    if (rc) return fail(MWB_ECUDA, "upload failed");
+    S.level_seed = tail.seed;
+    S.level_env_offset = tail.env_offset;
   }
   if (sync_stream(h->stream) != 0) return fail(MWB_ECUDA, "sync failed");
   return MWB_OK;
@@ -1942,9 +2046,25 @@ extern "C" int mwb_state_array(mwb_handle* h, int which, void** dev_ptr, int64_t
     case MWB_ARRAY_ENT_Y: *dev_ptr = h->S.ent_py; *count = E * N; break;
     case MWB_ARRAY_ENT_Z: *dev_ptr = h->S.ent_pz; *count = E * N; break;
     case MWB_ARRAY_ENT_DIR: *dev_ptr = h->S.ent_dir; *count = E * N; break;
+    case MWB_ARRAY_ENV_LEVEL:
+    case MWB_ARRAY_NEXT_LEVEL:
+    case MWB_ARRAY_LEVEL_WEIGHTS:
+      if (!h->S.next_level) return fail(MWB_ESTATE, "level changes are off (mwb_enable_level_changes)");
+      if (which == MWB_ARRAY_ENV_LEVEL) { *dev_ptr = h->S.env_level; *count = N; }                       // int32 [N]
+      else if (which == MWB_ARRAY_NEXT_LEVEL) { *dev_ptr = h->S.next_level; *count = N; }                // int32 [N]
+      else { *dev_ptr = (void*)h->S.level_weights; *count = h->S.num_levels; }                           // float32 [L]
+      break;
     default: return fail(MWB_EINVAL, "unknown array");
   }
   return MWB_OK;
+}
+
+extern "C" int mwb_state_in_host_memory(void) {
+#ifdef MWB_HOSTSIM
+  return 1;
+#else
+  return 0;
+#endif
 }
 
 extern "C" int mwb_get_state(mwb_handle* h, const mwb_state_view* out) {

@@ -24,14 +24,63 @@ MWB_DEV void draw_room_textures(const DevState& S, int i, const mwb_room* rooms,
     }
 }
 
+// splitmix64 (Steele, Lea, Flood 2014): the output at position k of the generator seeded with `seed`
+MWB_DEV uint64_t splitmix64_at(uint64_t seed, uint64_t k) {
+  uint64_t z = seed + (k + 1) * 0x9E3779B97F4A7C15ull;
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  return z ^ (z >> 31);
+}
+
+// The level env i runs from this reset on (mwb_enable_level_changes; include/mwb.h states the rule and the draw).
+// Every lane of the warp computes the same value from the same loads; the stores follow a warp barrier, so that no
+// lane reads a value another lane has already replaced.
+MWB_DEV int resolve_level(const DevState& S, int i) {
+  MWB_WARP_SYNC();
+  const int cur = S.env_level[i];
+  const int pending = S.next_level[i];
+  uint32_t draws = S.level_draws[i];
+  int lvl = cur;
+  if (pending >= 0 && pending < S.num_levels) {
+    lvl = pending;
+  } else {
+    float total = 0.0f;
+    for (int l = 0; l < S.num_levels; ++l) {
+      const float w = S.level_weights[l];
+      if (w > 0.0f) total = f_add(total, w);
+    }
+    if (total > 0.0f) {
+      const uint64_t k = ((uint64_t)((uint32_t)S.level_env_offset + (uint32_t)i) << 32) | draws;
+      const uint32_t u24 = (uint32_t)(splitmix64_at(S.level_seed, k) >> 40);
+      const float target = f_mul(f_mul((float)u24, 5.9604644775390625e-08f), total);   // u24 * 2^-24 * total
+      float cdf = 0.0f;
+      for (int l = 0; l < S.num_levels; ++l) {
+        const float w = S.level_weights[l];
+        if (!(w > 0.0f)) continue;
+        cdf = f_add(cdf, w);
+        lvl = l;
+        if (cdf > target) break;
+      }
+      ++draws;
+    }
+  }
+  MWB_WARP_SYNC();
+  if (pending != -1) S.next_level[i] = -1;
+  S.level_draws[i] = draws;
+  S.env_level[i] = lvl;
+  MWB_WARP_SYNC();
+  return lvl;
+}
+
 MWB_DEV void device_reset(const DevState& S, int i) {
   const size_t N = S.N;
   NpRng rng = load_rng(S, i);
-  const LevelDev& L = env_level_of(S, i);
+  const int lvl = S.next_level ? resolve_level(S, i) : S.env_level[i];
+  const LevelDev& L = S.levels[lvl];
   const mwb_params& P = L.params;
   const mwb_op* ops = S.ops + L.op_first;
   const int num_ops = L.num_ops;
-  const int g = geom_index(S, i);
+  const int g = S.shared_geom ? lvl : i;
   const mwb_room* rooms = S.rooms + (size_t)g * S.R;
   int n_rooms = S.num_rooms[g];
 

@@ -12,6 +12,15 @@
 #define MWB_MAX_BINS 640         // half-tiles of one entity's screen box that can be binned (160x120 frame: 600)
 #define MWB_BIN_REFS 6           // bin references per listed triangle the index buffer has room for
 
+// K1 runs an env's scalar logic on all 32 lanes of a warp with identical values (every store writes the same value).
+// The read-modify-write sequences on per-env state (step counter, RNG stream, entity list edits, level resolution) rely
+// on the lanes not drifting apart between the loads and the stores: explicit warp barriers pin that down.
+#ifdef __CUDA_ARCH__
+#define MWB_WARP_SYNC() __syncwarp()
+#else
+#define MWB_WARP_SYNC()
+#endif
+
 struct TriRec;
 struct MeshSegInfo;
 struct MazeDev;
@@ -97,7 +106,15 @@ struct DevState {
   int32_t num_protos;
   const mwb_op* ops;            // every level's reset program, one after another
   const LevelDev* levels;       // [levels] rule, truncation, params, program slice
-  const int32_t* env_level;     // [N] level of each env (all 0 on a one-level handle)
+  int32_t* env_level;           // [N] level of each env (all 0 on a one-level handle); with level changes on, the
+                                //     resets rewrite it (device_reset: resolve_level)
+  int32_t num_levels;
+  // level changes at resets (mwb_enable_level_changes); null on a handle without them
+  int32_t* next_level;          // [N] pending assignment, -1 = none
+  uint32_t* level_draws;        // [N] level draws made so far (counter of the draw hash)
+  const float* level_weights;   // [num_levels] sampling weights, all <= 0 = keep the level
+  uint64_t level_seed;
+  int32_t level_env_offset;     // global index of env 0 (sharded runs)
   int32_t domain_rand;
   int32_t autoreset;
   // StochasticActionWrapper on the device (reference wrappers.py:49-71): per step one uniform() draw from

@@ -23,7 +23,8 @@ class ShardedMiniWorld:
 
     def __init__(self, level, total_envs, dist=None, device=0, env_level=None, **kwargs):
         """`level` may be a sequence of levels as for BatchedMiniWorld; `env_level` is then the assignment of all
-        `total_envs` envs (default: contiguous near-equal blocks), and this rank runs its slice of it."""
+        `total_envs` envs (default: contiguous near-equal blocks), and this rank runs its slice of it.  With
+        `dynamic_levels=True` (and `level_seed`) the level draws of global env i are those of the single-process run."""
         from .batched import BatchedMiniWorld, default_env_level
         self.dist = dist
         self.rank = dist.get_rank() if dist is not None else 0
@@ -40,6 +41,8 @@ class ShardedMiniWorld:
             kwargs["env_level"] = env_level[self.start:self.start + self.count]
         elif env_level is not None:
             raise ValueError("env_level assigns envs to levels: pass `level` as a sequence of levels")
+        if kwargs.get("dynamic_levels"):
+            kwargs["env_offset"] = self.start      # level draws keyed by the global env index: same draws as one process
         self.local = BatchedMiniWorld(level, self.count, device=device, **kwargs)
 
     def reset(self, seed):

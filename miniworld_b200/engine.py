@@ -10,7 +10,7 @@ import os
 
 import numpy as np
 
-ABI_VERSION = 7
+ABI_VERSION = 8
 RULE_NONE, RULE_GOAL, RULE_PICKUP, RULE_SIDEWALK, RULE_SIGN, RULE_HEALTH, RULE_PUTNEXT = 0, 1, 2, 3, 4, 5, 6
 SURF_WALL, SURF_FLOOR, SURF_CEIL = 0, 1, 2
 OP_END, OP_CHOICE, OP_UNIFORM, OP_PLACE, OP_MAZE, OP_IFEQ, OP_PUT = 0, 1, 2, 3, 4, 5, 6
@@ -128,7 +128,7 @@ EXPORTS = (
     "mwb_render_top_view", "mwb_visible_ents", "mwb_set_action_noise",
     "mwb_snapshot_size", "mwb_snapshot", "mwb_restore", "mwb_set_obs_format",
     "mwb_flag_write", "mwb_flag_wait_geq", "mwb_flag_mode", "mwb_state_array", "mwb_debug_camera", "mwb_set_obs_peer",
-    "mwb_set_levels",
+    "mwb_set_levels", "mwb_enable_level_changes", "mwb_state_in_host_memory",
 )
 OBS_FORMATS = {"hwc": 0, "cwh": 1, "grey": 2}
 
@@ -166,6 +166,8 @@ def load_library():
     lib.mwb_set_template.argtypes = [vp, C.POINTER(Geometry)]
     lib.mwb_set_program.argtypes = [vp, vp, C.c_int]
     lib.mwb_set_levels.argtypes = [vp, C.c_int, vp, vp, vp, C.c_int, vp]
+    lib.mwb_enable_level_changes.argtypes = [vp, C.c_uint64, C.c_int32]
+    lib.mwb_state_in_host_memory.argtypes = []
     lib.mwb_seed.argtypes = [vp, vp, C.c_int, vp]
     lib.mwb_reset.argtypes = [vp, vp, C.c_int, vp]
     lib.mwb_set_world.argtypes = [vp, vp, C.c_int, vp]
@@ -323,6 +325,9 @@ class Engine:
         self.max_ents, self.max_rooms = int(max_ents), int(max_rooms)
         self._tex_uploaded = 0
         self._mesh_uploaded = 0
+        self.num_levels = 1
+        # the CPU build of the kernels (tests) keeps its "device" arrays in host memory
+        self.host_memory = bool(self.lib.mwb_state_in_host_memory())
 
     def _check(self, rc):
         if rc != 0:
@@ -445,6 +450,12 @@ class Engine:
         self._keep = [lv["geometry"] for lv in levels]
         self._check(self.lib.mwb_set_levels(self.h, n, C.cast(table, C.c_void_p), C.cast(geoms, C.c_void_p),
                                             _ptr(ops), len(ops), _ptr(env_level)))
+        self.num_levels = n
+
+    def enable_level_changes(self, seed=0, env_offset=0):
+        """Levels change at resets from now on (mwb_enable_level_changes): pending assignments ("next_level") and
+        draws from "level_weights", keyed by `seed` and the env's global index env_offset + i."""
+        self._check(self.lib.mwb_enable_level_changes(self.h, int(seed) & (2 ** 64 - 1), int(env_offset)))
 
     # ---- reset
     def seed(self, env_ids, states):
@@ -521,16 +532,27 @@ class Engine:
         """uint32[N] (numpy or CUDA tensor): bit e = entity slot e passes the reference's occlusion query."""
         self._check(self.lib.mwb_visible_ents(self.h, _dev_or_host_ptr(mask), stream))
 
-    ARRAYS = {"counter": (0, "<i4"), "step_count": (1, "<i4"), "ent_x": (2, "<f8"), "ent_y": (3, "<f8"),
-              "ent_z": (4, "<f8"), "ent_dir": (5, "<f8")}
+    # name -> (mwb_state_array id, element type, leading axis: "env" = [N] or [k, N], "level" = [n_levels])
+    ARRAYS = {"counter": (0, "<i4", "env"), "step_count": (1, "<i4", "env"), "ent_x": (2, "<f8", "env"),
+              "ent_y": (3, "<f8", "env"), "ent_z": (4, "<f8", "env"), "ent_dir": (5, "<f8", "env"),
+              "env_level": (6, "<i4", "env"), "next_level": (7, "<i4", "env"), "level_weights": (8, "<f4", "level")}
 
     def state_array(self, name):
-        """Zero-copy view of a per-env device state array (mwb_state_array) as an object with
-        __cuda_array_interface__: "counter" / "step_count" int32 [N]; "ent_x|y|z|dir" float64 [max_ents, N]."""
-        which, typestr = self.ARRAYS[name]
+        """Zero-copy view of a state array (mwb_state_array) as an object with __cuda_array_interface__:
+        "counter" / "step_count" int32 [N]; "ent_x|y|z|dir" float64 [max_ents, N]; with level changes on,
+        "env_level" / "next_level" int32 [N] and "level_weights" float32 [n_levels].  On the host build of the
+        kernels the arrays live in host memory, and the view is a numpy array over the same memory instead."""
+        which, typestr, axis = self.ARRAYS[name]
         ptr, count = C.c_void_p(), C.c_int64()
         self._check(self.lib.mwb_state_array(self.h, which, C.byref(ptr), C.byref(count)))
-        shape = (self.N,) if count.value == self.N else (count.value // self.N, self.N)
+        if axis == "level" or count.value == self.N:
+            shape = (count.value,)
+        else:
+            shape = (count.value // self.N, self.N)
+        if self.host_memory:
+            dt = np.dtype(typestr)
+            buf = (C.c_char * (count.value * dt.itemsize)).from_address(ptr.value)
+            return np.frombuffer(buf, dt).reshape(shape)
 
         class _View:
             __cuda_array_interface__ = {"shape": shape, "typestr": typestr, "data": (ptr.value, False), "version": 3, "strides": None}
