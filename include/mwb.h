@@ -413,8 +413,10 @@ int mwb_restore(mwb_handle* h, const void* blob, size_t bytes);
 /* number of kernels this handle has launched so far (bench.py's gpu_launches) */
 int64_t mwb_launch_count(mwb_handle* h);
 
-/* capacity faults (must stay 0): frames whose culled triangle list did not fit the kernel's budget, device-side maze
- * generation that ran out of room / quad / segment capacity (the env is left empty instead of searching forever) */
+/* capacity faults (must stay 0): frames whose culled triangle list did not fit the kernel's budget, frames that keep
+ * more than 65 535 triangles after culling (triangle ids are 16-bit and 0xFFFF is the sky: about 26 full Balls in
+ * view; such a frame renders wrong), device-side maze generation that ran out of room / quad / segment capacity (the
+ * env is left empty instead of searching forever) */
 int64_t mwb_overflow_count(mwb_handle* h);
 
 /* Device-side timing of the two kernels: when enabled, every K1 / K2 launch is bracketed by

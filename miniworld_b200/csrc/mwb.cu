@@ -433,6 +433,7 @@ static void hostsim_render_t(const DevState& S, const RenderAssets& A, const Vie
       tris.push_back(rec);
       pairable.push_back(0);
     }
+    if (tris.size() > MWB_MAX_SLOTS) *S.fault += 1;     // like K2: slots are 16-bit
     // like K2, visit the triangles front to back by their nearest possible depth; slots keep draw order
     std::vector<int> order(tris.size());
     std::vector<float> zmin(tris.size());

@@ -445,6 +445,7 @@ render_kernel(DevState S, RenderAssets A, ViewSpec view, int fmt, uint8_t* __res
       sg.base = slot;
       slot += (sg.count + 1) & ~1;       // even bases: slot parity == record parity inside every list (quad pairs)
     }
+    if (slot > MWB_MAX_SLOTS) atomicAdd(overflow, 1);
   }
   __syncthreads();
   const int nsegs = 1 + fmap.n_ents + (fmap.agent_task >= 0 ? 1 : 0);

@@ -31,6 +31,9 @@
 #define MWB_FAR 100.0
 #define MWB_MAX_LEVELS 12
 #define MWB_SKY_KEY 0xFFFF0000u
+// A frame numbers the triangles it keeps with 16-bit slots (the low half of a sample key, the exact-queue item's
+// low bits); id 0xFFFF names the sky.  A frame needing more slots renders wrong and is counted as a capacity fault.
+#define MWB_MAX_SLOTS 65535
 
 struct TexDev {
   int32_t w, h, nlev, pad;

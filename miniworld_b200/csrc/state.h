@@ -55,7 +55,8 @@ struct DevState {
   int32_t* num_picked;          // [N]
   int32_t* needs_reset;         // [N] set by a terminated|truncated step when autoreset
   unsigned long long* episodes_done;   // [1] device counter of episode-ending steps
-  int32_t* fault;               // [1] capacity faults: K2 triangle lists that overflowed, device world generation that ran
+  int32_t* fault;               // [1] capacity faults: K2 triangle lists that overflowed or needed more than MWB_MAX_SLOTS
+                                //     slots, device world generation that ran
                                 //     out of room / quad / segment capacity (mwb_overflow_count; must stay 0)
   double* cam;                  // [4][N]  cam_height, cam_fwd_disp, cam_pitch, cam_fov_y
   double* envp;                 // [12][N] sky_color, light_pos, light_color, light_ambient
