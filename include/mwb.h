@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define MWB_ABI_VERSION 8
+#define MWB_ABI_VERSION 9
 
 /* error codes */
 #define MWB_OK 0
@@ -340,6 +340,19 @@ typedef struct mwb_maze_desc {
   const double* cdf;                 /* [2 rows cols - 1] cumulative room_probs (list order fixed) */
 } mwb_maze_desc;
 int mwb_set_maze(mwb_handle* h, const mwb_maze_desc* maze);
+
+/* Maze levels in a level table (curricula over maze sizes: MazeS2 -> MazeS3 -> Maze, next to fixed-layout levels).
+ * Valid on a shared_geometry = 1 handle after mwb_set_levels (MWB_ESTATE otherwise).  Level `level` (MWB_EINVAL
+ * outside [0, L)) becomes a per-env-world level: every reset of an env at that level carves a fresh maze from these
+ * templates into the env's own world, as mwb_set_maze does for a one-level handle.  MWB_ECAPACITY when the maze has more
+ * than MWB_MAZE_MAX_CELLS (256) cells or does not fit max_rooms (2c - 1 for c cells), max_quads (8c - 2) or max_segs
+ * (4c).  The first call adds one world block per env after the L templates (every env, since level changes can move
+ * any env into a maze level) and fixes the level table (mwb_set_levels returns MWB_ESTATE from then on).  An env's
+ * world holds its last maze until its next reset; envs at template levels read their level's template.
+ * K2 then keeps each level's triangle lists in shared memory or HBM by the level's own size (levels above 512 triangle
+ * records: HBM), and snapshots carry the per-env worlds, marked as such in the header (a restore into a handle without
+ * per-env worlds, or the other way round, fails with MWB_ESTATE before anything else is compared). */
+int mwb_set_level_maze(mwb_handle* h, int level, const mwb_maze_desc* maze);
 
 /* static geometry of one env as currently on the device (tests, debugging); arrays sized by the
  * handle's max_rooms / max_quads / max_segs */

@@ -94,7 +94,10 @@ class BatchedMiniWorld:
     """`level`: a level id or class, or a sequence of them to run several levels side by side in one batch (multi-task
     or curriculum training; env i runs level `env_level[i]`).  With a sequence, `level_kwargs` may be a sequence
     aligned with it, and the observation size, MSAA, domain randomisation, auto-reset and action noise are per batch.
-    Maze-family levels (per-env geometry) and Sign (dict observation) cannot share a batch with other levels.
+    Sign (dict observation) cannot share a batch with other levels.  Maze-family levels can with
+    `per_env_worlds=True`: each env then gets a world block of its own, which a reset at a Maze level fills with a
+    fresh maze (about 123 KB per env with an 8 x 8 Maze in the table, plus about 204 KB per env of HBM triangle
+    lists; about 18 KB per env when the largest maze is MazeS3).  Without a Maze level the flag changes nothing.
 
     `dynamic_levels=True` (with a sequence of levels) lets envs move between levels at their resets, never
     mid-episode: a pending assignment from `set_env_level` wins, otherwise the next level is drawn on the device from
@@ -103,13 +106,14 @@ class BatchedMiniWorld:
 
     def __init__(self, level, num_envs, obs_width=80, obs_height=60, domain_rand=False, autoreset=True,
                  msaa_samples=8, device=0, want_depth=False, level_kwargs=None, obs_format="hwc", env_level=None,
-                 dynamic_levels=False, level_seed=0, env_offset=0):
+                 dynamic_levels=False, level_seed=0, env_offset=0, per_env_worlds=False):
         self.num_envs = int(num_envs)
         self.obs_width, self.obs_height = int(obs_width), int(obs_height)
         self.domain_rand = bool(domain_rand)
         self.want_depth = bool(want_depth)
         self.device = int(device)
         self.dynamic_levels = bool(dynamic_levels)
+        self.per_env_worlds = bool(per_env_worlds)
         if isinstance(level, (list, tuple)):
             self._init_levels(list(level), level_kwargs, env_level, msaa_samples, autoreset)
         else:
@@ -117,6 +121,9 @@ class BatchedMiniWorld:
                 raise ValueError("env_level assigns envs to levels: pass `level` as a sequence of levels")
             if self.dynamic_levels:
                 raise ValueError("dynamic_levels moves envs between levels: pass `level` as a sequence of levels")
+            if self.per_env_worlds:
+                raise ValueError("per_env_worlds lets Maze levels join a level table: pass `level` as a sequence of "
+                                 "levels (a single Maze level always has per-env worlds)")
             self._init_level(level, level_kwargs, msaa_samples, autoreset)
         self._level_views = None
         if self.dynamic_levels:
@@ -235,7 +242,7 @@ class BatchedMiniWorld:
         dr = {"domain_rand": True} if self.domain_rand else {}
         classes = [_resolve_level(lv) for lv in levels]
         names = [lv if isinstance(lv, str) else lv.__name__ for lv in levels]
-        pes, table, protos = [], [], []
+        pes, table, protos, mazes = [], [], [], []
         caps, max_placed = [0, 0, 0], 2
         for name, cls, kw in zip(names, classes, kwargs):
             pe = cls(device=None, obs_width=self.obs_width, obs_height=self.obs_height, **dr, **kw)
@@ -246,14 +253,27 @@ class BatchedMiniWorld:
                 raise ValueError("%s cannot share a batch with other levels: its observation is a dict" % name)
             prog = ResetProgram()
             pe.device_program(prog)
+            maze = None
             if prog.uses_maze:
-                raise ValueError("%s (Maze family) cannot share a batch with other levels: its geometry is per env" % name)
+                if not self.per_env_worlds:
+                    raise ValueError("%s (Maze family) cannot share a batch with other levels: its geometry is per env "
+                                     "(pass per_env_worlds=True to give every env a world of its own)" % name)
+                # a table has no host resets: the device templates must reproduce host-generated mazes exactly
+                from .maze_lowering import MazeTemplate
+                try:
+                    maze = MazeTemplate(cls, domain_rand=self.domain_rand, **kw)
+                    maze.verify(seeds=(0,))
+                except AssertionError as e:
+                    raise ValueError("%s: its maze templates do not reproduce host-generated worlds, and a level table "
+                                     "cannot hold host-reset levels" % name) from e
+                mazes.append((len(table), maze, pack.room_cdf(pe.room_probs)))
             ops = prog.op_array()
             moved = (ops["op"] == OP_PLACE) | (ops["op"] == OP_PUT)     # the ops whose `a` is a proto index
             ops["a"][moved] += len(protos)
             protos.extend(prog.protos)
             geom = pack.pack_geometry(pe)
-            caps = [max(c, len(g)) for c, g in zip(caps, geom)]
+            slack = (0, 8, 8) if maze is not None else (0, 0, 0)         # as a one-level Maze handle is sized
+            caps = [max(c, len(g) + s) for c, g, s in zip(caps, geom, slack)]
             max_placed = max(max_placed, prog.num_placed)
             table.append(dict(rule=(_RULES[rule[0]], rule[1]), max_episode_steps=int(min(pe.max_episode_steps, 2 ** 31 - 1)),
                               params=pe.params, geometry=geom, ops=ops))
@@ -273,6 +293,8 @@ class BatchedMiniWorld:
         self.engine.sync_assets()
         self.engine.set_protos(np.array(protos, PROTO_DTYPE))
         self.engine.set_levels(table, self._env_level)
+        for lvl, tmpl, cdf in mazes:
+            self.engine.set_level_maze(lvl, tmpl, cdf)
         # a level's `info` key is returned only when every level defines it the same way
         infos = [dict(getattr(pe, "device_info", None) or {}) for pe in pes]
         self._device_info = {k: v for k, v in infos[0].items() if all(i.get(k) == v for i in infos[1:])}

@@ -24,6 +24,7 @@ struct MazeDev {
 };
 
 #define MWB_MAZE_MAX_CELLS 256
+#define MWB_MAZE_CDF_STRIDE (2 * MWB_MAZE_MAX_CELLS)   // doubles per level in DevState::maze_cdf (2 cells - 1 used)
 
 MWB_DEV void maze_put_room(mwb_room* dst, const mwb_room& src, double dx, double dz, double cdf) {
   mwb_room r = src;
@@ -61,9 +62,9 @@ MWB_DEV void maze_put_seg(mwb_seg* dst, const mwb_seg& src, double dx, double dz
   dst->bz = d_add(src.bz, dz);
 }
 
-// Generates env i's rooms / quads / segments (per-env geometry blocks).  Returns false if the
-// capacities of the handle are too small.
-MWB_DEV bool maze_generate(const DevState& S, const MazeDev& M, const double* cdf, int i, NpRng& rng) {
+// Generates an env's rooms / quads / segments into geometry block g (the env's own world) from its level's
+// templates M and room cdf.  Returns false if the capacities of the handle are too small.
+MWB_DEV bool maze_generate(const DevState& S, const MazeDev& M, const double* cdf, int g, NpRng& rng) {
   const int R = M.rows, C = M.cols, cells = R * C;
   if (cells > MWB_MAZE_MAX_CELLS || 2 * cells - 1 > S.R) return false;
   // ---- topology: iterative form of visit() -------------------------------------------------
@@ -116,9 +117,9 @@ MWB_DEV bool maze_generate(const DevState& S, const MazeDev& M, const double* cd
     if (!pushed) --depth;
   }
   // ---- geometry, in the reference's list order: grid rooms row by row, then connectors ---------
-  mwb_room* rooms = S.rooms + (size_t)i * S.R;
-  mwb_quad* quads = S.quads + (size_t)i * S.Q;
-  mwb_seg* segs = S.segs + (size_t)i * S.S;
+  mwb_room* rooms = S.rooms + (size_t)g * S.R;
+  mwb_quad* quads = S.quads + (size_t)g * S.Q;
+  mwb_seg* segs = S.segs + (size_t)g * S.S;
   int nr = 0, nq = 0, ns = 0;
   for (int cj = 0; cj < R; ++cj)
     for (int ci = 0; ci < C; ++ci) {
@@ -145,8 +146,8 @@ MWB_DEV bool maze_generate(const DevState& S, const MazeDev& M, const double* cd
     maze_put_seg(segs + ns++, M.conn_segs[d][1], dx, dz);
     ++nr;
   }
-  S.num_rooms[i] = nr;
-  S.num_quads[i] = nq;
-  S.num_segs[i] = ns;
+  S.num_rooms[g] = nr;
+  S.num_quads[g] = nq;
+  S.num_segs[g] = ns;
   return true;
 }

@@ -113,9 +113,14 @@ struct mwb_handle {
   int32_t* d_ids;
   int* d_overflow;
   WorldUpload* d_upload;
-  int tri_cap;
-  bool smem_tris;
+  int tri_cap;                    // K2: the largest level's triangle capacity (visit-order arrays, HBM list stride)
+  int smem_recs;                  // K2: triangle records in shared memory (largest shared-memory level), 0 = none
   int stage_bytes;
+  size_t room_tris_recs;          // records S.room_tris has room for
+  bool level_mazes;               // mwb_set_level_maze succeeded: per-env worlds after the level templates
+  std::vector<int32_t> level_quads;   // quads of every level's worlds (per-level K2 planning of a table with mazes)
+  std::vector<MazeDev> mazes_h;       // host copies of S.maze / S.maze_cdf, one entry per level
+  std::vector<double> maze_cdf_h;
   bool have_params, have_protos, have_template;
   bool have_level_table;          // mwb_set_levels succeeded (mwb_enable_level_changes needs it)
   // level table (host copies of S.levels / S.env_level / S.ops); a handle that never calls mwb_set_levels has one level
@@ -295,15 +300,9 @@ MWB_DEV void scatter_one(const DevState& S, const WorldUpload& u) {
     S.ent_dir[e * N + i] = u.ents[e].dir;
     for (int k = 0; k < 3; ++k) S.ent_col[((size_t)e * 3 + k) * N + i] = u.ents[e].color[k];
   }
-  if (!S.shared_geom) {
-    const mwb_room* rooms = S.rooms + (size_t)i * S.R;
-    for (int r = 0; r < S.num_rooms[i]; ++r)
-      for (int k = 0; k < 3; ++k) S.room_tex[((size_t)i * S.R + r) * 3 + k] = rooms[r].tex_id[k];
-  } else {
-    const int g = geom_index(S, i);
-    for (int r = 0; r < S.num_rooms[g]; ++r)
-      for (int k = 0; k < 3; ++k) S.room_tex[((size_t)i * S.R + r) * 3 + k] = S.rooms[(size_t)g * S.R + r].tex_id[k];
-  }
+  const int g = geom_index(S, i);
+  for (int r = 0; r < S.num_rooms[g]; ++r)
+    for (int k = 0; k < 3; ++k) S.room_tex[((size_t)i * S.R + r) * 3 + k] = S.rooms[(size_t)g * S.R + r].tex_id[k];
 }
 
 MWB_DEV void gather_one(const DevState& S, int i, WorldUpload& u) {
@@ -523,7 +522,7 @@ static void hostsim_render(const DevState& S, const RenderAssets& A, const ViewS
 // row-contiguous stores -- what makes the peer-memory observation path efficient over NVLink (8-byte
 // scattered segments reach ~190 GB/s into one GPU, 128-byte lines several times that).
 static int k2_list_bytes(const mwb_handle* h) {
-  const K2Layout L = k2_layout(h->smem_tris, h->tri_cap, h->stage_bytes, k2_halves_per_part(h->S.obs_w, h->S.obs_h, h->k2_parts), 0);
+  const K2Layout L = k2_layout(h->smem_recs, h->tri_cap, h->stage_bytes, k2_halves_per_part(h->S.obs_w, h->S.obs_h, h->k2_parts), 0);
   return (int)L.stage_off;
 }
 static int k2_frame_stage_bytes(const mwb_handle* h) {
@@ -568,8 +567,88 @@ static int ensure_k2_smem(mwb_handle* h, int smem) {
 }
 #endif
 
+// K2's triangle-list residence and quad staging.  Every room quad and box face can yield two set-up triangles; lists
+// of up to MWB_SMEM_TRI_CAP records live in shared memory, larger ones in HBM (S.room_tris), and a level's static
+// quads are staged in shared memory (TMA bulk copy) when they fit in 16 KB.  A handle without Maze levels in a table
+// decides once from its capacities, for every level alike.  A table with Maze levels (mwb_set_level_maze) decides per
+// level from the level's own quads, so that one 8 x 8 maze does not move every other env's lists to HBM: the shared
+// memory holds the largest shared-memory level's records, the visit-order arrays the largest level's.
+#define MWB_SMEM_TRI_CAP 512
+static void plan_k2(mwb_handle* h) {
+  const int E = h->cfg.max_ents;
+  const auto stage_of = [](int quads) {
+    const int bytes = (int)(((size_t)quads * sizeof(mwb_quad) + 15) & ~(size_t)15);
+    return bytes > MWB_STAGE_QUAD_BYTES_HOST ? 0 : bytes;
+  };
+  if (!h->level_mazes) {
+    h->tri_cap = 2 * (h->cfg.max_quads + 6 * E) + 2;   // + the top view's agent marker
+    h->smem_recs = h->tri_cap <= MWB_SMEM_TRI_CAP ? h->tri_cap : 0;
+    h->stage_bytes = stage_of(h->cfg.max_quads);
+    for (LevelDev& D : h->levels) {
+      D.tri_cap = h->tri_cap;
+      D.tris_hbm = h->smem_recs == 0;
+    }
+    return;
+  }
+  h->tri_cap = h->smem_recs = h->stage_bytes = 0;
+  for (size_t l = 0; l < h->levels.size(); ++l) {
+    LevelDev& D = h->levels[l];
+    D.tri_cap = 2 * (h->level_quads[l] + 6 * E) + 2;
+    D.tris_hbm = D.tri_cap > MWB_SMEM_TRI_CAP;
+    h->tri_cap = std::max(h->tri_cap, (int)D.tri_cap);
+    if (!D.tris_hbm) h->smem_recs = std::max(h->smem_recs, (int)D.tri_cap);
+    h->stage_bytes = std::max(h->stage_bytes, stage_of(h->level_quads[l]));
+  }
+}
+
+// HBM triangle lists for every env (level changes can move any env into a level that needs them)
+static int ensure_room_tris(mwb_handle* h) {
+  bool any = false;
+  for (const LevelDev& D : h->levels) any = any || D.tris_hbm;
+  const size_t recs = (size_t)h->S.N * h->k2_parts * h->tri_cap;
+  if (!any || recs <= h->room_tris_recs) return MWB_OK;
+  auto it = std::find(h->allocs.begin(), h->allocs.end(), (void*)h->S.room_tris);
+  if (h->S.room_tris && it != h->allocs.end()) {
+    dev_free(h->S.room_tris);
+    h->allocs.erase(it);
+  }
+  h->S.room_tris = nullptr;
+  h->room_tris_recs = 0;
+  TriRec* buf = nullptr;
+  if (alloc_arr(h, &buf, recs)) return fail(MWB_ECUDA, "triangle list allocation failed");
+  h->S.room_tris = buf;
+  h->room_tris_recs = recs;
+  return MWB_OK;
+}
+
+// MWB_DEBUG=1: K2's launch shape (and, for a table with Maze levels, where each level's triangle lists live)
+static void k2_report(mwb_handle* h) {
+#ifndef MWB_HOSTSIM
+  if (!getenv("MWB_DEBUG")) return;
+  int nb = 0;
+  const int launch_smem = k2_smem_bytes(h);
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k2_kernels[k2_index(h)], k2_threads(h), launch_smem);
+  std::string levels;
+  if (h->level_mazes) {
+    levels = ", shared-memory records " + std::to_string(h->smem_recs) + ", HBM lists: levels";
+    bool none = true;
+    for (size_t l = 0; l < h->levels.size(); ++l)
+      if (h->levels[l].tris_hbm) {
+        levels += " " + std::to_string(l);
+        none = false;
+      }
+    if (none) levels += " none";
+  }
+  fprintf(stderr, "[mwb] K2 %d threads, %dx MSAA: dynamic smem %d B (local destination), parts %d, resident blocks/SM %d%s\n",
+          k2_threads(h), h->S.msaa, launch_smem, h->k2_parts, nb, levels.c_str());
+#else
+  (void)h;
+#endif
+}
+
 // ------------------------------------------------------------------ ABI: lifetime
 extern "C" const char* mwb_last_error(void) { return g_err.c_str(); }
+static int upload_levels(mwb_handle* h);
 
 extern "C" int mwb_create(const mwb_config* cfg, mwb_handle** out) {
   if (!cfg || !out) return fail(MWB_EINVAL, "null argument");
@@ -595,6 +674,8 @@ extern "C" int mwb_create(const mwb_config* cfg, mwb_handle** out) {
   h->frames_copied = false;
   h->have_params = h->have_protos = h->have_template = false;
   h->have_level_table = false;
+  h->level_mazes = false;
+  h->room_tris_recs = 0;
 #ifndef MWB_HOSTSIM
   h->atlas = nullptr;
 #endif
@@ -634,7 +715,7 @@ extern "C" int mwb_create(const mwb_config* cfg, mwb_handle** out) {
   S.R = cfg->max_rooms;
   S.Q = (cfg->max_quads + 1) & ~1;   // even: per-env quad blocks stay 16-byte aligned (TMA source)
   S.S = cfg->max_segs;
-  S.shared_geom = cfg->shared_geometry;
+  S.env_geom = 0;
   S.obs_w = cfg->obs_width;
   S.obs_h = cfg->obs_height;
   S.msaa = cfg->msaa_samples;
@@ -646,6 +727,8 @@ extern "C" int mwb_create(const mwb_config* cfg, mwb_handle** out) {
     L0.rule_kind = cfg->rule_kind;
     L0.rule_arg = cfg->rule_arg;
     L0.max_episode_steps = cfg->max_episode_steps;
+    L0.maze = -1;
+    L0.env_worlds = cfg->shared_geometry ? 0 : 1;   // shared_geometry = 0: one world per env, no template
     h->levels.assign(1, L0);
     h->env_level.assign(N, 0);
     S.num_levels = 1;
@@ -722,20 +805,11 @@ extern "C" int mwb_create(const mwb_config* cfg, mwb_handle** out) {
     if (h->k2_parts > maxp) h->k2_parts = maxp;
     if (h->k2_parts < 1) h->k2_parts = 1;
   }
-  h->tri_cap = 2 * (cfg->max_quads + 6 * cfg->max_ents) + 2;   // + the top view's agent marker
-  h->smem_tris = h->tri_cap <= 512;
-  if (!h->smem_tris) {
-    TriRec* buf = nullptr;
-    if (alloc_arr(h, &buf, (size_t)N * h->k2_parts * h->tri_cap)) {
-      mwb_destroy(h);
-      return fail(MWB_ECUDA, "triangle list allocation failed");
-    }
-    S.room_tris = buf;
+  plan_k2(h);
+  if (ensure_room_tris(h) || upload_levels(h)) {
+    mwb_destroy(h);
+    return MWB_ECUDA;
   }
-  // static quads are staged in shared memory (TMA bulk copy) when they fit in 16 KB; the
-  // quad capacity is kept even so that every env's block starts 16-byte aligned
-  h->stage_bytes = (int)(((size_t)cfg->max_quads * sizeof(mwb_quad) + 15) & ~(size_t)15);
-  if (h->stage_bytes > MWB_STAGE_QUAD_BYTES_HOST) h->stage_bytes = 0;
 #ifndef MWB_HOSTSIM
   {
     cudaFuncAttributes fa;
@@ -751,13 +825,7 @@ extern "C" int mwb_create(const mwb_config* cfg, mwb_handle** out) {
     mwb_destroy(h);
     return fail(MWB_ECUDA, "cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed");
   }
-  if (getenv("MWB_DEBUG")) {
-    int nb = 0;
-    const int launch_smem = k2_smem_bytes(h);
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k2_kernels[k2_index(h)], k2_threads(h), launch_smem);
-    fprintf(stderr, "[mwb] K2 %d threads, %dx MSAA: dynamic smem %d B (local destination), parts %d, resident blocks/SM %d\n",
-            k2_threads(h), h->S.msaa, launch_smem, h->k2_parts, nb);
-  }
+  k2_report(h);
 #endif
   *out = h;
   return MWB_OK;
@@ -1030,6 +1098,7 @@ static int drain(mwb_handle* h) {
 static int upload_levels(mwb_handle* h) {
   int rc = drain(h);
   if (rc) return rc;
+  plan_k2(h);
   rc |= h2d((void*)h->S.levels, h->levels.data(), h->levels.size() * sizeof(LevelDev), h->stream);
   if (!h->S.next_level)
     rc |= h2d((void*)h->S.env_level, h->env_level.data(), h->env_level.size() * sizeof(int32_t), h->stream);
@@ -1116,7 +1185,7 @@ static int upload_geometry(mwb_handle* h, size_t g, const mwb_geometry* geo) {
 
 extern "C" int mwb_set_template(mwb_handle* h, const mwb_geometry* g) {
   if (!h || !g) return fail(MWB_EINVAL, "null argument");
-  if (!h->S.shared_geom) return fail(MWB_ESTATE, "handle was created with shared_geometry = 0");
+  if (!h->cfg.shared_geometry) return fail(MWB_ESTATE, "handle was created with shared_geometry = 0");
   int rc = upload_geometry(h, 0, g);
   if (!rc) h->have_template = true;
   return rc;
@@ -1168,8 +1237,9 @@ static int grow_geometry(mwb_handle* h, int G) {
 extern "C" int mwb_set_levels(mwb_handle* h, int n_levels, const mwb_level* levels, const mwb_geometry* templates,
                               const mwb_op* ops, int n_ops, const int32_t* env_level) {
   if (!h || !levels || !templates || !ops || !env_level) return fail(MWB_EINVAL, "null argument");
-  if (!h->S.shared_geom) return fail(MWB_EINVAL, "a level table needs shared_geometry = 1 (per-env worlds have no templates)");
+  if (!h->cfg.shared_geometry) return fail(MWB_EINVAL, "a level table needs shared_geometry = 1 (per-env worlds have no templates)");
   if (h->S.next_level) return fail(MWB_ESTATE, "the level table is fixed once level changes are on");
+  if (h->level_mazes) return fail(MWB_ESTATE, "the level table is fixed once it has Maze levels (mwb_set_level_maze)");
   if (n_levels <= 0) return fail(MWB_EINVAL, "n_levels must be positive");
   if (n_levels > MWB_LEVEL_CAP) return fail(MWB_ECAPACITY, "more than MWB_LEVEL_CAP levels");
   if (n_ops <= 0) return fail(MWB_EINVAL, "empty op array");
@@ -1203,7 +1273,10 @@ extern "C" int mwb_set_levels(mwb_handle* h, int n_levels, const mwb_level* leve
     D.max_episode_steps = levels[l].max_episode_steps;
     D.op_first = levels[l].op_first;
     D.num_ops = levels[l].num_ops;
+    D.maze = -1;
   }
+  h->level_quads.resize(n_levels);
+  for (int l = 0; l < n_levels; ++l) h->level_quads[l] = templates[l].num_quads;
   h->env_level.assign(env_level, env_level + S.N);
   h->ops_h.assign(ops, ops + n_ops);
   rc = upload_ops(h);
@@ -1249,12 +1322,9 @@ static int current_level(mwb_handle* h, int env, int32_t* out) {
   return rc ? fail(MWB_ECUDA, "readback failed") : MWB_OK;
 }
 
-extern "C" int mwb_set_maze(mwb_handle* h, const mwb_maze_desc* mz) {
-  if (!h || !mz || !mz->cdf) return fail(MWB_EINVAL, "null argument");
-  if (h->S.shared_geom) return fail(MWB_ESTATE, "Maze needs per-env geometry (shared_geometry = 0)");
+// Level `level`'s Maze templates and room cdf -> S.maze[level] / S.maze_cdf[level] (the caller checked the sizes)
+static int put_maze(mwb_handle* h, int level, const mwb_maze_desc* mz) {
   const int cells = mz->rows * mz->cols;
-  if (cells <= 0 || cells > MWB_MAZE_MAX_CELLS) return fail(MWB_ECAPACITY, "maze too large");
-  if (2 * cells - 1 > h->S.R) return fail(MWB_ECAPACITY, "max_rooms too small for this maze");
   MazeDev m;
   memset(&m, 0, sizeof(m));
   m.rows = mz->rows;
@@ -1268,20 +1338,97 @@ extern "C" int mwb_set_maze(mwb_handle* h, const mwb_maze_desc* mz) {
   memcpy(m.conn_room, mz->conn_room, sizeof(m.conn_room));
   memcpy(m.conn_quads, mz->conn_quads, sizeof(m.conn_quads));
   memcpy(m.conn_segs, mz->conn_segs, sizeof(m.conn_segs));
-  int rc = replace_buf(&h->maze, &m, sizeof(m), h->stream);
-  if (!rc) rc = replace_buf(&h->maze_cdf, mz->cdf, (size_t)(2 * cells - 1) * sizeof(double), h->stream);
+  const size_t L = h->levels.size();
+  h->mazes_h.resize(L);
+  h->maze_cdf_h.resize(L * MWB_MAZE_CDF_STRIDE, 0.0);
+  h->mazes_h[level] = m;
+  std::copy(mz->cdf, mz->cdf + (2 * cells - 1), h->maze_cdf_h.begin() + (size_t)level * MWB_MAZE_CDF_STRIDE);
+  int rc = drain(h);
+  if (!rc) rc = replace_buf(&h->maze, h->mazes_h.data(), L * sizeof(MazeDev), h->stream);
+  if (!rc) rc = replace_buf(&h->maze_cdf, h->maze_cdf_h.data(), h->maze_cdf_h.size() * sizeof(double), h->stream);
   if (rc) return rc;
   h->S.maze = (const MazeDev*)h->maze;
   h->S.maze_cdf = (const double*)h->maze_cdf;
+  h->levels[level].maze = level;
+  return upload_levels(h);
+}
+
+extern "C" int mwb_set_maze(mwb_handle* h, const mwb_maze_desc* mz) {
+  if (!h || !mz || !mz->cdf) return fail(MWB_EINVAL, "null argument");
+  if (h->cfg.shared_geometry) return fail(MWB_ESTATE, "Maze needs per-env geometry (shared_geometry = 0)");
+  const int cells = mz->rows * mz->cols;
+  if (cells <= 0 || cells > MWB_MAZE_MAX_CELLS) return fail(MWB_ECAPACITY, "maze too large");
+  if (2 * cells - 1 > h->S.R) return fail(MWB_ECAPACITY, "max_rooms too small for this maze");
+  return put_maze(h, 0, mz);
+}
+
+// Geometry blocks [L, L + N) of a level table: one world per env, after the L templates (kept)
+static int add_env_worlds(mwb_handle* h) {
+  DevState& S = h->S;
+  const int L = (int)h->levels.size();
+  if (h->geom_blocks < L + S.N) {
+    std::vector<int32_t> nr(L), nq(L), ns(L);
+    std::vector<mwb_room> rooms((size_t)L * S.R);
+    std::vector<mwb_quad> quads((size_t)L * S.Q);
+    std::vector<mwb_seg> segs((size_t)L * S.S);
+    int rc = stream_enter(h, h->stream);
+    rc |= d2h(nr.data(), S.num_rooms, L * sizeof(int32_t), h->stream);
+    rc |= d2h(nq.data(), S.num_quads, L * sizeof(int32_t), h->stream);
+    rc |= d2h(ns.data(), S.num_segs, L * sizeof(int32_t), h->stream);
+    rc |= d2h(rooms.data(), S.rooms, rooms.size() * sizeof(mwb_room), h->stream);
+    rc |= d2h(quads.data(), S.quads, quads.size() * sizeof(mwb_quad), h->stream);
+    rc |= d2h(segs.data(), S.segs, segs.size() * sizeof(mwb_seg), h->stream);
+    rc |= sync_stream(h->stream);
+    if (rc) return fail(MWB_ECUDA, "template readback failed");
+    if ((rc = grow_geometry(h, L + S.N)) != 0) return rc;
+    rc |= h2d(S.num_rooms, nr.data(), L * sizeof(int32_t), h->stream);
+    rc |= h2d(S.num_quads, nq.data(), L * sizeof(int32_t), h->stream);
+    rc |= h2d(S.num_segs, ns.data(), L * sizeof(int32_t), h->stream);
+    rc |= h2d(S.rooms, rooms.data(), rooms.size() * sizeof(mwb_room), h->stream);
+    rc |= h2d(S.quads, quads.data(), quads.size() * sizeof(mwb_quad), h->stream);
+    rc |= h2d(S.segs, segs.data(), segs.size() * sizeof(mwb_seg), h->stream);
+    rc |= sync_stream(h->stream);
+    if (rc) return fail(MWB_ECUDA, "template upload failed");
+  }
+  S.env_geom = L;
+  h->level_mazes = true;
+  return MWB_OK;
+}
+
+extern "C" int mwb_set_level_maze(mwb_handle* h, int level, const mwb_maze_desc* mz) {
+  if (!h || !mz || !mz->cdf) return fail(MWB_EINVAL, "null argument");
+  if (!h->cfg.shared_geometry || !h->have_level_table)
+    return fail(MWB_ESTATE, "Maze levels in a table need a shared_geometry = 1 handle and mwb_set_levels first");
+  if (level < 0 || level >= (int)h->levels.size()) return fail(MWB_EINVAL, "level out of range");
+  const int cells = mz->rows * mz->cols;
+  if (cells <= 0 || cells > MWB_MAZE_MAX_CELLS) return fail(MWB_ECAPACITY, "maze too large");
+  // a maze of c cells is a spanning tree: 2c - 1 rooms, 8c - 2 quads and 4c segments, whatever the episode draws
+  if (2 * cells - 1 > h->S.R) return fail(MWB_ECAPACITY, "max_rooms too small for this maze");
+  if (8 * cells - 2 > h->cfg.max_quads) return fail(MWB_ECAPACITY, "max_quads too small for this maze");
+  if (4 * cells > h->S.S) return fail(MWB_ECAPACITY, "max_segs too small for this maze");
+  int rc = h->level_mazes ? MWB_OK : add_env_worlds(h);
+  if (rc) return rc;
+  h->levels[level].env_worlds = 1;
+  h->level_quads[level] = 8 * cells - 2;
+  plan_k2(h);
+  if ((rc = ensure_room_tris(h)) != 0 || (rc = put_maze(h, level, mz)) != 0) return rc;
+  k2_report(h);
+  return MWB_OK;
+}
+
+// geometry block env `env` reads (geom_index in state.h), from the host's view of its level
+static int env_geom_block(mwb_handle* h, int env, size_t* g) {
+  int32_t lvl = 0;
+  if (current_level(h, env, &lvl) != MWB_OK) return MWB_ECUDA;
+  *g = h->levels[lvl].env_worlds ? (size_t)h->S.env_geom + env : (size_t)lvl;
   return MWB_OK;
 }
 
 extern "C" int mwb_get_geometry(mwb_handle* h, int env, int32_t counts[3], mwb_room* rooms, mwb_quad* quads, mwb_seg* segs) {
   if (!h || !counts) return fail(MWB_EINVAL, "null argument");
   if (env < 0 || env >= h->S.N) return fail(MWB_EINVAL, "env out of range");
-  int32_t lvl = 0;
-  if (h->S.shared_geom && current_level(h, env, &lvl) != MWB_OK) return MWB_ECUDA;
-  const size_t g = h->S.shared_geom ? (size_t)lvl : (size_t)env;
+  size_t g = 0;
+  if (env_geom_block(h, env, &g) != MWB_OK) return MWB_ECUDA;
   int rc = 0;
   rc |= stream_enter(h, h->stream);
   rc |= d2h(&counts[0], h->S.num_rooms + g, sizeof(int32_t), h->stream);
@@ -1340,7 +1487,7 @@ extern "C" int mwb_seed(mwb_handle* h, const int32_t* env_ids, int n, const mwb_
 extern "C" int mwb_reset(mwb_handle* h, const int32_t* env_ids, int n, void* stream) {
   if (!h) return fail(MWB_EINVAL, "null handle");
   if (!h->have_params || !h->have_protos || !h->S.ops) return fail(MWB_ESTATE, "params / protos / program not set");
-  if (h->S.shared_geom && !h->have_template) return fail(MWB_ESTATE, "template not set");
+  if (h->cfg.shared_geometry && !h->have_template) return fail(MWB_ESTATE, "template not set");
   stream_t s = stream ? (stream_t)stream : h->stream;
   if (!env_ids) n = h->S.N;
   if (n <= 0 || n > h->S.N) return fail(MWB_EINVAL, "bad count");
@@ -1381,8 +1528,10 @@ extern "C" int mwb_set_world(mwb_handle* h, const int32_t* env_ids, int n, const
     u.env = env_ids ? env_ids[t] : t;
     if (u.env < 0 || u.env >= h->S.N) return fail(MWB_EINVAL, "env id out of range");
     if (w.num_slots > h->S.E || w.num_slots > MWB_MAX_ENTS_CAP) return fail(MWB_ECAPACITY, "too many entities");
-    if (!h->S.shared_geom) {
-      int rc = upload_geometry(h, (size_t)u.env, &w.geom);
+    if (!h->cfg.shared_geometry || h->level_mazes) {     // an env that runs a level with per-env worlds: its own block
+      int32_t lvl = 0;
+      int rc = current_level(h, u.env, &lvl);
+      if (!rc && h->levels[lvl].env_worlds) rc = upload_geometry(h, (size_t)h->S.env_geom + u.env, &w.geom);
       if (rc) return rc;
     }
     u.num_slots = w.num_slots;
@@ -1589,7 +1738,7 @@ static int launch_k2(mwb_handle* h, uint8_t* obs, float* depth, int env0, int co
   }
   h->obs_is_peer = h->obs_peer_hint >= 0 ? h->obs_peer_hint != 0 : h->peer_result;
   const int smem = k2_smem_bytes(h), fstage = k2_frame_stage_bytes(h);
-  const K2Layout lay = k2_layout(h->smem_tris, h->tri_cap, h->stage_bytes, k2_halves_per_part(h->S.obs_w, h->S.obs_h, h->k2_parts), fstage);
+  const K2Layout lay = k2_layout(h->smem_recs, h->tri_cap, h->stage_bytes, k2_halves_per_part(h->S.obs_w, h->S.obs_h, h->k2_parts), fstage);
   if (ensure_k2_smem(h, smem)) return fail(MWB_ECUDA, "cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed");
   prof_mark(h, h->ev_k2, s);
   k2_kernels[k2_index(h)]<<<count * h->k2_parts, k2_threads(h), smem, s>>>(h->S, h->A, h->view, h->obs_format, obs, depth, env0,
@@ -1839,9 +1988,23 @@ extern "C" int mwb_visible_ents(mwb_handle* h, uint32_t* mask, void* stream) {
 // ------------------------------------------------------------------ ABI: snapshot / restore
 // Every array that changes while episodes run (entity lists, counters, camera / lighting parameters, RNG
 // streams, pending-reset flags) plus the geometry currently on the device, in one fixed order.
-// the magic names the blob's mode: a handle with level changes on writes (and needs) the level-change section
+// the magic names the blob's mode: a handle with level changes on writes (and needs) the level-change section, and a
+// level table with Maze levels carries the per-env worlds after the templates
 static const uint32_t kSnapMagic = 0x5342574du;               // "MWBS"
 static const uint32_t kSnapMagicLevelChanges = 0x4c42574du;   // "MWBL"
+static const uint32_t kSnapMagicWorlds = 0x5742574du;         // "MWBW": level table with per-env worlds
+static const uint32_t kSnapMagicWorldsLevelChanges = 0x5842574du;   // "MWBX": ... and level changes on
+
+static uint32_t snapshot_magic(const mwb_handle* h) {
+  if (h->level_mazes) return h->S.next_level ? kSnapMagicWorldsLevelChanges : kSnapMagicWorlds;
+  return h->S.next_level ? kSnapMagicLevelChanges : kSnapMagic;
+}
+static const char* snapshot_mode(uint32_t magic) {
+  return magic == kSnapMagic ? "level changes off, no per-env worlds"
+         : magic == kSnapMagicLevelChanges ? "level changes on, no per-env worlds"
+         : magic == kSnapMagicWorlds ? "level changes off, per-env worlds"
+                                     : "level changes on, per-env worlds";
+}
 
 struct SnapHeader {
   uint32_t magic, abi;
@@ -1849,8 +2012,10 @@ struct SnapHeader {
   uint64_t bytes;
 };
 
-// geometry blocks a snapshot carries: one template per level, or one world per env
-static size_t snapshot_blocks(const mwb_handle* h) { return h->S.shared_geom ? h->levels.size() : (size_t)h->S.N; }
+// geometry blocks a snapshot carries: one template per level, then one world per env if some level has them
+static size_t snapshot_blocks(const mwb_handle* h) {
+  return h->cfg.shared_geometry && !h->level_mazes ? h->levels.size() : (size_t)h->S.env_geom + h->S.N;
+}
 
 // the level-change section of a snapshot: next_level [N], level_draws [N], level_weights [L], then this
 struct LevelChangeTail {
@@ -1887,7 +2052,7 @@ static SnapHeader snapshot_header(mwb_handle* h) {
   std::vector<std::pair<void*, size_t>> v;
   snapshot_arrays(h, v);
   SnapHeader hd;
-  hd.magic = h->S.next_level ? kSnapMagicLevelChanges : kSnapMagic;
+  hd.magic = snapshot_magic(h);
   hd.abi = MWB_ABI_VERSION;
   hd.N = h->S.N; hd.E = h->S.E; hd.R = h->S.R; hd.Q = h->S.Q; hd.S = h->S.S;
   hd.G = (int32_t)snapshot_blocks(h);
@@ -1944,17 +2109,19 @@ extern "C" int mwb_restore(mwb_handle* h, const void* blob, size_t bytes) {
   SnapHeader hd;
   if (bytes < sizeof(hd)) return fail(MWB_EINVAL, "not a snapshot");
   memcpy(&hd, blob, sizeof(hd));
-  if ((hd.magic != kSnapMagic && hd.magic != kSnapMagicLevelChanges) || hd.abi != want.abi)
+  if ((hd.magic != kSnapMagic && hd.magic != kSnapMagicLevelChanges && hd.magic != kSnapMagicWorlds &&
+       hd.magic != kSnapMagicWorldsLevelChanges) || hd.abi != want.abi)
     return fail(MWB_EABI, "snapshot from another ABI version");
   const bool dynamic = h->S.next_level != nullptr;
   if (hd.magic != want.magic)
-    return fail(MWB_ESTATE, dynamic ? "snapshot of a handle without level changes (this one has them on)"
-                                    : "snapshot of a handle with level changes on (this one has them off)");
+    return fail(MWB_ESTATE, std::string("snapshot of a handle with ") + snapshot_mode(hd.magic) + " (this one has " +
+                                snapshot_mode(want.magic) + ")");
   if (hd.N != want.N || hd.E != want.E || hd.R != want.R || hd.Q != want.Q || hd.S != want.S)
     return fail(MWB_EINVAL, "snapshot does not match this handle's configuration");
+  const bool shared = h->cfg.shared_geometry != 0;
   if (hd.G != want.G || hd.bytes != want.bytes)
-    return fail(h->S.shared_geom ? MWB_ESTATE : MWB_EINVAL, h->S.shared_geom ? "snapshot of a handle with another number of levels"
-                                                                            : "snapshot does not match this handle's configuration");
+    return fail(shared ? MWB_ESTATE : MWB_EINVAL, shared ? "snapshot of a handle with another number of levels"
+                                                         : "snapshot does not match this handle's configuration");
   if (bytes < hd.bytes) return fail(MWB_EINVAL, "snapshot truncated");
   std::vector<std::pair<void*, size_t>> v;
   snapshot_arrays(h, v);

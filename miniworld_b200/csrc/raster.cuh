@@ -42,9 +42,10 @@ static inline
 #ifdef __CUDACC__
 __host__ __device__
 #endif
-K2Layout k2_layout(bool smem_tris, int tri_cap, int stage_bytes, int halves_per_part, int frame_stage_bytes) {
+// smem_recs: triangle records of the levels whose lists live in shared memory; tri_cap: the largest level's capacity
+K2Layout k2_layout(int smem_recs, int tri_cap, int stage_bytes, int halves_per_part, int frame_stage_bytes) {
   K2Layout L;
-  const int tri_bytes = smem_tris ? tri_cap * (int)sizeof(TriRec) : 0;
+  const int tri_bytes = smem_recs * (int)sizeof(TriRec);
   const int cap2 = (tri_cap + 1) & ~1;
   L.order_off = tri_bytes;
   L.zkey_off = L.order_off + cap2 * 2;
@@ -293,9 +294,12 @@ render_kernel(DevState S, RenderAssets A, ViewSpec view, int fmt, uint8_t* __res
   // large frames are cut into `parts` blocks per env (each redoes the cheap geometry phase and
   // rasterises its share of the half-tiles), which evens out the load when few envs are resident
   const int i = env0 + (int)blockIdx.x / parts, part = (int)blockIdx.x % parts;
-  // set-up triangles of rooms + boxes: shared memory, or this env's HBM block for big levels
-  const size_t tri_bytes = S.room_tris ? 0 : (size_t)tri_cap * sizeof(TriRec);
-  TriRec* tris = S.room_tris ? S.room_tris + ((size_t)i * parts + part) * tri_cap : reinterpret_cast<TriRec*>(smem_raw);
+  // set-up triangles of rooms + boxes: shared memory, or this env's HBM block for big levels (per level: the
+  // env's own capacity bounds its list; tri_cap, the largest level's, is the stride of the HBM blocks)
+  const LevelDev& lv = env_level_of(S, i);
+  const int own_cap = lv.tri_cap;
+  const size_t tri_bytes = (size_t)lay.order_off;     // the shared-memory records come first
+  TriRec* tris = lv.tris_hbm ? S.room_tris + ((size_t)i * parts + part) * tri_cap : reinterpret_cast<TriRec*>(smem_raw);
   __shared__ Camera cam;
   __shared__ FrameMap fmap;
   __shared__ Segment segs[MWB_MAX_SEGS];
@@ -399,7 +403,7 @@ render_kernel(DevState S, RenderAssets A, ViewSpec view, int fmt, uint8_t* __res
     }
     if (keep) {
       const int pos = ntris + woff + incl - 1;
-      if (pos < tri_cap) {
+      if (pos < own_cap) {
         tris[pos] = rec;
         atomicAdd(&seg_count[seg], 1);
       }
@@ -407,7 +411,7 @@ render_kernel(DevState S, RenderAssets A, ViewSpec view, int fmt, uint8_t* __res
     ntris += total;
     __syncthreads();
   }
-  const int n_res = ntris < tri_cap ? ntris : tri_cap;
+  const int n_res = ntris < own_cap ? ntris : own_cap;
   // (while thread 0 fills the segment table, everybody computes the depth keys of the visiting order: neither needs the other)
   for (int t = tid; t < n_res; t += THREADS) {
     const TriRec& T = tris[t];
@@ -416,7 +420,7 @@ render_kernel(DevState S, RenderAssets A, ViewSpec view, int fmt, uint8_t* __res
   }
   if (tid == 0) {
     next_half = h_begin + WARPS;
-    if (ntris > tri_cap) atomicAdd(overflow, 1);
+    if (ntris > own_cap) atomicAdd(overflow, 1);
     // segment table: smem-resident lists are contiguous in draw order; mesh lists live in HBM
     int smem_pos = 0, slot = 0;
     const int last = fmap.n_ents + (fmap.agent_task >= 0 ? 1 : 0);

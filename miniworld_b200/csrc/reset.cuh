@@ -7,8 +7,9 @@
 // GPU lands on the same poses, colours and camera parameters as `env.reset()` in Python.
 // The level's `_gen_world()` is lowered on the host into a short program of
 // CHOICE / UNIFORM / PLACE / PUT / IFEQ ops (miniworld_b200/program.py); room layout comes from the
-// static template of the env's level, and the program is that level's slice of the op array.  Levels whose topology is random per episode (Maze) reset on the
-// host and arrive through mwb_set_world instead.
+// static template of the env's level, and the program is that level's slice of the op array.  Maze levels carve a
+// fresh world into the env's own geometry block (maze.cuh) from their level's templates; Maze variants whose
+// templates do not reproduce the host exactly reset on the host and arrive through mwb_set_world instead.
 #pragma once
 #include "maze.cuh"
 #include "physics.cuh"
@@ -80,7 +81,9 @@ MWB_DEV void device_reset(const DevState& S, int i) {
   const mwb_params& P = L.params;
   const mwb_op* ops = S.ops + L.op_first;
   const int num_ops = L.num_ops;
-  const int g = S.shared_geom ? lvl : i;
+  // the geometry of the level this episode runs: the env's own world (regenerated below by a Maze program) or the
+  // level's template, so that an env leaving a Maze level stops reading its old world
+  const int g = geom_block(S, i, lvl);
   const mwb_room* rooms = S.rooms + (size_t)g * S.R;
   int n_rooms = S.num_rooms[g];
 
@@ -108,7 +111,7 @@ MWB_DEV void device_reset(const DevState& S, int i) {
     const mwb_op& op = ops[pc];
     if (op.op == MWB_OP_END) break;
     if (op.op == MWB_OP_MAZE) {          // per-episode topology: regenerate this env's rooms
-      if (S.maze != nullptr && !S.shared_geom && maze_generate(S, *S.maze, S.maze_cdf, i, rng)) {
+      if (L.maze >= 0 && L.env_worlds && maze_generate(S, S.maze[L.maze], S.maze_cdf + (size_t)L.maze * MWB_MAZE_CDF_STRIDE, g, rng)) {
         n_rooms = S.num_rooms[g];
       } else {
         // out of capacity (unreachable when the host sized the handle from a generated maze, mwb_set_maze): placing

@@ -2,8 +2,9 @@
 //
 // Layout rule: every per-env scalar is an array [N] (env index fastest) so that the
 // one-thread-per-env physics kernel reads and writes fully coalesced; per-entity fields are
-// [max_ents][N].  Static room geometry is either one shared template per level (levels
-// without per-episode topology; env_level picks the block) or [N][capacity] blocks (Maze).  Nothing here is ever
+// [max_ents][N].  Static room geometry is one shared template per level (levels without per-episode
+// topology) followed, when some level is a Maze, by one world block per env; geom_index picks the block
+// from the env's level.  Nothing here is ever
 // re-laid-out between kernels: the physics kernel and the rasteriser read the same arrays.
 #pragma once
 #include "../../include/mwb.h"
@@ -32,12 +33,15 @@ struct LevelDev {
   int32_t rule_kind, rule_arg;
   int32_t max_episode_steps;
   int32_t op_first, num_ops;    // slice of DevState::ops
-  int32_t reserved;
+  int32_t maze;                 // index of the level's Maze templates in DevState::maze / maze_cdf, -1 = none
+  int32_t env_worlds;           // 1: every env of the level has its own world (geometry block env_geom + i)
+  int32_t tri_cap;              // K2: room + box triangle records one frame of the level can keep
+  int32_t tris_hbm;             // K2: 1 = those records live in DevState::room_tris, 0 = in shared memory
 };
 
 struct DevState {
   int32_t N, E, R, Q, S;        // envs, entity slots, room / quad / segment capacity
-  int32_t shared_geom;
+  int32_t env_geom;             // geometry block of env 0's own world (after the level templates)
   int32_t obs_w, obs_h, msaa;
 
   // ---- dynamic per-env state ----
@@ -73,8 +77,9 @@ struct DevState {
   int32_t* rng_has32;
   uint32_t* rng_cache;
 
-  // ---- geometry: [levels][capacity] (shared templates) or [N][capacity] (per-env worlds) ----
-  int32_t* num_rooms;           // [levels or N]
+  // ---- geometry: [env_geom + N][capacity] -- one template per level, then one world per env when some level has
+  //      per-env worlds (shared_geometry = 0 handles: env_geom = 0, worlds only; template-only handles: no worlds) ----
+  int32_t* num_rooms;           // [blocks]
   int32_t* num_quads;
   int32_t* num_segs;
   mwb_room* rooms;
@@ -97,12 +102,12 @@ struct DevState {
   double* cam_trig;             // [6][N]  cos, sin of heading, pitch, half field of view
   float* ent_cs;                // [E][2][N]  cos, sin of the slot's glRotatef angle (the form its prototype's render() uses)
   const float* depth_lut;       // [65536] depth16 code -> metres (depth_code_to_metres of every code), or null
-  TriRec* room_tris;            // [N][tri_cap] room + box triangle lists in HBM for levels whose lists do
-                                //   not fit shared memory (Maze); null = lists live in shared memory
+  TriRec* room_tris;            // [N][parts][tri_cap] room + box triangle lists in HBM for the envs of levels whose
+                                //   lists do not fit shared memory (LevelDev::tris_hbm); null = no such level
 
   // ---- level definition ----
-  const MazeDev* maze;          // Maze templates (mwb_set_maze) or null
-  const double* maze_cdf;
+  const MazeDev* maze;          // [levels] Maze templates (mwb_set_maze, mwb_set_level_maze) or null
+  const double* maze_cdf;       // [levels][MWB_MAZE_CDF_STRIDE] cumulative room probabilities
   const mwb_proto* protos;      // shared by all levels
   int32_t num_protos;
   const mwb_op* ops;            // every level's reset program, one after another
@@ -124,8 +129,9 @@ struct DevState {
   double act_prob;
 };
 
-// Block of the geometry arrays env i reads: its level's template, or its own world
-MWB_DEV int geom_index(const DevState& S, int i) { return S.shared_geom ? S.env_level[i] : i; }
+// Block of the geometry arrays env i reads while it runs level lvl: its own world, or the level's template
+MWB_DEV int geom_block(const DevState& S, int i, int lvl) { return S.levels[lvl].env_worlds ? S.env_geom + i : lvl; }
+MWB_DEV int geom_index(const DevState& S, int i) { return geom_block(S, i, S.env_level[i]); }
 MWB_DEV const LevelDev& env_level_of(const DevState& S, int i) { return S.levels[S.env_level[i]]; }
 
 MWB_DEV NpRng load_rng(const DevState& S, int i) {

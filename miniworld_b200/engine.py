@@ -10,7 +10,7 @@ import os
 
 import numpy as np
 
-ABI_VERSION = 8
+ABI_VERSION = 9
 RULE_NONE, RULE_GOAL, RULE_PICKUP, RULE_SIDEWALK, RULE_SIGN, RULE_HEALTH, RULE_PUTNEXT = 0, 1, 2, 3, 4, 5, 6
 SURF_WALL, SURF_FLOOR, SURF_CEIL = 0, 1, 2
 OP_END, OP_CHOICE, OP_UNIFORM, OP_PLACE, OP_MAZE, OP_IFEQ, OP_PUT = 0, 1, 2, 3, 4, 5, 6
@@ -128,7 +128,7 @@ EXPORTS = (
     "mwb_render_top_view", "mwb_visible_ents", "mwb_set_action_noise",
     "mwb_snapshot_size", "mwb_snapshot", "mwb_restore", "mwb_set_obs_format",
     "mwb_flag_write", "mwb_flag_wait_geq", "mwb_flag_mode", "mwb_state_array", "mwb_debug_camera", "mwb_set_obs_peer",
-    "mwb_set_levels", "mwb_enable_level_changes", "mwb_state_in_host_memory",
+    "mwb_set_levels", "mwb_enable_level_changes", "mwb_state_in_host_memory", "mwb_set_level_maze",
 )
 OBS_FORMATS = {"hwc": 0, "cwh": 1, "grey": 2}
 
@@ -185,6 +185,7 @@ def load_library():
     lib.mwb_launch_count.restype = C.c_int64
     lib.mwb_abi_sizes.argtypes = [i32p, C.c_int]
     lib.mwb_set_maze.argtypes = [vp, C.POINTER(MazeDesc)]
+    lib.mwb_set_level_maze.argtypes = [vp, C.c_int, C.POINTER(MazeDesc)]
     lib.mwb_get_geometry.argtypes = [vp, C.c_int, i32p, vp, vp, vp]
     lib.mwb_shared_alloc.argtypes = [C.c_int, C.c_size_t, C.POINTER(vp), C.c_char_p]
     lib.mwb_shared_open.argtypes = [C.c_int, C.c_char_p, C.POINTER(vp)]
@@ -394,6 +395,15 @@ class Engine:
 
     def set_maze(self, tmpl, cdf):
         """tmpl: maze_lowering.MazeTemplate; cdf: float64[2 rows cols - 1]."""
+        d = self._maze_desc(tmpl, cdf)
+        self._check(self.lib.mwb_set_maze(self.h, C.byref(d)))
+
+    def set_level_maze(self, level, tmpl, cdf):
+        """Level `level` of the table (set_levels) becomes a Maze level with per-env worlds (mwb_set_level_maze)."""
+        d = self._maze_desc(tmpl, cdf)
+        self._check(self.lib.mwb_set_level_maze(self.h, int(level), C.byref(d)))
+
+    def _maze_desc(self, tmpl, cdf):
         d = MazeDesc()
         d.rows, d.cols, d.pitch = tmpl.rows, tmpl.cols, tmpl.pitch
 
@@ -412,7 +422,7 @@ class Engine:
         put(d.conn_segs, np.array([c[2] for c in tmpl.conn], SEG_DTYPE))
         self._maze_cdf = np.ascontiguousarray(cdf, np.float64)
         d.cdf = self._maze_cdf.ctypes.data
-        self._check(self.lib.mwb_set_maze(self.h, C.byref(d)))
+        return d
 
     def get_geometry(self, env):
         counts = (C.c_int32 * 3)()
