@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define MWB_ABI_VERSION 9
+#define MWB_ABI_VERSION 10
 
 /* error codes */
 #define MWB_OK 0
@@ -101,7 +101,7 @@ typedef struct mwb_config {
   int32_t max_rooms, max_quads, max_segs, max_ents;   /* per-env capacities                      */
   int32_t rule_kind;         /* MWB_RULE_*                                                       */
   int32_t rule_arg;          /* GOAL: entity slot of the box; PICKUP: num_objs                   */
-  int32_t domain_rand;       /* MiniWorldEnv(domain_rand=...) (miniworld.py:478)                 */
+  int32_t domain_rand;       /* MiniWorldEnv(domain_rand=...) (miniworld.py:478) of level 0      */
   int32_t max_episode_steps; /* (miniworld.py:472)                                               */
   int32_t autoreset;         /* 1: the step after terminated|truncated resets on the device      */
   int32_t reserved[4];
@@ -276,20 +276,25 @@ int mwb_set_template(mwb_handle* h, const mwb_geometry* g);                /* sh
 int mwb_set_program(mwb_handle* h, const mwb_op* ops, int n);              /* lowered _gen_world  */
 
 /* Several levels in one batch (the reference's vector env built from a list of env constructors, each with its own
- * level id and kwargs).  A handle holds a table of levels; mwb_create's rule fields, mwb_set_params, mwb_set_template
- * and mwb_set_program fill level 0 of it, so a handle that never calls mwb_set_levels runs one level.
+ * level id and kwargs).  A handle holds a table of levels; mwb_create's rule fields and domain_rand, mwb_set_params,
+ * mwb_set_template and mwb_set_program fill level 0 of it, so a handle that never calls mwb_set_levels runs one level.
  * mwb_set_levels replaces the whole table: level l gets templates[l] as its static rooms and the reset program
  * ops[op_first, op_first + num_ops).  env_level[i] names the level of env i; the proto table (mwb_set_protos) is
  * shared, so each level's ops address it with absolute indices.  Only for shared_geometry = 1 handles (MWB_EINVAL
  * otherwise); MWB_ECAPACITY for more than MWB_LEVEL_CAP levels, a program longer than MWB_MAX_OPS or a template
- * above the handle's max_rooms / max_quads / max_segs; MWB_EINVAL for an env_level entry outside [0, n_levels).
- * Per-handle settings (observation size, MSAA, domain_rand, autoreset, action noise) apply to every level. */
+ * above the handle's max_rooms / max_quads / max_segs; MWB_EINVAL for an env_level entry outside [0, n_levels) or a
+ * domain_rand other than 0 or 1.
+ * Each level has its own domain_rand: an env's reset draws (texture variants, sky and light, entity colours, agent
+ * camera) follow the flag of the level it resets into, and its per-step draws the flag of its episode's level, so rows
+ * that share a level definition but differ in the flag (and in their params' ranges) make a randomisation curriculum.
+ * The flag is table data, not env state: snapshots do not carry it.
+ * Per-handle settings (observation size, MSAA, autoreset, action noise) apply to every level. */
 typedef struct mwb_level {
   int32_t rule_kind;         /* MWB_RULE_*                                                       */
   int32_t rule_arg;
   int32_t max_episode_steps;
   int32_t op_first, num_ops; /* this level's slice of the shared op array                        */
-  int32_t reserved;
+  int32_t domain_rand;       /* 0 or 1: MiniWorldEnv(domain_rand=...) of this level              */
   mwb_params params;
 } mwb_level;
 int mwb_set_levels(mwb_handle* h, int n_levels, const mwb_level* levels, const mwb_geometry* templates /*[n_levels]*/,

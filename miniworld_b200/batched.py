@@ -83,6 +83,16 @@ def sample_level(seed, global_env, draw, weights):
     return pick
 
 
+def _definition_kwargs(kwargs, domain_rand):
+    """Keyword arguments of a level's definition instance.  The level's own `domain_rand` wins; without one, the batch's
+    `domain_rand` is the default.  The keyword is passed only when it is on, since Sign takes none (it fixes the flag
+    off itself, like the reference).  The level's flag is then the `domain_rand` that instance ends up with."""
+    kw = dict(kwargs or {})
+    if domain_rand and "domain_rand" not in kw:
+        kw["domain_rand"] = True
+    return kw
+
+
 def default_env_level(num_envs, n_levels):
     """Level of each env when none is given: contiguous, near-equal blocks in the order the levels were listed (the
     first num_envs % n_levels levels get one env more)."""
@@ -93,7 +103,10 @@ def default_env_level(num_envs, n_levels):
 class BatchedMiniWorld:
     """`level`: a level id or class, or a sequence of them to run several levels side by side in one batch (multi-task
     or curriculum training; env i runs level `env_level[i]`).  With a sequence, `level_kwargs` may be a sequence
-    aligned with it, and the observation size, MSAA, domain randomisation, auto-reset and action noise are per batch.
+    aligned with it; the observation size, MSAA, auto-reset and action noise are per batch.
+    Domain randomisation is per level: a level's kwargs may set `domain_rand`, and `domain_rand` here is the default
+    for levels whose kwargs do not.  Rows of one level id that differ in the flag (or in `params` ranges) form a
+    randomisation curriculum: an env's resets draw by the flag of the level it resets into.
     Sign (dict observation) cannot share a batch with other levels.  Maze-family levels can with
     `per_env_worlds=True`: each env then gets a world block of its own, which a reset at a Maze level fills with a
     fresh maze (about 123 KB per env with an 8 x 8 Maze in the table, plus about 204 KB per env of HBM triangle
@@ -147,10 +160,10 @@ class BatchedMiniWorld:
         self.level_kwargs = dict(level_kwargs or {})
 
         # a definition-only instance of the level: layout, params, rule, action space
-        dr = {"domain_rand": True} if self.domain_rand else {}     # (Sign fixes domain_rand itself, like the reference)
-        self.proto_env = self.level_cls(device=None, obs_width=obs_width, obs_height=obs_height, **dr,
-                                        **self.level_kwargs)
+        kw = _definition_kwargs(self.level_kwargs, self.domain_rand)
+        self.proto_env = self.level_cls(device=None, obs_width=obs_width, obs_height=obs_height, **kw)
         pe = self.proto_env
+        self.domain_rand = bool(pe.domain_rand)          # the level's flag decides (level_kwargs may set it)
         self.action_space = pe.action_space                  # per-env space: `step` takes one action per env
         self.single_action_space = pe.action_space           # (gymnasium.vector naming)
         self.single_observation_space = pe.observation_space
@@ -172,7 +185,7 @@ class BatchedMiniWorld:
                 # host-generated worlds exactly; otherwise fall back to host-side resets
                 from .maze_lowering import MazeTemplate
                 try:
-                    tmpl = MazeTemplate(self.level_cls, domain_rand=self.domain_rand, **self.level_kwargs)
+                    tmpl = MazeTemplate(self.level_cls, **kw)
                     tmpl.verify(seeds=(0,))
                     self.maze_template = tmpl
                 except AssertionError:
@@ -239,13 +252,13 @@ class BatchedMiniWorld:
                                                                                      env_level.shape))
         if env_level.size and (env_level.min() < 0 or env_level.max() >= n):
             raise ValueError("env_level entries must lie in [0, %d)" % n)
-        dr = {"domain_rand": True} if self.domain_rand else {}
         classes = [_resolve_level(lv) for lv in levels]
         names = [lv if isinstance(lv, str) else lv.__name__ for lv in levels]
         pes, table, protos, mazes = [], [], [], []
         caps, max_placed = [0, 0, 0], 2
         for name, cls, kw in zip(names, classes, kwargs):
-            pe = cls(device=None, obs_width=self.obs_width, obs_height=self.obs_height, **dr, **kw)
+            kw = _definition_kwargs(kw, self.domain_rand)
+            pe = cls(device=None, obs_width=self.obs_width, obs_height=self.obs_height, **kw)
             rule = getattr(pe, "device_rule", None)
             if rule is None or getattr(pe, "device_program", None) is None:
                 raise ValueError("%s resets on the host only; a batch of several levels needs device reset programs" % name)
@@ -261,7 +274,7 @@ class BatchedMiniWorld:
                 # a table has no host resets: the device templates must reproduce host-generated mazes exactly
                 from .maze_lowering import MazeTemplate
                 try:
-                    maze = MazeTemplate(cls, domain_rand=self.domain_rand, **kw)
+                    maze = MazeTemplate(cls, **kw)
                     maze.verify(seeds=(0,))
                 except AssertionError as e:
                     raise ValueError("%s: its maze templates do not reproduce host-generated worlds, and a level table "
@@ -276,7 +289,7 @@ class BatchedMiniWorld:
             caps = [max(c, len(g) + s) for c, g, s in zip(caps, geom, slack)]
             max_placed = max(max_placed, prog.num_placed)
             table.append(dict(rule=(_RULES[rule[0]], rule[1]), max_episode_steps=int(min(pe.max_episode_steps, 2 ** 31 - 1)),
-                              params=pe.params, geometry=geom, ops=ops))
+                              params=pe.params, geometry=geom, ops=ops, domain_rand=int(bool(pe.domain_rand))))
             pes.append(pe)
         self.level_ids, self.proto_envs, self._env_level = names, pes, env_level.astype(np.int32)
         self.level_cls, self.level_kwargs, self.proto_env = None, kwargs, None
@@ -288,7 +301,7 @@ class BatchedMiniWorld:
         self.autoreset = bool(autoreset)
         self.engine = Engine(self.num_envs, self.obs_width, self.obs_height, msaa_samples, shared_geometry=True,
                              max_rooms=caps[0], max_quads=caps[1], max_segs=caps[2], max_ents=max_placed,
-                             rule=table[0]["rule"], domain_rand=self.domain_rand,
+                             rule=table[0]["rule"], domain_rand=table[0]["domain_rand"],
                              max_episode_steps=table[0]["max_episode_steps"], autoreset=self.autoreset, device=self.device)
         self.engine.sync_assets()
         self.engine.set_protos(np.array(protos, PROTO_DTYPE))

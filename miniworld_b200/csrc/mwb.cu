@@ -243,12 +243,13 @@ MWB_DEV void step_one(const DevState& S, int i, const int32_t* actions, const do
       MWB_WARP_SYNC();
     }
     double fs, fd, ts;
-    const mwb_params& P = env_level_of(S, i).params;
+    const LevelDev& L = env_level_of(S, i);   // the level of this episode: its params and its domain_rand
+    const mwb_params& P = L.params;
     if (step_params) {
       fs = step_params[i * 3 + 0];
       fd = step_params[i * 3 + 1];
       ts = step_params[i * 3 + 2];
-    } else if (S.domain_rand) {   // params.sample(rand, ...) x3, always, before the action is read
+    } else if (L.domain_rand) {   // params.sample(rand, ...) x3, always, before the action is read
       NpRng r = load_rng(S, i);
       fs = rng_uniform(r, P.forward_step_lo, P.forward_step_rng);
       fd = rng_uniform(r, P.forward_drift_lo, P.forward_drift_rng);
@@ -719,7 +720,6 @@ extern "C" int mwb_create(const mwb_config* cfg, mwb_handle** out) {
   S.obs_w = cfg->obs_width;
   S.obs_h = cfg->obs_height;
   S.msaa = cfg->msaa_samples;
-  S.domain_rand = cfg->domain_rand;
   S.autoreset = cfg->autoreset;
   {
     LevelDev L0;
@@ -727,6 +727,7 @@ extern "C" int mwb_create(const mwb_config* cfg, mwb_handle** out) {
     L0.rule_kind = cfg->rule_kind;
     L0.rule_arg = cfg->rule_arg;
     L0.max_episode_steps = cfg->max_episode_steps;
+    L0.domain_rand = cfg->domain_rand;
     L0.maze = -1;
     L0.env_worlds = cfg->shared_geometry ? 0 : 1;   // shared_geometry = 0: one world per env, no template
     h->levels.assign(1, L0);
@@ -1249,6 +1250,9 @@ extern "C" int mwb_set_levels(mwb_handle* h, int n_levels, const mwb_level* leve
     if (L.num_ops > MWB_MAX_OPS) return fail(MWB_ECAPACITY, "level " + std::to_string(l) + ": program longer than MWB_MAX_OPS");
     if (L.num_ops <= 0 || L.op_first < 0 || L.op_first + L.num_ops > n_ops)
       return fail(MWB_EINVAL, "level " + std::to_string(l) + ": program slice outside the op array");
+    if (L.domain_rand != 0 && L.domain_rand != 1)
+      return fail(MWB_EINVAL, "level " + std::to_string(l) + ": domain_rand must be 0 or 1, got " +
+                                  std::to_string(L.domain_rand));
     const mwb_geometry& g = templates[l];
     if (g.num_rooms < 0 || g.num_quads < 0 || g.num_segs < 0 || g.num_rooms > S.R || g.num_quads > h->cfg.max_quads ||
         g.num_segs > S.S)
@@ -1273,6 +1277,7 @@ extern "C" int mwb_set_levels(mwb_handle* h, int n_levels, const mwb_level* leve
     D.max_episode_steps = levels[l].max_episode_steps;
     D.op_first = levels[l].op_first;
     D.num_ops = levels[l].num_ops;
+    D.domain_rand = levels[l].domain_rand;
     D.maze = -1;
   }
   h->level_quads.resize(n_levels);

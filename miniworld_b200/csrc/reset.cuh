@@ -15,12 +15,13 @@
 #include "physics.cuh"
 
 // the first place_entity triggers _gen_static_data: per room Texture.get(wall / floor / ceil), each one
-// rng.integers(0, n_variants) under domain randomisation (opengl.py:113-145)
-MWB_DEV void draw_room_textures(const DevState& S, int i, const mwb_room* rooms, int n_rooms, NpRng& rng) {
+// rng.integers(0, n_variants) under domain randomisation of the env's level (opengl.py:113-145)
+MWB_DEV void draw_room_textures(const DevState& S, int i, const mwb_room* rooms, int n_rooms, bool domain_rand,
+                                NpRng& rng) {
   for (int r = 0; r < n_rooms; ++r)
     for (int k = 0; k < 3; ++k) {
       int v = 0;
-      if (S.domain_rand) v = (int)rng_integers(rng, (uint32_t)rooms[r].tex_count[k]);
+      if (domain_rand) v = (int)rng_integers(rng, (uint32_t)rooms[r].tex_count[k]);
       S.room_tex[((size_t)i * S.R + r) * 3 + k] = rooms[r].tex_first[k] + v;
     }
 }
@@ -77,6 +78,8 @@ MWB_DEV void device_reset(const DevState& S, int i) {
   const size_t N = S.N;
   NpRng rng = load_rng(S, i);
   const int lvl = S.next_level ? resolve_level(S, i) : S.env_level[i];
+  // the resolved level decides everything below, its domain_rand included: a reset that switches levels draws by the
+  // new level's flag (read at each use: the row's address is live anyway, a cached copy would cost step_kernel a spill)
   const LevelDev& L = S.levels[lvl];
   const mwb_params& P = L.params;
   const mwb_op* ops = S.ops + L.op_first;
@@ -132,7 +135,7 @@ MWB_DEV void device_reset(const DevState& S, int i) {
     }
     if (op.op == MWB_OP_PUT) {
       if (!static_done && op.b == 0) {
-        draw_room_textures(S, i, rooms, n_rooms, rng);
+        draw_room_textures(S, i, rooms, n_rooms, L.domain_rand != 0, rng);
         static_done = true;
       }
       const mwb_proto& pr = S.protos[op.a];
@@ -155,7 +158,7 @@ MWB_DEV void device_reset(const DevState& S, int i) {
       freg[op.a & 7] = rng_uniform(rng, op.f[0], d_sub(op.f[1], op.f[0]));
     } else if (op.op == MWB_OP_PLACE) {
       if (!static_done) {
-        draw_room_textures(S, i, rooms, n_rooms, rng);
+        draw_room_textures(S, i, rooms, n_rooms, L.domain_rand != 0, rng);
         static_done = true;
       }
       int proto = op.a;
@@ -188,10 +191,10 @@ MWB_DEV void device_reset(const DevState& S, int i) {
   const double* rngs[4] = {P.sky_color_rng, P.light_pos_rng, P.light_color_rng, P.light_ambient_rng};
   for (int q = 0; q < 4; ++q)
     for (int k = 0; k < 3; ++k)
-      S.envp[(size_t)(q * 3 + k) * N + i] = S.domain_rand ? rng_uniform(rng, los[q][k], rngs[q][k]) : defs[q][k];
+      S.envp[(size_t)(q * 3 + k) * N + i] = L.domain_rand ? rng_uniform(rng, los[q][k], rngs[q][k]) : defs[q][k];
 
   // for ent in self.entities: ent.randomize(params, rand)
-  if (S.domain_rand) {
+  if (L.domain_rand) {
     for (int e = 0; e < slots; ++e) {
       const mwb_proto& pr = S.protos[S.ent_proto[e * N + i]];
       if (pr.kind == MWB_KIND_BOX) {

@@ -37,6 +37,7 @@ struct LevelDev {
   int32_t env_worlds;           // 1: every env of the level has its own world (geometry block env_geom + i)
   int32_t tri_cap;              // K2: room + box triangle records one frame of the level can keep
   int32_t tris_hbm;             // K2: 1 = those records live in DevState::room_tris, 0 = in shared memory
+  int32_t domain_rand;          // MiniWorldEnv(domain_rand=...) of the level: per-step and reset draws of its envs
 };
 
 struct DevState {
@@ -121,7 +122,6 @@ struct DevState {
   const float* level_weights;   // [num_levels] sampling weights, all <= 0 = keep the level
   uint64_t level_seed;
   int32_t level_env_offset;     // global index of env 0 (sharded runs)
-  int32_t domain_rand;
   int32_t autoreset;
   // StochasticActionWrapper on the device (reference wrappers.py:49-71): per step one uniform() draw from
   // the env's own stream; below act_prob the chosen action stands, else act_random (< 0: integers(0, 6))

@@ -10,7 +10,7 @@ import os
 
 import numpy as np
 
-ABI_VERSION = 9
+ABI_VERSION = 10
 RULE_NONE, RULE_GOAL, RULE_PICKUP, RULE_SIDEWALK, RULE_SIGN, RULE_HEALTH, RULE_PUTNEXT = 0, 1, 2, 3, 4, 5, 6
 SURF_WALL, SURF_FLOOR, SURF_CEIL = 0, 1, 2
 OP_END, OP_CHOICE, OP_UNIFORM, OP_PLACE, OP_MAZE, OP_IFEQ, OP_PUT = 0, 1, 2, 3, 4, 5, 6
@@ -109,7 +109,7 @@ class StateView(C.Structure):
 
 class Level(C.Structure):
     _fields_ = [("rule_kind", C.c_int32), ("rule_arg", C.c_int32), ("max_episode_steps", C.c_int32),
-                ("op_first", C.c_int32), ("num_ops", C.c_int32), ("reserved", C.c_int32), ("params", Params)]
+                ("op_first", C.c_int32), ("num_ops", C.c_int32), ("domain_rand", C.c_int32), ("params", Params)]
 
 
 def _expected_sizes():
@@ -441,8 +441,9 @@ class Engine:
 
     def set_levels(self, levels, env_level):
         """Several levels in one handle (mwb_set_levels).  levels: list of dicts with "rule" (kind, arg),
-        "max_episode_steps", "params" (DomainParams), "geometry" (rooms, quads, segs) and "ops" (this level's
-        program, proto indices already absolute); env_level: int [num_envs] level of each env."""
+        "max_episode_steps", "params" (DomainParams), "geometry" (rooms, quads, segs), "ops" (this level's
+        program, proto indices already absolute) and optionally "domain_rand" (0 or 1; default: the handle's
+        construction flag); env_level: int [num_envs] level of each env."""
         n = len(levels)
         table = (Level * n)()
         geoms = (Geometry * n)()
@@ -452,6 +453,7 @@ class Engine:
             rec.rule_kind, rec.rule_arg = int(lv["rule"][0]), int(lv["rule"][1])
             rec.max_episode_steps = int(lv["max_episode_steps"])
             rec.op_first, rec.num_ops = first, len(lv["ops"])
+            rec.domain_rand = int(lv.get("domain_rand", self.cfg.domain_rand))
             rec.params = lower_params(lv["params"])
             geoms[k] = self._geometry(*lv["geometry"])
             first += len(lv["ops"])
