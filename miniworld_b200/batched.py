@@ -93,6 +93,59 @@ def _definition_kwargs(kwargs, domain_rand):
     return kw
 
 
+class _LevelDef:
+    """What the engine needs for one level: a single-level batch has one, a level table one per row."""
+    rule = program = maze = maze_cdf = None
+    num_placed = 0
+
+
+def _define_level(level, kwargs, domain_rand, obs_width, obs_height):
+    """Build `level`'s definition instance with `kwargs` and lower it: rule, reset program, Maze templates, geometry,
+    capacities.  A level without a `device_rule` keeps `rule` None and is not lowered further (its batch rejects it).
+    `program` is None when the level resets on the host: it has no `device_program`, or it is a Maze whose templates
+    do not reproduce host-generated worlds (`maze_error` holds why)."""
+    d = _LevelDef()
+    d.cls = _resolve_level(level)
+    d.name = level if isinstance(level, str) else level.__name__
+    kw = _definition_kwargs(kwargs, domain_rand)
+    d.pe = pe = d.cls(device=None, obs_width=obs_width, obs_height=obs_height, **kw)
+    d.domain_rand = bool(pe.domain_rand)                 # the level's flag decides (its kwargs may set it)
+    rule = getattr(pe, "device_rule", None)
+    if rule is None:
+        return d
+    d.rule = _RULES[rule[0]], rule[1]
+    d.geometry = pack.pack_geometry(pe)
+    d.max_episode_steps = int(min(pe.max_episode_steps, 2 ** 31 - 1))     # math.inf: never truncates
+    d.device_info = dict(getattr(pe, "device_info", None) or {})
+    d.device_obs_extra = dict(getattr(pe, "device_obs_extra", None) or {})
+    d.uses_maze, d.maze_error = False, None
+    if getattr(pe, "device_program", None) is not None:
+        prog = ResetProgram()
+        pe.device_program(prog)
+        d.uses_maze = prog.uses_maze
+        if prog.uses_maze:
+            # per-episode topology on the device: only if the translated templates reproduce host-generated worlds
+            # exactly; otherwise the level resets on the host
+            from .maze_lowering import MazeTemplate
+            try:
+                tmpl = MazeTemplate(d.cls, **kw)
+                tmpl.verify(seeds=(0,))
+                d.maze, d.maze_cdf = tmpl, pack.room_cdf(pe.room_probs)
+            except AssertionError as e:
+                d.maze_error = e
+        if d.maze_error is None:
+            d.program, d.num_placed = prog, prog.num_placed
+    slack = 8 if d.maze is not None else 0               # Maze levels: 8 quads and 8 segments of slack
+    rooms, quads, segs = d.geometry
+    d.caps = (len(rooms), len(quads) + slack, len(segs) + slack)
+    return d
+
+
+def _common(dicts):
+    """The entries every dict has, with equal values."""
+    return {k: v for k, v in dicts[0].items() if all(d.get(k) == v for d in dicts[1:])}
+
+
 def default_env_level(num_envs, n_levels):
     """Level of each env when none is given: contiguous, near-equal blocks in the order the levels were listed (the
     first num_envs % n_levels levels get one env more)."""
@@ -127,8 +180,9 @@ class BatchedMiniWorld:
         self.device = int(device)
         self.dynamic_levels = bool(dynamic_levels)
         self.per_env_worlds = bool(per_env_worlds)
-        if isinstance(level, (list, tuple)):
-            self._init_levels(list(level), level_kwargs, env_level, msaa_samples, autoreset)
+        table = isinstance(level, (list, tuple))
+        if table:
+            defs = self._init_levels(list(level), level_kwargs, env_level)
         else:
             if env_level is not None:
                 raise ValueError("env_level assigns envs to levels: pass `level` as a sequence of levels")
@@ -137,7 +191,8 @@ class BatchedMiniWorld:
             if self.per_env_worlds:
                 raise ValueError("per_env_worlds lets Maze levels join a level table: pass `level` as a sequence of "
                                  "levels (a single Maze level always has per-env worlds)")
-            self._init_level(level, level_kwargs, msaa_samples, autoreset)
+            defs = self._init_level(level, level_kwargs)
+        self._init_engine(defs, table, msaa_samples, autoreset)
         self._level_views = None
         if self.dynamic_levels:
             self.level_seed, self.env_offset = int(level_seed), int(env_offset)
@@ -154,85 +209,21 @@ class BatchedMiniWorld:
         self._torch = None
         self._bufs = None
 
-    def _init_level(self, level, level_kwargs, msaa_samples, autoreset):
-        obs_width, obs_height, device = self.obs_width, self.obs_height, self.device
-        self.level_cls = _resolve_level(level)
-        self.level_kwargs = dict(level_kwargs or {})
-
-        # a definition-only instance of the level: layout, params, rule, action space
-        kw = _definition_kwargs(self.level_kwargs, self.domain_rand)
-        self.proto_env = self.level_cls(device=None, obs_width=obs_width, obs_height=obs_height, **kw)
-        pe = self.proto_env
-        self.domain_rand = bool(pe.domain_rand)          # the level's flag decides (level_kwargs may set it)
-        self.action_space = pe.action_space                  # per-env space: `step` takes one action per env
-        self.single_action_space = pe.action_space           # (gymnasium.vector naming)
-        self.single_observation_space = pe.observation_space
-        self.max_episode_steps = pe.max_episode_steps
-        rule = getattr(pe, "device_rule", None)
-        if rule is None:
+    def _init_level(self, level, level_kwargs):
+        d = _define_level(level, level_kwargs, self.domain_rand, self.obs_width, self.obs_height)
+        if d.rule is None:
             raise TypeError("%s has no `device_rule`; use world.MiniWorldEnv (single env) for levels whose "
-                            "step() rule is not lowered" % self.level_cls.__name__)
-        rule = _RULES[rule[0]], rule[1]
-        self.device_reset = getattr(pe, "device_program", None) is not None
-
-        rooms, quads, segs = pack.pack_geometry(pe)
-        self.maze_template = None
-        if self.device_reset:
-            self.program = ResetProgram()
-            pe.device_program(self.program)
-            if self.program.uses_maze:
-                # per-episode topology on the device: only if the translated templates reproduce
-                # host-generated worlds exactly; otherwise fall back to host-side resets
-                from .maze_lowering import MazeTemplate
-                try:
-                    tmpl = MazeTemplate(self.level_cls, **kw)
-                    tmpl.verify(seeds=(0,))
-                    self.maze_template = tmpl
-                except AssertionError:
-                    self.device_reset = False
-        if self.device_reset:
-            protos = self.program.proto_array()
-            max_ents = max(2, self.program.num_placed)     # exact: K2's shared-memory triangle capacity scales with it
-            caps = (len(rooms), len(quads), len(segs))
-            if self.maze_template is not None:
-                caps = (len(rooms), len(quads) + 8, len(segs) + 8)
-        else:
-            self.program = None
-            protos = None
-            max_ents = 8
-            caps = tuple(int(1.25 * n) + 4 for n in (len(rooms), len(quads), len(segs)))
-        shared = self.device_reset and self.maze_template is None
-        self.engine = Engine(self.num_envs, obs_width, obs_height, msaa_samples,
-                             shared_geometry=shared, max_rooms=caps[0], max_quads=caps[1],
-                             max_segs=caps[2], max_ents=max_ents, rule=rule, domain_rand=self.domain_rand,
-                             max_episode_steps=int(min(self.max_episode_steps, 2 ** 31 - 1)),   # math.inf: never truncates
-                             autoreset=autoreset and self.device_reset,
-                             device=device)
-        self.autoreset = bool(autoreset)
-        eng = self.engine
-        eng.sync_assets()
-        eng.set_params(pe.params)
-        if self.device_reset:
-            eng.set_protos(protos)
-            if self.maze_template is not None:
-                eng.set_maze(self.maze_template, pack.room_cdf(pe.room_probs))
-            else:
-                eng.set_template(rooms, quads, segs)
-            eng.set_program(self.program.op_array())
-        else:
-            # host-reset levels: one worker env per slot keeps that env's RNG stream
-            self._workers = [None] * self.num_envs
-            self._host_done = np.zeros(self.num_envs, bool)
+                            "step() rule is not lowered" % d.cls.__name__)
+        self.level_cls, self.level_kwargs, self.proto_env = d.cls, dict(level_kwargs or {}), d.pe
+        self.domain_rand = d.domain_rand
+        self.max_episode_steps = d.pe.max_episode_steps
         self.level_ids = [level]
-        self.proto_envs = [pe]
         self._env_level = np.zeros(self.num_envs, np.int32)
-        self._device_info = dict(getattr(pe, "device_info", None) or {})
-        self._device_obs_extra = dict(getattr(pe, "device_obs_extra", None) or {})
+        return [d]
 
-    def _init_levels(self, levels, level_kwargs, env_level, msaa_samples, autoreset):
-        """Several levels in one handle: each level's program is built, the proto tables are concatenated (each
-        program's proto indices moved by its level's offset), capacities are the maxima over the levels, and the
-        level table goes to the engine in one mwb_set_levels call."""
+    def _init_levels(self, levels, level_kwargs, env_level):
+        """Several levels in one handle: every level needs a device reset program, and Maze-family levels need
+        per-env worlds and templates that reproduce host-generated mazes (a table has no host resets)."""
         n = len(levels)
         if n == 0:
             raise ValueError("empty level list")
@@ -252,66 +243,82 @@ class BatchedMiniWorld:
                                                                                      env_level.shape))
         if env_level.size and (env_level.min() < 0 or env_level.max() >= n):
             raise ValueError("env_level entries must lie in [0, %d)" % n)
-        classes = [_resolve_level(lv) for lv in levels]
-        names = [lv if isinstance(lv, str) else lv.__name__ for lv in levels]
-        pes, table, protos, mazes = [], [], [], []
-        caps, max_placed = [0, 0, 0], 2
-        for name, cls, kw in zip(names, classes, kwargs):
-            kw = _definition_kwargs(kw, self.domain_rand)
-            pe = cls(device=None, obs_width=self.obs_width, obs_height=self.obs_height, **kw)
-            rule = getattr(pe, "device_rule", None)
-            if rule is None or getattr(pe, "device_program", None) is None:
-                raise ValueError("%s resets on the host only; a batch of several levels needs device reset programs" % name)
-            if rule[0] == "sign":
-                raise ValueError("%s cannot share a batch with other levels: its observation is a dict" % name)
-            prog = ResetProgram()
-            pe.device_program(prog)
-            maze = None
-            if prog.uses_maze:
-                if not self.per_env_worlds:
-                    raise ValueError("%s (Maze family) cannot share a batch with other levels: its geometry is per env "
-                                     "(pass per_env_worlds=True to give every env a world of its own)" % name)
-                # a table has no host resets: the device templates must reproduce host-generated mazes exactly
-                from .maze_lowering import MazeTemplate
-                try:
-                    maze = MazeTemplate(cls, **kw)
-                    maze.verify(seeds=(0,))
-                except AssertionError as e:
-                    raise ValueError("%s: its maze templates do not reproduce host-generated worlds, and a level table "
-                                     "cannot hold host-reset levels" % name) from e
-                mazes.append((len(table), maze, pack.room_cdf(pe.room_probs)))
-            ops = prog.op_array()
-            moved = (ops["op"] == OP_PLACE) | (ops["op"] == OP_PUT)     # the ops whose `a` is a proto index
-            ops["a"][moved] += len(protos)
-            protos.extend(prog.protos)
-            geom = pack.pack_geometry(pe)
-            slack = (0, 8, 8) if maze is not None else (0, 0, 0)         # as a one-level Maze handle is sized
-            caps = [max(c, len(g) + s) for c, g, s in zip(caps, geom, slack)]
-            max_placed = max(max_placed, prog.num_placed)
-            table.append(dict(rule=(_RULES[rule[0]], rule[1]), max_episode_steps=int(min(pe.max_episode_steps, 2 ** 31 - 1)),
-                              params=pe.params, geometry=geom, ops=ops, domain_rand=int(bool(pe.domain_rand))))
-            pes.append(pe)
-        self.level_ids, self.proto_envs, self._env_level = names, pes, env_level.astype(np.int32)
+        for lv in levels:
+            _resolve_level(lv)                           # an unknown id fails before any level is built
+        defs = []
+        for lv, kw in zip(levels, kwargs):
+            d = _define_level(lv, kw, self.domain_rand, self.obs_width, self.obs_height)
+            if d.rule is None or (d.program is None and not d.uses_maze):
+                raise ValueError("%s resets on the host only; a batch of several levels needs device reset programs"
+                                 % d.name)
+            if d.rule[0] == RULE_SIGN:
+                raise ValueError("%s cannot share a batch with other levels: its observation is a dict" % d.name)
+            if d.uses_maze and not self.per_env_worlds:
+                raise ValueError("%s (Maze family) cannot share a batch with other levels: its geometry is per env "
+                                 "(pass per_env_worlds=True to give every env a world of its own)" % d.name)
+            if d.program is None:
+                raise ValueError("%s: its maze templates do not reproduce host-generated worlds, and a level table "
+                                 "cannot hold host-reset levels" % d.name) from d.maze_error
+            defs.append(d)
+        self.level_ids = [d.name for d in defs]
         self.level_cls, self.level_kwargs, self.proto_env = None, kwargs, None
-        largest = max(pes, key=lambda pe: pe.action_space.n)
+        self.max_episode_steps = [d.pe.max_episode_steps for d in defs]     # per level
+        self._env_level = env_level.astype(np.int32)
+        return defs
+
+    def _init_engine(self, defs, table, msaa_samples, autoreset):
+        """Create the handle and program it in one of three ways: a single level that resets on the host (worlds
+        uploaded per env at its resets), a single Maze level with device templates (a world per env, no shared
+        template), or a level table through mwb_set_levels -- which is how every other single level is set up, as a
+        table of one row.  Capacities are the maxima over the levels; level 0 fills mwb_create's rule fields."""
+        d0 = defs[0]
+        self.proto_envs = [d.pe for d in defs]
+        largest = max(self.proto_envs, key=lambda pe: pe.action_space.n)
         self.action_space = self.single_action_space = largest.action_space
-        self.single_observation_space = pes[0].observation_space
-        self.max_episode_steps = [pe.max_episode_steps for pe in pes]     # per level
-        self.device_reset, self.maze_template, self.program = True, None, None
+        self.single_observation_space = d0.pe.observation_space
+        self.device_reset = all(d.program is not None for d in defs)
+        self.program, self.maze_template = (None, None) if table else (d0.program, d0.maze)
         self.autoreset = bool(autoreset)
-        self.engine = Engine(self.num_envs, self.obs_width, self.obs_height, msaa_samples, shared_geometry=True,
-                             max_rooms=caps[0], max_quads=caps[1], max_segs=caps[2], max_ents=max_placed,
-                             rule=table[0]["rule"], domain_rand=table[0]["domain_rand"],
-                             max_episode_steps=table[0]["max_episode_steps"], autoreset=self.autoreset, device=self.device)
-        self.engine.sync_assets()
-        self.engine.set_protos(np.array(protos, PROTO_DTYPE))
-        self.engine.set_levels(table, self._env_level)
-        for lvl, tmpl, cdf in mazes:
-            self.engine.set_level_maze(lvl, tmpl, cdf)
-        # a level's `info` key is returned only when every level defines it the same way
-        infos = [dict(getattr(pe, "device_info", None) or {}) for pe in pes]
-        self._device_info = {k: v for k, v in infos[0].items() if all(i.get(k) == v for i in infos[1:])}
-        self._device_obs_extra = {}
+        if self.device_reset:
+            caps = [max(c) for c in zip(*(d.caps for d in defs))]
+            # exact: K2's shared-memory triangle capacity scales with max_ents
+            max_ents = max([2] + [d.num_placed for d in defs])
+        else:
+            caps = [int(1.25 * len(g)) + 4 for g in d0.geometry]
+            max_ents = 8
+        self.engine = eng = Engine(self.num_envs, self.obs_width, self.obs_height, msaa_samples,
+                                   shared_geometry=self.device_reset and self.maze_template is None,
+                                   max_rooms=caps[0], max_quads=caps[1], max_segs=caps[2], max_ents=max_ents,
+                                   rule=d0.rule, domain_rand=d0.domain_rand, max_episode_steps=d0.max_episode_steps,
+                                   autoreset=self.autoreset and self.device_reset, device=self.device)
+        eng.sync_assets()
+        if not self.device_reset:
+            eng.set_params(d0.pe.params)
+            # host-reset levels: one worker env per slot keeps that env's RNG stream
+            self._workers = [None] * self.num_envs
+            self._host_done = np.zeros(self.num_envs, bool)
+        elif self.maze_template is not None:
+            eng.set_params(d0.pe.params)
+            eng.set_protos(self.program.proto_array())
+            eng.set_maze(self.maze_template, d0.maze_cdf)
+            eng.set_program(self.program.op_array())
+        else:
+            rows, protos = [], []
+            for d in defs:
+                ops = d.program.op_array()
+                moved = (ops["op"] == OP_PLACE) | (ops["op"] == OP_PUT)     # the ops whose `a` is a proto index
+                ops["a"][moved] += len(protos)
+                protos.extend(d.program.protos)
+                rows.append(dict(rule=d.rule, max_episode_steps=d.max_episode_steps, params=d.pe.params,
+                                 geometry=d.geometry, ops=ops, domain_rand=int(d.domain_rand)))
+            eng.set_protos(np.array(protos, PROTO_DTYPE))
+            eng.set_levels(rows, self._env_level)
+            for lvl, d in enumerate(defs):
+                if d.maze is not None:
+                    eng.set_level_maze(lvl, d.maze, d.maze_cdf)
+        # a level's `info` key / extra observation is returned only when every level defines it the same way
+        self._device_info = _common([d.device_info for d in defs])
+        self._device_obs_extra = _common([d.device_obs_extra for d in defs])
 
     # ------------------------------------------------------------------ buffers
     def _ensure_torch(self):

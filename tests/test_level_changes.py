@@ -1,41 +1,18 @@
 """Level changes at episode boundaries (mwb_enable_level_changes, BatchedMiniWorld(dynamic_levels=True)): pending
 assignments, the device-side level draw against its numpy restatement, snapshots, sharding and errors.  CPU cases
 run the kernels' host build; `gpu` cases run libmwb.so on the device."""
-import os
-import sys
-
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from level_parity import (STATE_KEYS, Follower, full_state, gpu_curriculum, model_levels, replay_draws, run_sharded,
+                          seed_reset, short_level)
 
 MIX = ["MiniWorld-Hallway-v0", "MiniWorld-FourRooms-v0", "MiniWorld-PickupObjects-v0", "MiniWorld-CollectHealth-v0",
        "MiniWorld-PutNext-v0", "MiniWorld-TMazeLeft-v0", "MiniWorld-Sidewalk-v0", "MiniWorld-OneRoomS6Fast-v0",
        "MiniWorld-ThreeRooms-v0"]
-STATE_KEYS = ("agent_pos", "agent_dir", "step_count", "rng", "num_picked_up", "carrying")
-
-
-def _short(name, steps):
-    """The level `name` truncated after `steps` steps: many resets in a short rollout."""
-    from miniworld_b200.envs import LEVELS
-    base = LEVELS[name]
-
-    def __init__(self, **kw):
-        base.__init__(self, **kw)
-        self.max_episode_steps = steps
-    return type("Short" + base.__name__, (base,), {"__init__": __init__})
-
-
-SHORT = [_short("MiniWorld-OneRoomS6Fast-v0", 7), _short("MiniWorld-Hallway-v0", 9), _short("MiniWorld-FourRooms-v0", 8),
-         _short("MiniWorld-PickupObjects-v0", 10)]
-
-
-def seed_reset(env, seeds, ids=None):
-    """reset(seed=...) without the render: mwb_seed + mwb_reset of the listed envs."""
-    from miniworld_b200.engine import RNG_DTYPE, rng_state_of
-    ids = np.arange(env.num_envs, dtype=np.int32) if ids is None else np.asarray(ids, np.int32)
-    env.engine.seed(ids, np.array([rng_state_of(int(s)) for s in seeds], RNG_DTYPE))
-    env.engine.reset(None if len(ids) == env.num_envs else ids)
+SHORT_IDS = [("MiniWorld-OneRoomS6Fast-v0", 7), ("MiniWorld-Hallway-v0", 9), ("MiniWorld-FourRooms-v0", 8),
+             ("MiniWorld-PickupObjects-v0", 10)]
+SHORT = [short_level(*lv) for lv in SHORT_IDS]
 
 
 def host_world_matches(env, i, cls, carried, domain_rand):
@@ -55,30 +32,6 @@ def host_world_matches(env, i, cls, carried, domain_rand):
     want = rng_state_of(pe.np_random)
     for f in want.dtype.names:
         assert st["rng"][i][f] == want[f], f
-
-
-class Follower:
-    """A one-env batch of env i's new level, seeded with the stream env i carried into its switch, stepped with env i's
-    actions: env i must equal it bit for bit."""
-
-    def __init__(self, cls, i, carried, domain_rand):
-        from miniworld_b200.batched import BatchedMiniWorld
-        from miniworld_b200.engine import RNG_DTYPE
-        self.i = i
-        self.env = BatchedMiniWorld(cls, 1, domain_rand=domain_rand, want_depth=True)
-        self.env.engine.seed([0], np.array([carried], RNG_DTYPE))
-        self.env.engine.reset()
-        self.out, self.steps = None, 0
-
-    def step_and_check(self, acts, out, st, render):
-        i = self.i
-        self.out = self.env.step_host(acts[i:i + 1], self.out, render=render)
-        for key in ("reward", "terminated", "truncated") + (("obs", "depth") if render else ()):
-            assert np.array_equal(out[key][i], self.out[key][0]), (i, key)
-        s1 = self.env.get_state(rng=True)
-        for key in STATE_KEYS:
-            assert np.array_equal(st[key][i], s1[key][0]), (i, key)
-        self.steps += 1
 
 
 # ------------------------------------------------------------------ CPU (kernels' host build)
@@ -139,16 +92,16 @@ def test_pending_assignment_takes_effect_at_the_next_reset(hostsim_path):
         acts = rng.integers(0, 3, N).astype(np.int32)
         render = t % 5 == 0
         out = env.step_host(acts, out, render=render)
-        st = env.get_state(rng=True)
+        st = full_state(env)
         for f in followers.values():
             if f.steps < 30:
-                f.step_and_check(acts, out, st, render)
+                f.step_and_check(acts, out, st, render, t)
         for i in range(N):
             if prev_done[i] and i in target and i not in switched:     # env i reset in this step
                 level[i] = target[i]
                 switched.add(i)
                 host_world_matches(env, i, SHORT[level[i]], carried[i], dr)
-                followers[i] = Follower(SHORT[level[i]], i, carried[i], dr)
+                followers[i] = Follower((SHORT[level[i]], {}), i, carried[i], dr)
         assert np.array_equal(env.env_level, level), t
         prev_done = (out["terminated"] | out["truncated"]).astype(bool)
     assert switched == set(target) and all(f.steps >= 30 for f in followers.values())
@@ -162,22 +115,6 @@ def test_pending_assignment_takes_effect_at_the_next_reset(hostsim_path):
     for f in followers.values():
         f.env.close()
     env.close()
-
-
-def model_levels(seed, offset, level, draws, pending, weights, resetting):
-    """The numpy restatement of one step's level resolution for the envs in `resetting` (in place)."""
-    from miniworld_b200.batched import sample_level
-    L = len(weights)
-    for i in np.nonzero(resetting)[0]:
-        p = int(pending[i])
-        if 0 <= p < L:
-            level[i] = p
-        else:
-            d = sample_level(seed, offset + i, draws[i], weights)
-            if d is not None:
-                level[i] = d
-                draws[i] += 1
-        pending[i] = -1
 
 
 def test_level_draws_equal_numpy_restatement(hostsim_path):
@@ -309,59 +246,9 @@ def test_construction_and_argument_errors(hostsim_path):
 
 
 # ------------------------------------------------------------------ multi-process sharding (gloo, host build)
-def _sharded_worker(rank, world, port, hostsim, total, steps, q):
-    sys.path.insert(0, ROOT)
-    sys.path.insert(0, os.path.join(ROOT, "tests"))
-    import torch
-    import torch.distributed as dist
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
-    dist.init_process_group("gloo", rank=rank, world_size=world)
-    from miniworld_b200 import engine
-    from miniworld_b200.dist import ShardedMiniWorld
-    engine._override_library_for_tests(hostsim)
-    env = ShardedMiniWorld(SHORT, total, dist=dist, domain_rand=True, dynamic_levels=True, level_seed=77)
-    seed_reset(env.local, [1000 + env.start + k for k in range(env.count)])
-    env.local.set_level_weights([1, 2, 0, 3])
-    acts_all = torch.as_tensor(np.random.default_rng(5).integers(0, 3, size=(steps, total), dtype=np.int32))
-    outs, out = [], None
-    for t in range(steps):
-        mine = env.scatter_actions(acts_all[t] if rank == 0 else None, like=torch.zeros(1))
-        out = env.local.step_host(mine.numpy(), out, render=t == steps - 1)
-        obs = env.gather_to_root(torch.as_tensor(out["obs"]))
-        rew = env.gather_to_root(torch.as_tensor(out["reward"]))
-        lvl = env.gather_to_root(torch.as_tensor(env.local.env_level))
-        if rank == 0:
-            outs.append((obs.numpy().copy(), rew.numpy().copy(), lvl.numpy().copy()))
-    if rank == 0:
-        q.put(outs)
-    dist.barrier()
-    dist.destroy_process_group()
-
-
 def test_sharded_dynamic_run_equals_single_process(hostsim_path):
-    import torch.multiprocessing as mp
-    from miniworld_b200.batched import BatchedMiniWorld
-    total, steps = 10, 30
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = 33500 + os.getpid() % 2000
-    procs = [ctx.Process(target=_sharded_worker, args=(r, 2, port, hostsim_path, total, steps, q)) for r in range(2)]
-    for p in procs:
-        p.start()
-    sharded = q.get(timeout=300)
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
-    env = BatchedMiniWorld(SHORT, total, domain_rand=True, dynamic_levels=True, level_seed=77)
-    seed_reset(env, 1000 + np.arange(total))
-    env.set_level_weights([1, 2, 0, 3])
-    start = env.env_level.copy()
-    acts_all = np.random.default_rng(5).integers(0, 3, size=(steps, total), dtype=np.int32)
-    out = None
-    for t in range(steps):
-        out = env.step_host(acts_all[t], out, render=t == steps - 1)
-        assert np.array_equal(out["reward"], sharded[t][1]) and np.array_equal(env.env_level, sharded[t][2]), t
-    assert np.array_equal(out["obs"], sharded[-1][0]) and 0 < out["obs"].mean() < 255
+    env, start = run_sharded(dict(levels=SHORT_IDS, domain_rand=True, level_seed=77, weights=[1, 2, 0, 3]), total=10,
+                             steps=30, port_base=33500)
     assert not np.array_equal(env.env_level, start)
     env.close()
 
@@ -371,70 +258,22 @@ GPU_LEVELS = ["MiniWorld-FourRooms-v0", "MiniWorld-Hallway-v0", "MiniWorld-OneRo
 
 
 def _gpu_run(N, steps, seed, level_seed, followers=None):
-    """4 levels, weights replaced every 50 steps by torch ops on the current stream.  Without `followers` the loop never
-    synchronises: the flags, levels and weights of every step are cloned on the device and returned.  `followers`
-    {env: switch step} replays the same run and checks those envs against one-env batches from the carried stream;
-    `checked` then maps each of them to the number of steps compared after its switch."""
+    """4 levels, weights replaced every 50 steps by torch ops on the current stream (gpu_curriculum)."""
     import torch
-    from miniworld_b200.batched import BatchedMiniWorld
-    env = BatchedMiniWorld(GPU_LEVELS, N, domain_rand=True, want_depth=True, dynamic_levels=True, level_seed=level_seed)
-    env.reset(seed=seed)
-    gen = torch.Generator(device="cuda")
-    gen.manual_seed(5)
-    acts_all = torch.randint(0, 3, (steps, N), dtype=torch.int32, device="cuda", generator=gen)
-    done_h, level_h, weight_h = [], [], []
-    live, checked = {}, {}
-    for t in range(steps):
-        if t % 50 == 0:
-            if t == 150:
-                env.level_weights.zero_()                                # keep every level for a while
-            else:
-                env.level_weights.copy_(torch.rand(len(GPU_LEVELS), device="cuda", generator=gen) - 0.2)
-        weight_h.append(env.level_weights.clone())
-        if followers is not None:
-            carried = None
-            for i, ts in followers.items():
-                if ts == t:
-                    carried = carried if carried is not None else env.get_state(rng=True)["rng"]
-                    live[i] = [None, carried[i].copy(), 0]
-        obs, rew, te, tr, info = env.step(acts_all[t])
-        if followers is None:
-            done_h.append((te | tr).clone())
-            level_h.append(info["level"].clone())
-            continue
-        for i, f in list(live.items()):
-            if f[0] is None:                                             # the switch step: env i just reset
-                f[0] = Follower(GPU_LEVELS[int(env.level_tensor[i])], i, f[1], True)
-                continue
-            out = {"reward": rew.cpu().numpy(), "terminated": te.cpu().numpy(), "truncated": tr.cpu().numpy(),
-                   "obs": obs.cpu().numpy(), "depth": info["depth"].cpu().numpy()}
-            f[0].step_and_check(acts_all[t].cpu().numpy(), out, env.get_state(rng=True), True)
-            checked[i] = f[0].steps
-            if out["terminated"][i] or out["truncated"][i] or f[0].steps >= 40:
-                f[0].env.close()
-                del live[i]
-    assert env.engine.overflow_count() == 0
-    return env, done_h, level_h, weight_h, checked
+
+    def weights(t, gen):
+        if t == 150:
+            return torch.zeros(len(GPU_LEVELS), device="cuda")               # keep every level for a while
+        return torch.rand(len(GPU_LEVELS), device="cuda", generator=gen) - 0.2
+    return gpu_curriculum([(lv, {}) for lv in GPU_LEVELS], N, steps, seed, level_seed, weights, domain_rand=True,
+                          followers=followers)
 
 
 @pytest.mark.gpu
 def test_gpu_device_curriculum_draws_equal_numpy_restatement(libmwb_path):
-    import torch
     N, steps, seed, level_seed = 4096, 300, 123, 99
     env, done_h, level_h, weight_h, _ = _gpu_run(N, steps, seed, level_seed)
-    done = torch.stack(done_h).cpu().numpy()
-    levels = torch.stack(level_h).cpu().numpy()
-    weights = torch.stack(weight_h).cpu().numpy()
-    level = env._env_level.copy()                  # the initial assignment
-    draws, pending = np.zeros(N, np.int64), np.full(N, -1)
-    switches = []
-    prev = np.zeros(N, bool)
-    for t in range(steps):
-        before = level.copy()
-        model_levels(level_seed, 0, level, draws, pending, weights[t], prev)
-        assert np.array_equal(levels[t], level), t
-        switches += [(int(i), t) for i in np.nonzero(level != before)[0]]
-        prev = done[t]
+    draws, switches = replay_draws(env, level_seed, done_h, level_h, weight_h)
     assert draws.sum() > N and len(switches) > 100
     env.close()
     # a seeded sample of switched envs: the episode after the switch equals a one-env batch from the carried stream
@@ -442,7 +281,7 @@ def test_gpu_device_curriculum_draws_equal_numpy_restatement(libmwb_path):
     pick = np.random.default_rng(0).choice(len(early), size=8, replace=False)
     followers = {}
     for k in pick:
-        i, t = early[k]
+        i, t = early[k][:2]
         followers.setdefault(i, t)
     env2, _, _, _, checked = _gpu_run(N, steps, seed, level_seed, followers=followers)
     assert set(checked) == set(followers) and min(checked.values()) >= 1 and sum(checked.values()) >= 2 * len(followers)

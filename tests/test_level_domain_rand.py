@@ -5,20 +5,17 @@ kernels' host build; `gpu` cases run libmwb.so on the device."""
 import ctypes as C
 import os
 import re
-import sys
 
 import numpy as np
 import pytest
 
-from test_level_changes import _short, model_levels
-from test_mixed_levels import STATE_KEYS, seed_reset
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from level_parity import (ROOT, STATE_KEYS, Follower, Lockstep, assert_env_equal, full_state, gpu_curriculum,
+                          replay_draws, run_sharded, seed_reset, short_level)
 
 # short episodes (8 / 9 / 10 steps) so that truncations and auto-resets happen inside the mix
-SHORT_FOURROOMS = _short("MiniWorld-FourRooms-v0", 8)
-SHORT_HALLWAY = _short("MiniWorld-Hallway-v0", 9)
-SHORT_PICKUP = _short("MiniWorld-PickupObjects-v0", 10)
+SHORT_FOURROOMS = short_level("MiniWorld-FourRooms-v0", 8)
+SHORT_HALLWAY = short_level("MiniWorld-Hallway-v0", 9)
+SHORT_PICKUP = short_level("MiniWorld-PickupObjects-v0", 10)
 OFF, ON = {"domain_rand": False}, {"domain_rand": True}
 MIXED_ROWS = [(SHORT_FOURROOMS, OFF), (SHORT_FOURROOMS, ON), (SHORT_PICKUP, OFF), (SHORT_PICKUP, ON),
               ("MiniWorld-PutNext-v0", ON), (SHORT_HALLWAY, OFF), ("MiniWorld-Sidewalk-v0", ON),
@@ -39,81 +36,6 @@ def narrowed_params(frac=0.25):
     return p
 
 
-def split_row(kwargs, batch_default=False):
-    """(flag, kwargs without the flag) of a row: the single-level batch that a row must equal gets the flag as its
-    batch argument."""
-    kw = dict(kwargs)
-    return bool(kw.pop("domain_rand", batch_default)), kw
-
-
-def single_of(level, kwargs, n, batch_default=False, **extra):
-    from miniworld_b200.batched import BatchedMiniWorld
-    flag, kw = split_row(kwargs, batch_default)
-    return BatchedMiniWorld(level, n, domain_rand=flag, level_kwargs=kw, want_depth=True, **extra)
-
-
-def assert_env_equal(sa, i, sb, j, where):
-    """Env i of state `sa` equals env j of state `sb`: STATE_KEYS plus everything domain randomisation draws (camera,
-    sky and light, entity colours, texture variants).  Capacities may differ: the smaller one is compared, and the
-    larger one's extra entity slots must be empty.  (Proto indices are not compared: a table shifts each level's.)"""
-    for key in STATE_KEYS + ("cam", "env_params"):
-        assert np.array_equal(sa[key][i], sb[key][j]), (where, key)
-    ea, eb = sa["ents"][i], sb["ents"][j]
-    E = min(len(ea), len(eb))
-    live = eb["proto"][:E] >= 0
-    assert np.array_equal(ea["proto"][:E] >= 0, live), (where, "live slots")
-    for f in ("pos", "dir", "color"):
-        assert np.array_equal(ea[f][:E][live], eb[f][:E][live]), (where, f)
-    assert (ea["proto"][E:] < 0).all() and (eb["proto"][E:] < 0).all(), where
-    if "room_tex" in sa and "room_tex" in sb:
-        R = min(sa["room_tex"].shape[1], sb["room_tex"].shape[1])
-        assert np.array_equal(sa["room_tex"][i, :R], sb["room_tex"][j, :R]), (where, "room_tex")
-
-
-def full_state(env):
-    return env.get_state(rng=True, room_tex=True)
-
-
-class Lockstep:
-    """A table (env i runs row i % L) and one single-level batch per row built with the row's flag, stepped with the
-    same actions."""
-
-    def __init__(self, rows, n_per, domain_rand=False, seed0=500, **kw):
-        from miniworld_b200.batched import BatchedMiniWorld
-        self.L, self.N = len(rows), n_per * len(rows)
-        self.el = np.arange(self.N, dtype=np.int32) % self.L
-        self.mix = BatchedMiniWorld([lv for lv, _ in rows], self.N, env_level=self.el, domain_rand=domain_rand,
-                                    want_depth=True, level_kwargs=[k for _, k in rows], **kw)
-        self.singles = [single_of(lv, k, n_per, domain_rand) for lv, k in rows]
-        for k, s in enumerate(self.singles):
-            assert bool(self.mix.proto_envs[k].domain_rand) == s.domain_rand == bool(s.engine.cfg.domain_rand)
-        self.seeds = seed0 + np.arange(self.N)
-        seed_reset(self.mix, self.seeds)
-        for k, s in enumerate(self.singles):
-            seed_reset(s, self.seeds[self.el == k])
-        self.own_n = np.array([self.singles[k].action_space.n for k in self.el])
-        self.out_m, self.outs = None, [None] * self.L
-
-    def step(self, acts, render):
-        self.out_m = self.mix.step_host(acts, self.out_m, render=render)
-        for k, s in enumerate(self.singles):
-            self.outs[k] = s.step_host(acts[self.el == k], self.outs[k], render=render)
-
-    def check(self, t, render):
-        sm = full_state(self.mix)
-        for k, s in enumerate(self.singles):
-            sel, o, ss = np.nonzero(self.el == k)[0], self.outs[k], full_state(s)
-            if o is not None:
-                for key in ("reward", "terminated", "truncated") + (("obs", "depth") if render else ()):
-                    assert np.array_equal(self.out_m[key][sel], o[key]), (t, k, key)
-            for j, i in enumerate(sel):
-                assert_env_equal(sm, i, ss, j, (t, k, int(i)))
-
-    def close(self):
-        for e in [self.mix] + self.singles:
-            e.close()
-
-
 # ------------------------------------------------------------------ CPU (kernels' host build)
 def test_mixed_flags_equal_single_level_batches(hostsim_path):
     ls = Lockstep(MIXED_ROWS, n_per=2)
@@ -123,7 +45,7 @@ def test_mixed_flags_equal_single_level_batches(hostsim_path):
     ls.check("reset", False)
     for t in range(70):
         render = t % 10 == 0 or t == 69
-        ls.step((rng.random(ls.N) * ls.own_n).astype(np.int32), render)
+        ls.step(ls.actions(rng), render)
         ls.check(t, render)
         ended += ls.out_m["terminated"] | ls.out_m["truncated"]
         if render:
@@ -208,28 +130,6 @@ def test_reference_trajectories_side_by_side(hostsim_path, case):
 
 SWITCH_ROWS = [(SHORT_FOURROOMS, OFF), (SHORT_FOURROOMS, ON), (SHORT_PICKUP, ON), (SHORT_PICKUP, OFF),
                ("MiniWorld-FourRooms-v0", dict(ON, params=narrowed_params()))]
-
-
-class Follower:
-    """A one-env batch of a row, built with the row's flag and seeded with the stream env i carried into its switch."""
-
-    def __init__(self, row, i, carried):
-        from miniworld_b200.engine import RNG_DTYPE
-        self.i = i
-        self.env = single_of(row[0], row[1], 1)
-        self.env.engine.seed([0], np.array([carried], RNG_DTYPE))
-        self.env.engine.reset()
-        self.out = None
-
-    def check_state(self, st, where):
-        assert_env_equal(st, self.i, full_state(self.env), 0, where)
-
-    def step_and_check(self, acts, out, st, render, where):
-        i = self.i
-        self.out = self.env.step_host(acts[i:i + 1], self.out, render=render)
-        for key in ("reward", "terminated", "truncated") + (("obs", "depth") if render else ()):
-            assert np.array_equal(out[key][i], self.out[key][0]), (where, i, key)
-        self.check_state(st, where)
 
 
 def test_level_changes_across_the_flag(hostsim_path):
@@ -427,66 +327,13 @@ def test_snapshot_restore_of_a_dynamic_mixed_flag_handle(hostsim_path):
 
 # ------------------------------------------------------------------ multi-process sharding (gloo, host build)
 SHARD_ROWS = [("MiniWorld-FourRooms-v0", OFF), ("MiniWorld-FourRooms-v0", dict(ON, params=narrowed_params())),
-              ("MiniWorld-FourRooms-v0", ON), (SHORT_HALLWAY, OFF), (SHORT_HALLWAY, ON)]
-
-
-def _sharded_worker(rank, world, port, hostsim, total, steps, q):
-    sys.path.insert(0, ROOT)
-    sys.path.insert(0, os.path.join(ROOT, "tests"))
-    import torch
-    import torch.distributed as dist
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
-    dist.init_process_group("gloo", rank=rank, world_size=world)
-    from miniworld_b200 import engine
-    from miniworld_b200.dist import ShardedMiniWorld
-    engine._override_library_for_tests(hostsim)
-    env = ShardedMiniWorld([lv for lv, _ in SHARD_ROWS], total, dist=dist, level_kwargs=[k for _, k in SHARD_ROWS],
-                           dynamic_levels=True, level_seed=31)
-    seed_reset(env.local, [1000 + env.start + k for k in range(env.count)])
-    env.local.set_level_weights([1, 1, 1, 2, 2])
-    acts_all = torch.as_tensor(np.random.default_rng(5).integers(0, 3, size=(steps, total), dtype=np.int32))
-    outs, out = [], None
-    for t in range(steps):
-        mine = env.scatter_actions(acts_all[t] if rank == 0 else None, like=torch.zeros(1))
-        out = env.local.step_host(mine.numpy(), out, render=t == steps - 1)
-        obs = env.gather_to_root(torch.as_tensor(out["obs"]))
-        rew = env.gather_to_root(torch.as_tensor(out["reward"]))
-        lvl = env.gather_to_root(torch.as_tensor(env.local.env_level))
-        par = env.gather_to_root(torch.as_tensor(env.local.get_state()["env_params"]))
-        if rank == 0:
-            outs.append((obs.numpy().copy(), rew.numpy().copy(), lvl.numpy().copy(), par.numpy().copy()))
-    if rank == 0:
-        q.put(outs)
-    dist.barrier()
-    dist.destroy_process_group()
+              ("MiniWorld-FourRooms-v0", ON), (("MiniWorld-Hallway-v0", 9), OFF), (("MiniWorld-Hallway-v0", 9), ON)]
 
 
 def test_sharded_mixed_flag_curriculum_equals_single_process(hostsim_path):
-    import torch.multiprocessing as mp
-    from miniworld_b200.batched import BatchedMiniWorld
-    total, steps = 10, 30
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = 37500 + os.getpid() % 2000
-    procs = [ctx.Process(target=_sharded_worker, args=(r, 2, port, hostsim_path, total, steps, q)) for r in range(2)]
-    for p in procs:
-        p.start()
-    sharded = q.get(timeout=300)
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
-    env = BatchedMiniWorld([lv for lv, _ in SHARD_ROWS], total, level_kwargs=[k for _, k in SHARD_ROWS],
-                           dynamic_levels=True, level_seed=31)
-    seed_reset(env, 1000 + np.arange(total))
-    env.set_level_weights([1, 1, 1, 2, 2])
-    start = env.env_level.copy()
-    acts_all = np.random.default_rng(5).integers(0, 3, size=(steps, total), dtype=np.int32)
-    out = None
-    for t in range(steps):
-        out = env.step_host(acts_all[t], out, render=t == steps - 1)
-        assert np.array_equal(out["reward"], sharded[t][1]) and np.array_equal(env.env_level, sharded[t][2]), t
-        assert np.array_equal(env.get_state()["env_params"], sharded[t][3]), t
-    assert np.array_equal(out["obs"], sharded[-1][0]) and 0 < out["obs"].mean() < 255
+    spec = dict(levels=[lv for lv, _ in SHARD_ROWS], level_kwargs=[k for _, k in SHARD_ROWS], level_seed=31,
+                weights=[1, 1, 1, 2, 2])
+    env, start = run_sharded(spec, total=10, steps=30, port_base=37500)
     assert not np.array_equal(env.env_level, start)
     env.close()
 
@@ -498,52 +345,10 @@ GPU_ROWS = [("MiniWorld-FourRooms-v0", OFF), ("MiniWorld-FourRooms-v0", dict(ON,
 
 
 def _gpu_run(N, steps, seed, level_seed, followers=None):
-    """The ladder with weights rewritten by torch on the current stream every 50 steps.  Without `followers` the loop
-    never synchronises and returns each step's flags, levels and weights.  `followers` {env: switch step} replays the
-    same run and compares those envs, frames included, every step against one-env batches of their new rows from the
-    carried stream; `checked` maps each to the number of steps compared after its switch."""
+    """The ladder with weights rewritten by torch on the current stream every 50 steps (gpu_curriculum)."""
     import torch
-    from miniworld_b200.batched import BatchedMiniWorld
-    env = BatchedMiniWorld([lv for lv, _ in GPU_ROWS], N, level_kwargs=[k for _, k in GPU_ROWS], want_depth=True,
-                           dynamic_levels=True, level_seed=level_seed)
-    env.reset(seed=seed)
-    gen = torch.Generator(device="cuda")
-    gen.manual_seed(5)
-    acts_all = torch.randint(0, 3, (steps, N), dtype=torch.int32, device="cuda", generator=gen)
-    done_h, level_h, weight_h = [], [], []
-    live, checked = {}, {}
-    for t in range(steps):
-        if t % 50 == 0:
-            env.level_weights.copy_(torch.rand(len(GPU_ROWS), device="cuda", generator=gen) - 0.1)
-        weight_h.append(env.level_weights.clone())
-        if followers is not None:
-            carried = None
-            for i, ts in followers.items():
-                if ts == t:
-                    carried = carried if carried is not None else env.get_state(rng=True)["rng"]
-                    live[i] = [None, carried[i].copy(), 0]
-        obs, rew, te, tr, info = env.step(acts_all[t])
-        if followers is None:
-            done_h.append((te | tr).clone())
-            level_h.append(info["level"].clone())
-            continue
-        st = full_state(env) if live else None
-        out = None
-        for i, f in list(live.items()):
-            if f[0] is None:                                             # the switch step: env i just reset
-                f[0] = Follower(GPU_ROWS[int(env.level_tensor[i])], i, f[1])
-                f[0].check_state(st, ("switch", t))
-                continue
-            if out is None:
-                out = {"reward": rew.cpu().numpy(), "terminated": te.cpu().numpy(), "truncated": tr.cpu().numpy(),
-                       "obs": obs.cpu().numpy(), "depth": info["depth"].cpu().numpy()}
-            f[0].step_and_check(acts_all[t].cpu().numpy(), out, st, True, t)
-            checked[i] = checked.get(i, 0) + 1
-            if out["terminated"][i] or out["truncated"][i] or checked[i] >= 40:
-                f[0].env.close()
-                del live[i]
-    assert env.engine.overflow_count() == 0
-    return env, done_h, level_h, weight_h, checked
+    weights = lambda t, gen: torch.rand(len(GPU_ROWS), device="cuda", generator=gen) - 0.1
+    return gpu_curriculum(GPU_ROWS, N, steps, seed, level_seed, weights, followers=followers)
 
 
 @pytest.mark.gpu
@@ -552,19 +357,7 @@ def test_gpu_mixed_flag_ladder_at_scale(libmwb_path):
     sms = torch.cuda.get_device_properties(0).multi_processor_count
     N, steps, seed, level_seed = max(4096, 12 * sms), 300, 321, 77
     env, done_h, level_h, weight_h, _ = _gpu_run(N, steps, seed, level_seed)
-    done = torch.stack(done_h).cpu().numpy()
-    levels = torch.stack(level_h).cpu().numpy()
-    weights = torch.stack(weight_h).cpu().numpy()
-    level = env._env_level.copy()
-    draws, pending = np.zeros(N, np.int64), np.full(N, -1)
-    switches = []
-    prev = np.zeros(N, bool)
-    for t in range(steps):
-        before = level.copy()
-        model_levels(level_seed, 0, level, draws, pending, weights[t], prev)
-        assert np.array_equal(levels[t], level), t
-        switches += [(int(i), t, int(before[i]), int(level[i])) for i in np.nonzero(level != before)[0]]
-        prev = done[t]
+    _, switches = replay_draws(env, level_seed, done_h, level_h, weight_h)
     env.close()
     flag = [k["domain_rand"] for _, k in GPU_ROWS]
     on_off = [sw for sw in switches if sw[1] < steps - 1 and flag[sw[2]] and not flag[sw[3]]]

@@ -4,14 +4,11 @@ depth and static geometry -- also after level changes across template and per-en
 CPU cases run the kernels' host build; `gpu` cases run libmwb.so on the device."""
 import os
 import re
-import sys
 
 import numpy as np
 import pytest
 
-from test_mixed_levels import STATE_KEYS, seed_reset
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from level_parity import STATE_KEYS, Follower, Lockstep, full_state, geometry_equal, run_sharded, seed_reset
 
 MAZE_KW = {"num_rows": 3, "num_cols": 5}        # non-square: a rows / cols mix-up changes the world
 MIX = [("MiniWorld-MazeS2-v0", {}), ("MiniWorld-MazeS3-v0", {}), ("MiniWorld-MazeS3Fast-v0", {}),
@@ -20,68 +17,8 @@ MIX = [("MiniWorld-MazeS2-v0", {}), ("MiniWorld-MazeS3-v0", {}), ("MiniWorld-Maz
 LADDER = ["MiniWorld-OneRoom-v0", "MiniWorld-MazeS2-v0", "MiniWorld-MazeS3-v0", "MiniWorld-Maze-v0"]
 
 
-def geometry_equal(a, b):
-    """mwb_get_geometry of two envs, compared field by field (struct padding is not part of the geometry; a template's
-    tex_id is its definition env's own draw, unused by device resets)."""
-    ga, gb = a.engine.get_geometry(a._i), b.engine.get_geometry(b._i)
-    for x, y in zip(ga, gb):
-        if len(x) != len(y):
-            return False
-        for f in x.dtype.names:
-            if f not in ("reserved", "tex_id") and not np.array_equal(x[f], y[f]):
-                return False
-    return True
-
-
-def geom(env, i):
-    env._i = i
-    return env
-
-
-class Lockstep:
-    """A mix (env i runs level i % L, with its own kwargs) and one batch per level, stepped with the same actions."""
-
-    def __init__(self, levels, n_per, domain_rand, seed0=500, **kw):
-        from miniworld_b200.batched import BatchedMiniWorld
-        self.L, self.N = len(levels), n_per * len(levels)
-        self.el = np.arange(self.N, dtype=np.int32) % self.L
-        self.mix = BatchedMiniWorld([lv for lv, _ in levels], self.N, env_level=self.el, domain_rand=domain_rand,
-                                    want_depth=True, level_kwargs=[k for _, k in levels], per_env_worlds=True, **kw)
-        self.singles = [BatchedMiniWorld(lv, n_per, domain_rand=domain_rand, want_depth=True, level_kwargs=k, **kw)
-                        for lv, k in levels]
-        assert all(s.device_reset for s in self.singles)
-        self.seeds = seed0 + np.arange(self.N)
-        seed_reset(self.mix, self.seeds)
-        for k, s in enumerate(self.singles):
-            seed_reset(s, self.seeds[self.el == k])
-        self.own_n = np.array([self.singles[k].action_space.n for k in self.el])
-        self.out_m, self.outs = None, [None] * self.L
-
-    def step(self, acts, render):
-        self.out_m = self.mix.step_host(acts, self.out_m, render=render)
-        for k, s in enumerate(self.singles):
-            self.outs[k] = s.step_host(acts[self.el == k], self.outs[k], render=render)
-
-    def check(self, t, render, geometry=False):
-        sm = self.mix.get_state(rng=True)
-        for k, s in enumerate(self.singles):
-            sel, o, ss = self.el == k, self.outs[k], s.get_state(rng=True)
-            for key in ("reward", "terminated", "truncated") + (("obs", "depth") if render else ()):
-                if o is not None:
-                    assert np.array_equal(self.out_m[key][sel], o[key]), (t, k, key)
-            for key in STATE_KEYS:
-                assert np.array_equal(sm[key][sel], ss[key]), (t, k, key)
-            if geometry:
-                for j, i in enumerate(np.nonzero(sel)[0]):
-                    assert geometry_equal(geom(self.mix, i), geom(s, j)), (t, k, i)
-
-    def close(self):
-        for e in [self.mix] + self.singles:
-            e.close()
-
-
 def run_parity(levels, n_per, steps, domain_rand, render_every, geometry_every):
-    ls = Lockstep(levels, n_per, domain_rand)
+    ls = Lockstep(levels, n_per, domain_rand, per_env_worlds=True)
     rng = np.random.default_rng(3)
     ended = np.zeros(ls.N, np.int64)
     ls.check("reset", False, geometry=True)
@@ -147,15 +84,6 @@ def test_reference_trajectories_inside_a_mix(hostsim_path, name):
     mix_trajectory(name, golden(name), steps=200 if name == "maze_dr" else None)
 
 
-def carried_follower(cls, carried, domain_rand=False):
-    from miniworld_b200.batched import BatchedMiniWorld
-    from miniworld_b200.engine import RNG_DTYPE
-    f = BatchedMiniWorld(cls, 1, domain_rand=domain_rand, want_depth=True)
-    f.engine.seed([0], np.array([carried], RNG_DTYPE))
-    f.engine.reset()
-    return f
-
-
 def test_level_changes_across_world_kinds(hostsim_path):
     """OneRoom -> Maze, Maze -> OneRoom and Maze -> MazeS2 by pending assignment: after the switch the env equals a
     fresh env of its new level seeded with the stream it carried (state, frames, geometry); weight draws follow
@@ -176,23 +104,17 @@ def test_level_changes_across_world_kinds(hostsim_path):
     env.set_env_level(ids, [moves[i] for i in ids])
     env.engine.reset(ids)
     assert list(env.env_level[ids]) == [moves[i] for i in ids]
-    followers = {int(i): carried_follower(LADDER[moves[int(i)]], carried[k]) for k, i in enumerate(ids)}
-    fouts = {i: None for i in followers}
+    followers = {int(i): Follower((LADDER[moves[int(i)]], {}), int(i), carried[k]) for k, i in enumerate(ids)}
     for t in range(12):
         acts = rng.integers(0, 3, N).astype(np.int32)
         render = t % 4 == 0
         out = env.step_host(acts, out, render=render)
-        st = env.get_state(rng=True)
+        st = full_state(env)
         for i, f in followers.items():
-            fouts[i] = f.step_host(acts[i:i + 1], fouts[i], render=render)
-            fs = f.get_state(rng=True)
-            for key in ("reward", "terminated", "truncated") + (("obs", "depth") if render else ()):
-                assert np.array_equal(out[key][i], fouts[i][key][0]), (t, i, key)
-            for key in STATE_KEYS:
-                assert np.array_equal(st[key][i], fs[key][0]), (t, i, key)
-            assert geometry_equal(geom(env, i), geom(f, 0)), (t, i)
+            f.step_and_check(acts, out, st, render, t)
+            assert geometry_equal(env, i, f.env, 0), (t, i)
     for f in followers.values():
-        f.close()
+        f.env.close()
     # weight-driven draws at resets of every env
     w = np.array([1.0, 0.5, 2.0, 1.5], np.float32)
     env.set_level_weights(w)
@@ -336,63 +258,14 @@ def test_flag_without_maze_levels_changes_nothing(hostsim_path):
     sa, sb = a.snapshot(), b.snapshot()
     assert len(sa) == len(sb) and bytes(sa[:4]) == bytes(sb[:4]) == b"MWBS"
     for i in range(4):
-        assert geometry_equal(geom(a, i), geom(b, i))
+        assert geometry_equal(a, i, b, i)
     a.close()
     b.close()
 
 
-def _sharded_worker(rank, world, port, hostsim, total, steps, q):
-    sys.path.insert(0, ROOT)
-    sys.path.insert(0, os.path.join(ROOT, "tests"))
-    import torch
-    import torch.distributed as dist
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
-    dist.init_process_group("gloo", rank=rank, world_size=world)
-    from miniworld_b200 import engine
-    from miniworld_b200.dist import ShardedMiniWorld
-    engine._override_library_for_tests(hostsim)
-    env = ShardedMiniWorld(LADDER, total, dist=dist, dynamic_levels=True, level_seed=12, per_env_worlds=True)
-    seed_reset(env.local, [1000 + env.start + k for k in range(env.count)])
-    env.local.set_level_weights([1, 2, 2, 1])
-    acts_all = torch.as_tensor(np.random.default_rng(5).integers(0, 3, size=(steps, total), dtype=np.int32))
-    outs, out = [], None
-    for t in range(steps):
-        mine = env.scatter_actions(acts_all[t] if rank == 0 else None, like=torch.zeros(1))
-        out = env.local.step_host(mine.numpy(), out, render=t == steps - 1)
-        obs = env.gather_to_root(torch.as_tensor(out["obs"]))
-        rew = env.gather_to_root(torch.as_tensor(out["reward"]))
-        lvl = env.gather_to_root(torch.as_tensor(env.local.env_level))
-        if rank == 0:
-            outs.append((obs.numpy().copy(), rew.numpy().copy(), lvl.numpy().copy()))
-    if rank == 0:
-        q.put(outs)
-    dist.barrier()
-    dist.destroy_process_group()
-
-
 def test_sharded_maze_curriculum_equals_single_process(hostsim_path):
-    import torch.multiprocessing as mp
-    from miniworld_b200.batched import BatchedMiniWorld
-    total, steps = 8, 30
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = 35500 + os.getpid() % 2000
-    procs = [ctx.Process(target=_sharded_worker, args=(r, 2, port, hostsim_path, total, steps, q)) for r in range(2)]
-    for p in procs:
-        p.start()
-    sharded = q.get(timeout=300)
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
-    env = BatchedMiniWorld(LADDER, total, dynamic_levels=True, level_seed=12, per_env_worlds=True)
-    seed_reset(env, 1000 + np.arange(total))
-    env.set_level_weights([1, 2, 2, 1])
-    acts_all = np.random.default_rng(5).integers(0, 3, size=(steps, total), dtype=np.int32)
-    out = None
-    for t in range(steps):
-        out = env.step_host(acts_all[t], out, render=t == steps - 1)
-        assert np.array_equal(out["reward"], sharded[t][1]) and np.array_equal(env.env_level, sharded[t][2]), t
-    assert np.array_equal(out["obs"], sharded[-1][0]) and 0 < out["obs"].mean() < 255
+    env, _ = run_sharded(dict(levels=LADDER, level_seed=12, per_env_worlds=True, weights=[1, 2, 2, 1]), total=8,
+                         steps=30, port_base=35500)
     env.close()
 
 
@@ -510,14 +383,12 @@ def test_gpu_maze_curriculum_at_scale(libmwb_path):
     sample = np.random.default_rng(0).choice(N, 16, replace=False)
     env.set_level_weights(np.zeros(len(LADDER)))
     env.engine.reset(sample.astype(np.int32))
-    st2 = env.get_state(rng=True)
+    st2 = full_state(env)
     for i in sample:
-        f = carried_follower(LADDER[int(lv[-1][i])], st["rng"][i], domain_rand=True)
-        fs = f.get_state(rng=True)
-        for key in STATE_KEYS:
-            assert np.array_equal(st2[key][i], fs[key][0]), (i, key)
-        assert geometry_equal(geom(env, int(i)), geom(f, 0)), i
-        f.close()
+        f = Follower((LADDER[int(lv[-1][i])], {}), int(i), st["rng"][i], batch_default=True)
+        f.check_state(st2, i)
+        assert geometry_equal(env, int(i), f.env, 0), i
+        f.env.close()
     assert env.engine.overflow_count() == 0
     env.close()
 

@@ -1,70 +1,23 @@
 """Several levels in one batch (mwb_set_levels): env i of a mixed batch must equal, bit for bit, env i of a batch of
 its own level seeded the same way -- rewards, flags, poses, step counters, RNG streams, frames and depth maps.
 CPU cases run the kernels' host build; `gpu` cases run libmwb.so on the device."""
-import os
-import sys
-
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from level_parity import STATE_KEYS, Lockstep, geometry_equal, run_sharded, seed_reset
 
 # every rule kind but Sign; OneRoomS6Fast brings its own params and a 50-step truncation, ThreeRooms an ImageFrame
 MIX = ["MiniWorld-Hallway-v0", "MiniWorld-FourRooms-v0", "MiniWorld-PickupObjects-v0", "MiniWorld-CollectHealth-v0",
        "MiniWorld-PutNext-v0", "MiniWorld-TMazeLeft-v0", "MiniWorld-Sidewalk-v0", "MiniWorld-OneRoomS6Fast-v0",
        "MiniWorld-ThreeRooms-v0"]
-STATE_KEYS = ("agent_pos", "agent_dir", "step_count", "rng", "num_picked_up", "carrying")
 
 
-def seed_reset(env, seeds, ids=None):
-    """reset(seed=...) without the render: mwb_seed + mwb_reset of the listed envs."""
-    from miniworld_b200.engine import RNG_DTYPE, rng_state_of
-    ids = np.arange(env.num_envs, dtype=np.int32) if ids is None else np.asarray(ids, np.int32)
-    env.engine.seed(ids, np.array([rng_state_of(int(s)) for s in seeds], RNG_DTYPE))
-    env.engine.reset(None if len(ids) == env.num_envs else ids)
-
-
-class Lockstep:
-    """A mixed batch (env i runs level i % L) and one batch per level, stepped with the same per-env actions."""
-
-    def __init__(self, levels, n_per, domain_rand, seed0=500, **kw):
-        from miniworld_b200.batched import BatchedMiniWorld
-        self.L, self.N = len(levels), n_per * len(levels)
-        self.el = np.arange(self.N, dtype=np.int32) % self.L
-        self.mix = BatchedMiniWorld(levels, self.N, env_level=self.el, domain_rand=domain_rand, want_depth=True, **kw)
-        self.singles = [BatchedMiniWorld(lv, n_per, domain_rand=domain_rand, want_depth=True, **kw) for lv in levels]
-        self.seeds = seed0 + np.arange(self.N)
-        seed_reset(self.mix, self.seeds)
-        for k, s in enumerate(self.singles):
-            seed_reset(s, self.seeds[self.el == k])
-        self.own_n = np.array([self.singles[k].action_space.n for k in self.el])
-        self.out_m, self.outs = None, [None] * self.L
-
-    def actions(self, rng, largest=False):
-        high = np.full(self.N, self.mix.single_action_space.n) if largest else self.own_n
-        return (rng.random(self.N) * high).astype(np.int32)
-
-    def step(self, acts, render):
-        self.out_m = self.mix.step_host(acts, self.out_m, render=render)
-        for k, s in enumerate(self.singles):
-            self.outs[k] = s.step_host(acts[self.el == k], self.outs[k], render=render)
-
-    def check(self, t, render):
-        sm = self.mix.get_state(rng=True)
-        for k, s in enumerate(self.singles):
-            sel, o, ss = self.el == k, self.outs[k], s.get_state(rng=True)
-            for key in ("reward", "terminated", "truncated") + (("obs", "depth") if render else ()):
-                assert np.array_equal(self.out_m[key][sel], o[key]), (t, self.mix.level_ids[k], key)
-            for key in STATE_KEYS:
-                assert np.array_equal(sm[key][sel], ss[key]), (t, self.mix.level_ids[k], key)
-
-    def close(self):
-        for e in [self.mix] + self.singles:
-            e.close()
+def rows(levels):
+    return [(lv, {}) for lv in levels]
 
 
 def run_parity(levels, n_per, steps, domain_rand, render_every, largest=False):
-    ls = Lockstep(levels, n_per, domain_rand)
+    ls = Lockstep(rows(levels), n_per, domain_rand)
     rng = np.random.default_rng(7)
     trunc = np.zeros(ls.N, np.int64)
     ended = np.zeros(ls.N, np.int64)
@@ -98,7 +51,7 @@ def test_out_of_space_actions_match_single_level_batches(hostsim_path):
 
 
 def test_subset_reset_visible_ents_and_geometry(hostsim_path):
-    ls = Lockstep(MIX, n_per=2, domain_rand=True)
+    ls = Lockstep(rows(MIX), n_per=2, domain_rand=True)
     rng = np.random.default_rng(11)
     for t in range(12):
         ls.step(ls.actions(rng), render=False)
@@ -120,13 +73,7 @@ def test_subset_reset_visible_ents_and_geometry(hostsim_path):
         s.visible_ents(v)
         assert np.array_equal(vis[ls.el == k], v)
     for i in (0, 5, 16):           # mwb_get_geometry goes through the env's level
-        want = ls.singles[ls.el[i]].engine.get_geometry(0)
-        got = ls.mix.engine.get_geometry(i)
-        for w, g in zip(want, got):
-            assert len(w) == len(g)
-            for field in w.dtype.names:
-                if field not in ("reserved", "tex_id"):     # tex_id: the definition env's own draw, unused by device resets
-                    assert np.array_equal(w[field], g[field]), (i, field)
+        assert geometry_equal(ls.singles[ls.el[i]], 0, ls.mix, i), i
     ls.close()
 
 
@@ -134,7 +81,7 @@ def test_snapshot_restore_and_assignment_check(hostsim_path):
     from miniworld_b200.batched import BatchedMiniWorld
     from miniworld_b200.engine import EngineError
     levels = MIX[:5]
-    ls = Lockstep(levels, n_per=2, domain_rand=True)
+    ls = Lockstep(rows(levels), n_per=2, domain_rand=True)
     rng = np.random.default_rng(3)
     acts = [ls.actions(rng) for _ in range(40)]
     for t in range(15):
@@ -260,56 +207,9 @@ def test_c_abi_rejects_bad_level_tables(hostsim_path):
 
 
 # ------------------------------------------------------------------ multi-process sharding (gloo, host build)
-def _sharded_worker(rank, world, port, hostsim, total, steps, q):
-    sys.path.insert(0, ROOT)
-    sys.path.insert(0, os.path.join(ROOT, "tests"))
-    import torch
-    import torch.distributed as dist
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
-    dist.init_process_group("gloo", rank=rank, world_size=world)
-    from miniworld_b200 import engine
-    from miniworld_b200.dist import ShardedMiniWorld
-    engine._override_library_for_tests(hostsim)
-    env = ShardedMiniWorld(MIX[:4], total, dist=dist, domain_rand=True)
-    seed_reset(env.local, [1000 + env.start + k for k in range(env.count)])
-    acts_all = torch.as_tensor(np.random.default_rng(5).integers(0, 3, size=(steps, total), dtype=np.int32))
-    outs, out = [], None
-    for t in range(steps):
-        mine = env.scatter_actions(acts_all[t] if rank == 0 else None, like=torch.zeros(1))
-        out = env.local.step_host(mine.numpy(), out, render=t == steps - 1)
-        obs = env.gather_to_root(torch.as_tensor(out["obs"]))
-        rew = env.gather_to_root(torch.as_tensor(out["reward"]))
-        if rank == 0:
-            outs.append((obs.numpy().copy(), rew.numpy().copy()))
-    if rank == 0:
-        q.put(outs)
-    dist.barrier()
-    dist.destroy_process_group()
-
-
 def test_sharded_mixed_run_equals_single_process(hostsim_path):
-    import torch.multiprocessing as mp
-    from miniworld_b200.batched import BatchedMiniWorld
-    total, steps = 10, 8
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = 31500 + os.getpid() % 2000
-    procs = [ctx.Process(target=_sharded_worker, args=(r, 2, port, hostsim_path, total, steps, q)) for r in range(2)]
-    for p in procs:
-        p.start()
-    sharded = q.get(timeout=300)
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
-    env = BatchedMiniWorld(MIX[:4], total, domain_rand=True)     # default assignment: blocks of 3, 3, 2, 2
-    assert env.env_level.tolist() == [0, 0, 0, 1, 1, 1, 2, 2, 3, 3]
-    seed_reset(env, 1000 + np.arange(total))
-    acts_all = np.random.default_rng(5).integers(0, 3, size=(steps, total), dtype=np.int32)
-    out = None
-    for t in range(steps):
-        out = env.step_host(acts_all[t], out, render=t == steps - 1)
-        assert np.array_equal(out["reward"], sharded[t][1])
-    assert np.array_equal(out["obs"], sharded[-1][0]) and 0 < out["obs"].mean() < 255
+    env, start = run_sharded(dict(levels=MIX[:4], domain_rand=True), total=10, steps=8, port_base=31500)
+    assert start.tolist() == [0, 0, 0, 1, 1, 1, 2, 2, 3, 3]     # default assignment: blocks of 3, 3, 2, 2
     env.close()
 
 
