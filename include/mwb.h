@@ -287,7 +287,8 @@ int mwb_set_program(mwb_handle* h, const mwb_op* ops, int n);              /* lo
  * Each level has its own domain_rand: an env's reset draws (texture variants, sky and light, entity colours, agent
  * camera) follow the flag of the level it resets into, and its per-step draws the flag of its episode's level, so rows
  * that share a level definition but differ in the flag (and in their params' ranges) make a randomisation curriculum.
- * The flag is table data, not env state: snapshots do not carry it.
+ * The flag is table data, not env state: snapshots do not carry it.  The rows' params are the initial content of the
+ * params table, which the caller may rewrite while the batch runs (MWB_ARRAY_LEVEL_PARAMS).
  * Per-handle settings (observation size, MSAA, autoreset, action noise) apply to every level. */
 typedef struct mwb_level {
   int32_t rule_kind;         /* MWB_RULE_*                                                       */
@@ -417,7 +418,8 @@ int mwb_visible_ents(mwb_handle* h, uint32_t* mask, void* stream);
 int mwb_get_state(mwb_handle* h, const mwb_state_view* out);
 
 /* ---- checkpointing: the complete restorable state of all N envs (entity lists, counters, camera and
- * lighting parameters, numpy streams, pending auto-resets, geometry on the device) as one host blob.
+ * lighting parameters, numpy streams, pending auto-resets, geometry on the device, the level params table and each
+ * env's max_forward_step) as one host blob.
  * Restoring into a handle created with the same configuration and level definition resumes every env
  * bit for bit.  (The reference has no equivalent: its state lives in Python objects.)  The blob of a handle with
  * several levels also carries env_level; restoring it into a handle with another level count or assignment fails
@@ -477,6 +479,27 @@ int mwb_debug_camera(mwb_handle* h, float* out /* host [num_envs][16] */);
 #define MWB_ARRAY_ENV_LEVEL 6       /* int32   [num_envs]  level of each env's current episode                   */
 #define MWB_ARRAY_NEXT_LEVEL 7      /* int32   [num_envs]  pending assignment for the next reset, -1 = none      */
 #define MWB_ARRAY_LEVEL_WEIGHTS 8   /* float32 [n_levels]  sampling weights of the next resets                   */
+/* on every handle with device resets (params and a reset program set; MWB_ESTATE otherwise, e.g. for a handle whose
+ * envs only ever get host-generated worlds through mwb_set_world), with or without level changes: */
+#define MWB_ARRAY_LEVEL_PARAMS 9    /* mwb_params [n_levels]  each level's DomainParams, count = n_levels records   */
+/* MWB_ARRAY_LEVEL_PARAMS: the level table's DomainParams, which mwb_set_params / mwb_set_levels fill and which the
+ * caller may then rewrite in place while the batch runs (automatic domain randomisation: widen a range once the
+ * policy succeeds at its edge), stream-ordered like LEVEL_WEIGHTS: a write enqueued on the stream of the next
+ * mwb_step / mwb_reset is seen by it.  Level l's row is what MiniWorldEnv.params is to every env whose current episode
+ * runs level l (reference miniworld.py:576-585, 677-680), and when each field is read decides when a write applies:
+ *   - forward_step, forward_drift, turn_step (default, _lo, _rng): read by mwb_step at every step, so a write applies
+ *     from the next step of every env of the level, mid-episode included (domain_rand on: uniform(lo, lo + rng),
+ *     off: the default);
+ *   - sky_color, light_pos, light_color, light_ambient, obj_color_bias, cam_height, cam_fwd_disp, cam_pitch,
+ *     cam_fov_y: read only at resets, so a write applies from each env's next reset; a running episode keeps the
+ *     values it drew (mwb_state_view cam / env_params, entity colours);
+ *   - max_forward_step: read only at resets too.  Each env keeps the value its last reset took (self.max_forward_step,
+ *     miniworld.py:581) for its near() thresholds (1.1 * max_forward_step, :975) and the carry position (:611), so an
+ *     episode in progress keeps its threshold.  Whoever writes raw rows must keep it equal to forward_step's max
+ *     (forward_step_lo + forward_step_rng as the reference's params.get_max("forward_step") would return it).
+ * Every _rng must be the float64 difference max - min (numpy's uniform(low, high) is low + (high - low) * random(),
+ * with high - low rounded once).  The domain_rand flag stays table data.  A handle whose rows are never written runs
+ * exactly as before.  Snapshots carry the table and every env's max_forward_step, and a restore adopts both. */
 int mwb_state_array(mwb_handle* h, int which, void** dev_ptr, int64_t* count);
 /* 1 when this library keeps the handle's state arrays (mwb_state_array) in host memory -- the CPU build of the kernels
  * used by the test suite -- and 0 for libmwb.so, whose arrays are device memory. */

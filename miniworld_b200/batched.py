@@ -22,9 +22,11 @@ performs the same step with pinned host buffers for callers that want numpy.
 import numpy as np
 
 from . import pack
-from .engine import (Engine, LEVEL_CAP, OP_PLACE, OP_PUT, PROTO_DTYPE, RULE_GOAL, RULE_NONE, RULE_HEALTH, RULE_PICKUP,
-                     RULE_PUTNEXT, RULE_SIDEWALK, RULE_SIGN, generator_from_state, rng_state_of, RNG_DTYPE)
+from .engine import (Engine, LEVEL_CAP, LOWERED_PARAMS, OP_PLACE, OP_PUT, PARAMS_COLUMN, PROTO_DTYPE, RULE_GOAL,
+                     RULE_NONE, RULE_HEALTH, RULE_PICKUP, RULE_PUTNEXT, RULE_SIDEWALK, RULE_SIGN, generator_from_state,
+                     rng_state_of, RNG_DTYPE)
 from .envs import LEVELS
+from .params import DomainParams
 from .program import ResetProgram
 
 
@@ -168,7 +170,11 @@ class BatchedMiniWorld:
     `dynamic_levels=True` (with a sequence of levels) lets envs move between levels at their resets, never
     mid-episode: a pending assignment from `set_env_level` wins, otherwise the next level is drawn on the device from
     `level_weights` (all zero, the default, keeps every env on its level).  The draws are keyed by `level_seed` and
-    the env's global index `env_offset + i` (ShardedMiniWorld sets the offset), not by the env's own numpy stream."""
+    the env's global index `env_offset + i` (ShardedMiniWorld sets the offset), not by the env's own numpy stream.
+
+    A level's params (`level_kwargs` `params=`) are the initial content of a table that `set_level_param` /
+    `set_level_params` rewrite while the batch runs (automatic domain randomisation), as the reference's
+    `env.params.set(...)` does: step ranges apply from the next step, the rest from each env's next reset."""
 
     def __init__(self, level, num_envs, obs_width=80, obs_height=60, domain_rand=False, autoreset=True,
                  msaa_samples=8, device=0, want_depth=False, level_kwargs=None, obs_format="hwc", env_level=None,
@@ -208,6 +214,8 @@ class BatchedMiniWorld:
         self._seeded = False
         self._torch = None
         self._bufs = None
+        self._params_view = None
+        self._params_written = False
 
     def _init_level(self, level, level_kwargs):
         d = _define_level(level, level_kwargs, self.domain_rand, self.obs_width, self.obs_height)
@@ -427,6 +435,105 @@ class BatchedMiniWorld:
         view = self.level_tensor
         return np.array(view) if isinstance(view, np.ndarray) else view.cpu().numpy()
 
+    # ------------------------------------------------------------------ level params at run time
+    def _level_params(self):
+        """The device's params table as float64 [n_levels, words] (mwb_params records): a torch CUDA tensor, or a
+        numpy array on the kernels' host build."""
+        if not self.device_reset:
+            raise TypeError("level params change at device resets; host-reset levels draw theirs in Python "
+                            "(set them on the level's own DomainParams)")
+        if self._params_view is None:
+            view = self.engine.state_array("level_params")
+            if not self.engine.host_memory:
+                torch = self._ensure_torch()
+                view = torch.as_tensor(view, device=torch.device("cuda", self.device))
+            self._params_view = view
+        return self._params_view
+
+    def set_level_param(self, level, name, default=None, min=None, max=None):
+        """Change one DomainParams entry of level `level` while the batch runs (automatic domain randomisation).
+        `name` is one of the twelve params the engine reads (engine.LOWERED_PARAMS) and must be a float param.  As
+        with DomainParams.set, `min` and `max` default to `default`.  With `default` None the level keeps its default
+        and `min` and `max` set the range (both or neither).  Values are floats, sequences, numpy arrays or CUDA
+        tensors, of the param's shape (() or (3,)).
+        The write is a few torch ops on the current stream, with no host sync.  The next `step` of every env at that
+        level draws forward_step / forward_drift / turn_step from the new range, mid-episode included; everything
+        else applies from each env's next reset, `max_forward_step` too (it follows forward_step's max).  The range
+        is stored as min and max - min, computed in float64 as numpy's uniform() forms it.  Host values are checked
+        as DomainParams.set checks them (shapes, min <= default <= max); tensor values are not checked."""
+        if name not in LOWERED_PARAMS:
+            raise KeyError("%r is not a param the engine reads; these are: %s" % (name, ", ".join(LOWERED_PARAMS)))
+        n_levels = len(self.level_ids)
+        if isinstance(level, bool) or not (isinstance(level, (int, np.integer)) and 0 <= int(level) < n_levels):
+            raise ValueError("level must be an int in [0, %d), got %r" % (n_levels, level))
+        level = int(level)
+        view = self._level_params()
+        p = self.proto_envs[level].params.params[name]
+        if p.type != "float":
+            raise TypeError("%r of level %d is a %s param; only float params can be set" % (name, level, p.type))
+        if default is not None:
+            min, max = default if min is None else min, default if max is None else max
+        elif (min is None) != (max is None):
+            raise ValueError("%r: without a default, give both min and max (or neither)" % name)
+        given = {key: v for key, v in (("default", default), ("min", min), ("max", max)) if v is not None}
+        shape = np.shape(p.default)
+        for key, v in given.items():
+            got = tuple(v.shape) if hasattr(v, "shape") else np.shape(v)
+            if got != shape:
+                raise ValueError("%s of %r must have shape %s, got %s" % (key, name, shape, got))
+        host = {key: np.asarray(v, np.float64) for key, v in given.items() if not hasattr(v, "is_cuda")}
+        for a, b in (("min", "default"), ("default", "max"), ("min", "max")):
+            if a in host and b in host and not np.all(host[b] >= host[a]):
+                raise ValueError("%r: %s %s is above %s %s" % (name, a, host[a], b, host[b]))
+        if not given:
+            return
+        c, k = PARAMS_COLUMN[name], int(np.prod(shape, dtype=int))
+        cols = {"default": slice(c, c + k), "min": slice(c + k, c + 2 * k)}
+        if isinstance(view, np.ndarray):
+            vals = {key: np.asarray(v.cpu() if hasattr(v, "cpu") else v, np.float64).reshape(k)
+                    for key, v in given.items()}
+            sub = np.subtract
+        else:
+            torch = self._torch
+            vals = {key: torch.as_tensor(v, dtype=torch.float64).to(view.device, non_blocking=True).reshape(k)
+                    for key, v in given.items()}
+            sub = torch.sub
+            self._params_written = True
+        for key in ("default", "min"):
+            if key in vals:
+                view[level, cols[key]] = vals[key]
+        if "max" in vals:
+            view[level, c + 2 * k:c + 3 * k] = sub(vals["max"], vals["min"])
+            if name == "forward_step":
+                view[level, PARAMS_COLUMN["max_forward_step"]] = vals["max"].reshape(())
+
+    def set_level_params(self, level, params):
+        """Write every param of `params` (a DomainParams) that the engine reads into level `level`, as
+        `set_level_param` does; entries the engine does not read (bot_radius, tex_rand, ...) are ignored, as at
+        construction."""
+        for name in LOWERED_PARAMS:
+            if name in params.params:
+                p = params.params[name]
+                self.set_level_param(level, name, p.default, p.min, p.max)
+
+    def get_level_params(self, level):
+        """Level `level`'s params as the device has them now, as a DomainParams (synchronises with the device).  The
+        table holds min and max - min, so `max` is read back as min + (max - min), except forward_step's, which is
+        max_forward_step.  The entries the engine does not read are the level's construction values."""
+        view = self._level_params()
+        row = np.array(view[level] if isinstance(view, np.ndarray) else view[level].cpu().numpy())
+        out = DomainParams()
+        out.params = dict(self.proto_envs[level].params.params)
+        for name in LOWERED_PARAMS:
+            c = PARAMS_COLUMN[name]
+            k = int(np.prod(np.shape(out.params[name].default), dtype=int))
+            lo = row[c + k:c + 2 * k]
+            hi = row[PARAMS_COLUMN["max_forward_step"]:][:1] if name == "forward_step" else lo + row[c + 2 * k:c + 3 * k]
+            vals = [row[c:c + k], lo, hi]
+            vals = [np.array(v) if k == 3 else float(v[0]) for v in vals]
+            out.params[name] = DomainParams.DomainParam(vals[0], vals[1], vals[2], "float")
+        return out
+
     def _wrap(self, obs):
         """Observation / info as the level's own step() shapes them (Sign: {"obs", "goal"}, sign.py:176)."""
         torch = self._torch
@@ -554,17 +661,24 @@ class BatchedMiniWorld:
         self.engine.restore(blob)
         self._seeded = True
 
+    def _torch_writes(self):
+        """True when torch work may write arrays the kernels read: next_level / level_weights (level changes on) or the
+        params table (once set_level_param has written it)."""
+        return (self.dynamic_levels or self._params_written) and not self.engine.host_memory
+
     def _level_stream(self):
-        """Stream for a call whose resets read next_level / level_weights: with level changes on, torch's current
-        stream, so that the resets run behind the torch work that wrote those arrays (set_env_level, set_level_weights,
-        in-place writes); otherwise None, the handle's own stream.  Calls with host outputs still return finished."""
-        if self.dynamic_levels and not self.engine.host_memory:
+        """Stream for a call whose steps and resets read next_level / level_weights or the params table: when torch
+        writes them, torch's current stream, so that the kernels run behind the torch work that wrote those arrays
+        (set_env_level, set_level_weights, set_level_param, in-place writes); otherwise None, the handle's own stream.
+        Calls with host outputs still return finished."""
+        if self._torch_writes():
             return _torch_stream(self._ensure_torch(), self.device)
         return None
 
     def _sync_level_writes(self):
-        """Finish torch writes to next_level / level_weights before the handle's own stream reads or replaces them."""
-        if self.dynamic_levels and not self.engine.host_memory:
+        """Finish torch writes to next_level / level_weights / the params table before the handle's own stream reads
+        or replaces them."""
+        if self._torch_writes():
             self._ensure_torch().cuda.current_stream(self.device).synchronize()
 
     def set_action_noise(self, prob=0.9, random_action=None):

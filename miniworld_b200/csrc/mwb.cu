@@ -125,6 +125,7 @@ struct mwb_handle {
   bool have_level_table;          // mwb_set_levels succeeded (mwb_enable_level_changes needs it)
   // level table (host copies of S.levels / S.env_level / S.ops); a handle that never calls mwb_set_levels has one level
   std::vector<LevelDev> levels;
+  std::vector<mwb_params> params_h;   // the params table as mwb_set_params / mwb_set_levels gave it (S.level_params)
   std::vector<int32_t> env_level;
   std::vector<mwb_op> ops_h;
   int geom_blocks;                // blocks the geometry arrays hold: N (per-env worlds) or at least levels.size()
@@ -243,8 +244,9 @@ MWB_DEV void step_one(const DevState& S, int i, const int32_t* actions, const do
       MWB_WARP_SYNC();
     }
     double fs, fd, ts;
-    const LevelDev& L = env_level_of(S, i);   // the level of this episode: its params and its domain_rand
-    const mwb_params& P = L.params;
+    // the level of this episode: its domain_rand, and its step ranges as they stand at this step
+    const LevelDev& L = env_level_of(S, i);
+    const mwb_params& P = env_params_of(S, i);
     if (step_params) {
       fs = step_params[i * 3 + 0];
       fd = step_params[i * 3 + 1];
@@ -290,6 +292,7 @@ MWB_DEV void scatter_one(const DevState& S, const WorldUpload& u) {
   S.ghost_slot[i] = -1;
   for (int k = 0; k < 4; ++k) S.cam[k * N + i] = u.cam[k];
   for (int k = 0; k < 12; ++k) S.envp[k * N + i] = u.envp[k];
+  S.env_mfs[i] = S.level_params[S.env_level[i]].max_forward_step;   // a host reset takes it like a device one
   for (int e = 0; e < S.E; ++e) {
     const bool live = e < u.num_slots && e < MWB_MAX_ENTS_CAP;
     S.ent_proto[e * N + i] = live ? u.ents[e].proto : -1;
@@ -740,7 +743,8 @@ extern "C" int mwb_create(const mwb_config* cfg, mwb_handle** out) {
 #define AL(field, count) if (!rc) rc = alloc_arr(h, &S.field, (count))
   AL(ent_proto, E * N); AL(ent_px, E * N); AL(ent_py, E * N); AL(ent_pz, E * N); AL(ent_dir, E * N);
   AL(ent_col, E * 3 * N); AL(ent_size, E * N); AL(num_slots, N); AL(agent_slot, N); AL(carrying, N); AL(step_count, N);
-  AL(num_picked, N); AL(needs_reset, N); AL(episodes_done, 1); AL(cam, 4 * N); AL(envp, 12 * N); AL(ghost_slot, N);
+  AL(num_picked, N); AL(needs_reset, N); AL(episodes_done, 1); AL(cam, 4 * N); AL(envp, 12 * N); AL(env_mfs, N);
+  AL(ghost_slot, N);
   AL(ghost_proto, N); AL(ghost_pose, 4 * N); AL(ghost_col, 3 * N);
   AL(rng_s_hi, N); AL(rng_s_lo, N); AL(rng_inc_hi, N); AL(rng_inc_lo, N); AL(rng_has32, N); AL(rng_cache, N);
   AL(num_rooms, G); AL(num_quads, G); AL(num_segs, G);
@@ -748,10 +752,13 @@ extern "C" int mwb_create(const mwb_config* cfg, mwb_handle** out) {
   AL(mesh_seg, N * E); AL(cam_trig, 6 * N); AL(ent_cs, E * 2 * N);
 #undef AL
   LevelDev* d_levels = nullptr;
+  mwb_params* d_level_params = nullptr;
   int32_t* d_env_level = nullptr;
   if (!rc) rc = alloc_arr(h, &d_levels, MWB_LEVEL_CAP);
+  if (!rc) rc = alloc_arr(h, &d_level_params, MWB_LEVEL_CAP);
   if (!rc) rc = alloc_arr(h, &d_env_level, N);      // zeros: every env runs level 0
   S.levels = d_levels;
+  S.level_params = d_level_params;
   S.env_level = d_env_level;
   if (!rc) rc = alloc_arr(h, &h->d_actions, N);
   if (!rc) rc = alloc_arr(h, &h->d_step_params, 3 * N);
@@ -1115,15 +1122,28 @@ static int upload_ops(mwb_handle* h) {
   return MWB_OK;
 }
 
-static void set_level_params(LevelDev& L, const mwb_params& p) {
-  L.params = p;
-  L.near_extra = 1.1 * p.max_forward_step;
+// the host copy of the level params -> S.level_params, and every env's max_forward_step from its level's row (the
+// table's initial content: from here on only the caller's in-place writes, resets and restores change them)
+static int upload_params(mwb_handle* h) {
+  int rc = drain(h);
+  if (rc) return rc;
+  const DevState& S = h->S;
+  rc |= h2d((void*)S.level_params, h->params_h.data(), h->params_h.size() * sizeof(mwb_params), h->stream);
+  std::vector<double> mfs((size_t)S.N);
+  if (!S.next_level) {
+    for (int i = 0; i < S.N; ++i) mfs[i] = h->params_h[h->env_level[i]].max_forward_step;
+    rc |= h2d(S.env_mfs, mfs.data(), mfs.size() * sizeof(double), h->stream);
+  }
+  rc |= sync_stream(h->stream);
+  return rc ? fail(MWB_ECUDA, "level params upload failed") : MWB_OK;
 }
 
 extern "C" int mwb_set_params(mwb_handle* h, const mwb_params* p) {
   if (!h || !p) return fail(MWB_EINVAL, "null argument");
-  set_level_params(h->levels[0], *p);
+  h->params_h.resize(h->levels.size());
+  h->params_h[0] = *p;
   int rc = upload_levels(h);
+  if (!rc) rc = upload_params(h);
   if (rc) return rc;
   h->have_params = true;
   return MWB_OK;
@@ -1268,10 +1288,11 @@ extern "C" int mwb_set_levels(mwb_handle* h, int n_levels, const mwb_level* leve
   for (int l = 0; l < n_levels && !rc; ++l) rc = upload_geometry(h, (size_t)l, &templates[l]);
   if (rc) return rc;
   h->levels.resize(n_levels);
+  h->params_h.resize(n_levels);
   for (int l = 0; l < n_levels; ++l) {
     LevelDev& D = h->levels[l];
     memset(&D, 0, sizeof(D));
-    set_level_params(D, levels[l].params);
+    h->params_h[l] = levels[l].params;
     D.rule_kind = levels[l].rule_kind;
     D.rule_arg = levels[l].rule_arg;
     D.max_episode_steps = levels[l].max_episode_steps;
@@ -1286,6 +1307,7 @@ extern "C" int mwb_set_levels(mwb_handle* h, int n_levels, const mwb_level* leve
   h->ops_h.assign(ops, ops + n_ops);
   rc = upload_ops(h);
   if (!rc) rc = upload_levels(h);
+  if (!rc) rc = upload_params(h);
   if (rc) return rc;
   h->S.num_levels = n_levels;
   h->have_params = h->have_template = true;
@@ -2050,6 +2072,8 @@ static void snapshot_arrays(mwb_handle* h, std::vector<std::pair<void*, size_t>>
   SA(rng_s_hi, N); SA(rng_s_lo, N); SA(rng_inc_hi, N); SA(rng_inc_lo, N); SA(rng_has32, N); SA(rng_cache, N);
   SA(num_rooms, G); SA(num_quads, G); SA(num_segs, G);
   SA(rooms, G * S.R); SA(quads, G * S.Q); SA(segs, G * S.S); SA(room_tex, N * S.R * 3);
+  // the level ranges are run-time state (MWB_ARRAY_LEVEL_PARAMS), and so is what each env's last reset took from them
+  SA(env_mfs, N); SA(level_params, h->levels.size());
 #undef SA
 }
 
@@ -2226,6 +2250,12 @@ extern "C" int mwb_state_array(mwb_handle* h, int which, void** dev_ptr, int64_t
       if (which == MWB_ARRAY_ENV_LEVEL) { *dev_ptr = h->S.env_level; *count = N; }                       // int32 [N]
       else if (which == MWB_ARRAY_NEXT_LEVEL) { *dev_ptr = h->S.next_level; *count = N; }                // int32 [N]
       else { *dev_ptr = (void*)h->S.level_weights; *count = h->S.num_levels; }                           // float32 [L]
+      break;
+    case MWB_ARRAY_LEVEL_PARAMS:
+      if (!h->have_params || !h->S.ops)
+        return fail(MWB_ESTATE, "the handle has no device resets (params and a reset program: mwb_set_levels, or "
+                                "mwb_set_params and mwb_set_program); host-generated worlds carry their own draws");
+      *dev_ptr = (void*)h->S.level_params; *count = (int64_t)h->levels.size();                            // mwb_params [L]
       break;
     default: return fail(MWB_EINVAL, "unknown array");
   }

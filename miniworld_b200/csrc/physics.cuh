@@ -108,7 +108,7 @@ struct CarryPos {
 // _get_carry_pos(agent_pos, ent): agent_pos + dir_vec * 1.05 * dist, lifted to stay visible
 MWB_DEV CarryPos carry_pos(const DevState& S, int i, double apx, double apz, double c, double s, int slot, double ar) {
   const EntDims pr = ent_dims(S, i, slot, S.protos[S.ent_proto[(size_t)slot * S.N + i]]);
-  const double mfs = env_level_of(S, i).params.max_forward_step;
+  const double mfs = S.env_mfs[i];   // self.max_forward_step, taken at the env's last reset
   double dist;   // agent.radius + ent.radius + max_forward_step, float32 as soon as ent.radius is
   if (pr.f32)
     dist = (double)f_add(f_add((float)ar, (float)pr.radius), (float)mfs);
@@ -181,7 +181,7 @@ MWB_DEV bool near_agent(const DevState& S, int i, int b, int as, double ar) {
   const double dz = d_sub(S.ent_pz[b * N + i], S.ent_pz[as * N + i]);
   const double d = d_sqrt(d_fma(dz, dz, d_fma(dy, dy, d_mul(dx, dx))));
   const EntDims pr = ent_dims(S, i, b, S.protos[bp]);
-  return d < near_threshold(pr.radius, pr.f32, ar, false, env_level_of(S, i).near_extra);
+  return d < near_threshold(pr.radius, pr.f32, ar, false, d_mul(1.1, S.env_mfs[i]));
 }
 
 // MiniWorldEnv.near(ent0, ent1) between two entities of the list
@@ -194,7 +194,7 @@ MWB_DEV bool near_pair(const DevState& S, int i, int a, int b) {
   const double dz = d_sub(S.ent_pz[a * N + i], S.ent_pz[b * N + i]);
   const double d = d_sqrt(d_fma(dz, dz, d_fma(dy, dy, d_mul(dx, dx))));
   const EntDims da = ent_dims(S, i, a, S.protos[pa]), db = ent_dims(S, i, b, S.protos[pb]);
-  return d < near_threshold(da.radius, da.f32, db.radius, db.f32, env_level_of(S, i).near_extra);
+  return d < near_threshold(da.radius, da.f32, db.radius, db.f32, d_mul(1.1, S.env_mfs[i]));
 }
 
 struct StepOut {

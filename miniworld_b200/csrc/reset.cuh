@@ -81,7 +81,7 @@ MWB_DEV void device_reset(const DevState& S, int i) {
   // the resolved level decides everything below, its domain_rand included: a reset that switches levels draws by the
   // new level's flag (read at each use: the row's address is live anyway, a cached copy would cost step_kernel a spill)
   const LevelDev& L = S.levels[lvl];
-  const mwb_params& P = L.params;
+  const mwb_params& P = S.level_params[lvl];   // the level's ranges as they stand at this reset
   const mwb_op* ops = S.ops + L.op_first;
   const int num_ops = L.num_ops;
   // the geometry of the level this episode runs: the env's own world (regenerated below by a Maze program) or the
@@ -104,6 +104,8 @@ MWB_DEV void device_reset(const DevState& S, int i) {
   S.cam[1 * N + i] = P.cam_fwd_disp;
   S.cam[2 * N + i] = P.cam_pitch;
   S.cam[3 * N + i] = P.cam_fov_y;
+  // self.max_forward_step = params.get_max("forward_step") (miniworld.py:581): the episode keeps it
+  S.env_mfs[i] = P.max_forward_step;
 
   int ireg[8];
   double freg[8];

@@ -26,10 +26,9 @@ struct TriRec;
 struct MeshSegInfo;
 struct MazeDev;
 
-// One row of the level table (mwb_set_levels): what K1 reads per env instead of per handle.
+// One row of the level table (mwb_set_levels): what K1 reads per env instead of per handle.  The row's DomainParams
+// live apart from it, in DevState::level_params, which callers may rewrite while the batch runs.
 struct LevelDev {
-  mwb_params params;
-  double near_extra;            // 1.1 * max_forward_step
   int32_t rule_kind, rule_arg;
   int32_t max_episode_steps;
   int32_t op_first, num_ops;    // slice of DevState::ops
@@ -65,6 +64,8 @@ struct DevState {
                                 //     out of room / quad / segment capacity (mwb_overflow_count; must stay 0)
   double* cam;                  // [4][N]  cam_height, cam_fwd_disp, cam_pitch, cam_fov_y
   double* envp;                 // [12][N] sky_color, light_pos, light_color, light_ambient
+  double* env_mfs;              // [N] max_forward_step the env's last reset took (miniworld.py:581): near() and the
+                                //     carry position read it, so an episode keeps it when its level's ranges change
   // object removed by the level rule AFTER this step's observation (pickupobjects.py:86-90)
   int32_t* ghost_slot;          // [N] -1 = none
   int32_t* ghost_proto;         // [N]
@@ -112,7 +113,9 @@ struct DevState {
   const mwb_proto* protos;      // shared by all levels
   int32_t num_protos;
   const mwb_op* ops;            // every level's reset program, one after another
-  const LevelDev* levels;       // [levels] rule, truncation, params, program slice
+  const LevelDev* levels;       // [levels] rule, truncation, program slice
+  const mwb_params* level_params;   // [levels] DomainParams of each level (MWB_ARRAY_LEVEL_PARAMS: writable in place,
+                                    //   stream-ordered); K1 reads the step ranges per step, the rest at resets
   int32_t* env_level;           // [N] level of each env (all 0 on a one-level handle); with level changes on, the
                                 //     resets rewrite it (device_reset: resolve_level)
   int32_t num_levels;
@@ -133,6 +136,7 @@ struct DevState {
 MWB_DEV int geom_block(const DevState& S, int i, int lvl) { return S.levels[lvl].env_worlds ? S.env_geom + i : lvl; }
 MWB_DEV int geom_index(const DevState& S, int i) { return geom_block(S, i, S.env_level[i]); }
 MWB_DEV const LevelDev& env_level_of(const DevState& S, int i) { return S.levels[S.env_level[i]]; }
+MWB_DEV const mwb_params& env_params_of(const DevState& S, int i) { return S.level_params[S.env_level[i]]; }
 
 MWB_DEV NpRng load_rng(const DevState& S, int i) {
   NpRng r;

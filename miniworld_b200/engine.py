@@ -47,6 +47,12 @@ class Params(C.Structure):
                 [("max_forward_step", C.c_double)])
 
 
+LOWERED_PARAMS = _VEC_PARAMS + _SCALAR_PARAMS     # the DomainParams entries the engine reads
+PARAMS_DOUBLES = C.sizeof(Params) // 8
+# field of mwb_params -> its column in a float64 view of the params table
+PARAMS_COLUMN = {name: getattr(Params, name).offset // 8 for name, _ in Params._fields_}
+
+
 class TexDesc(C.Structure):
     _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("offset", C.c_int64)]
 
@@ -544,26 +550,31 @@ class Engine:
         """uint32[N] (numpy or CUDA tensor): bit e = entity slot e passes the reference's occlusion query."""
         self._check(self.lib.mwb_visible_ents(self.h, _dev_or_host_ptr(mask), stream))
 
-    # name -> (mwb_state_array id, element type, leading axis: "env" = [N] or [k, N], "level" = [n_levels])
+    # name -> (mwb_state_array id, element type, leading axis: "env" = [N] or [k, N], "level" = [n_levels],
+    # "params" = [n_levels, PARAMS_DOUBLES] mwb_params records as float64 words)
     ARRAYS = {"counter": (0, "<i4", "env"), "step_count": (1, "<i4", "env"), "ent_x": (2, "<f8", "env"),
               "ent_y": (3, "<f8", "env"), "ent_z": (4, "<f8", "env"), "ent_dir": (5, "<f8", "env"),
-              "env_level": (6, "<i4", "env"), "next_level": (7, "<i4", "env"), "level_weights": (8, "<f4", "level")}
+              "env_level": (6, "<i4", "env"), "next_level": (7, "<i4", "env"), "level_weights": (8, "<f4", "level"),
+              "level_params": (9, "<f8", "params")}
 
     def state_array(self, name):
         """Zero-copy view of a state array (mwb_state_array) as an object with __cuda_array_interface__:
         "counter" / "step_count" int32 [N]; "ent_x|y|z|dir" float64 [max_ents, N]; with level changes on,
-        "env_level" / "next_level" int32 [N] and "level_weights" float32 [n_levels].  On the host build of the
-        kernels the arrays live in host memory, and the view is a numpy array over the same memory instead."""
+        "env_level" / "next_level" int32 [N] and "level_weights" float32 [n_levels]; with device resets,
+        "level_params" float64 [n_levels, PARAMS_DOUBLES] (column of a field: PARAMS_COLUMN).  On the host build of
+        the kernels the arrays live in host memory, and the view is a numpy array over the same memory instead."""
         which, typestr, axis = self.ARRAYS[name]
         ptr, count = C.c_void_p(), C.c_int64()
         self._check(self.lib.mwb_state_array(self.h, which, C.byref(ptr), C.byref(count)))
-        if axis == "level" or count.value == self.N:
+        if axis == "params":
+            shape = (count.value, PARAMS_DOUBLES)
+        elif axis == "level" or count.value == self.N:
             shape = (count.value,)
         else:
             shape = (count.value // self.N, self.N)
         if self.host_memory:
             dt = np.dtype(typestr)
-            buf = (C.c_char * (count.value * dt.itemsize)).from_address(ptr.value)
+            buf = (C.c_char * (int(np.prod(shape)) * dt.itemsize)).from_address(ptr.value)
             return np.frombuffer(buf, dt).reshape(shape)
 
         class _View:
