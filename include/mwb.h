@@ -329,6 +329,46 @@ int mwb_set_levels(mwb_handle* h, int n_levels, const mwb_level* levels, const m
  * changes are on / off while the blob's were off / on fails with MWB_ESTATE. */
 int mwb_enable_level_changes(mwb_handle* h, uint64_t seed, int32_t env_offset /* global index of env 0, >= 0 */);
 
+/* Episode seeds (level replay: restart an env on a chosen seed when its episode ends, and know which seed every
+ * finished episode ran).  Stands in for env.reset(seed=s) of the reference (gymnasium seeds self.np_random with
+ * Generator(PCG64(SeedSequence(s))), miniworld.py:551), decided per env on the device instead of by a host call.
+ * Valid on a handle with device resets (params and a reset program set: mwb_set_levels, or mwb_set_params and
+ * mwb_set_program; MWB_ESTATE otherwise, since host-generated worlds keep their streams on the host, and when already
+ * on).  It needs neither a level table nor level changes.  It allocates next_seed int64 [N] and episode_seed int64 [N],
+ * both all -1, which the caller reads and writes in place through mwb_state_array (MWB_ARRAY_NEXT_SEED /
+ * MWB_ARRAY_EPISODE_SEED), stream-ordered, without a sync.
+ *
+ * A seed is taken only at a reset: mwb_reset, and the next-step auto-reset inside mwb_step.  At every reset of env i,
+ * before anything is drawn:
+ *   1. if next_seed[i] >= 0: the env's numpy stream is replaced by the one SeedSequence(next_seed[i]) starts,
+ *      episode_seed[i] = next_seed[i], and next_seed[i] is cleared to -1;
+ *   2. otherwise the env continues its stream and episode_seed[i] = -1 (any negative next_seed counts as -1 and is
+ *      cleared).
+ * So env i then equals, bit for bit, a fresh env of its level after reset(seed=s): what mwb_seed with
+ * bit_generator.state of Generator(PCG64(SeedSequence(s))) followed by mwb_reset gives.  With level changes on, the
+ * level is resolved as before (the level draw never touches the env's stream): a reset that takes a pending level and
+ * a pending seed equals a fresh env of the new level after reset(seed=s).  episode_seed names the running episode; after
+ * a terminating step it still names the episode that ended, because the reset happens inside the next step.
+ * The stream of seed s, 0 <= s < 2^63, all 32-bit values mod 2^32:
+ *   entropy  = (s & 0xFFFFFFFF, s >> 32, 0, 0)       (SeedSequence pads the pool's input with zeros, so [s] for
+ *                                                     s < 2^32 and [low, high] otherwise are both this)
+ *   hashmix(v):  v ^= hc;  hc *= 0x931e8875;  v *= hc;  v ^= v >> 16      (hc starts at 0x43b0d7e5 and carries on
+ *                                                                          through every call below)
+ *   mix(x, y):   r = 0xca01f9dd * x - 0x4973f715 * y;  r ^= r >> 16
+ *   pool[k]  = hashmix(entropy[k])                    for k = 0..3
+ *   for src = 0..3, for dst = 0..3, src != dst:  pool[dst] = mix(pool[dst], hashmix(pool[src]))
+ *   w[k]     = pool[k % 4] ^ hc';  hc' *= 0x58f38ded;  w[k] *= hc';  w[k] ^= w[k] >> 16      for k = 0..7,
+ *              hc' starting at 0x8b51f9dd
+ *   q[k]     = w[2k] | w[2k + 1] << 32                for k = 0..3 (uint64)
+ *   inc      = (q[2] << 64 | q[3]) << 1 | 1           (mod 2^128)
+ *   state    = 0;  state = state * M + inc;  state += q[0] << 64 | q[1];  state = state * M + inc
+ *              (M = 0x2360ED051FC65DA44385DF649FCCF645);  has_uint32 = 0, uinteger = 0
+ * Handles that never call this behave exactly as before it existed, and the addition changes no struct and no existing
+ * entry point, so MWB_ABI_VERSION stays as it is and blobs of such handles restore as before.  Snapshots of a handle with episode seeds on carry
+ * both arrays, are marked as such in the header, and a restore adopts them; restoring a blob into a handle whose
+ * episode seeds are on / off while the blob's were off / on fails with MWB_ESTATE before anything else is compared. */
+int mwb_enable_episode_seeds(mwb_handle* h);
+
 /* Maze level (reference envs/maze.py): every episode's world is a translate-and-select of these
  * templates -- one grid cell and one connector room per neighbour direction, in the order of
  * maze.py:110 `orders = [(0, 1), (0, -1), (-1, 0), (1, 0)]` as (dj, di).  All records are for
@@ -425,7 +465,7 @@ int mwb_get_state(mwb_handle* h, const mwb_state_view* out);
  * several levels also carries env_level; restoring it into a handle with another level count or assignment fails
  * with MWB_ESTATE (handles with level changes on: see mwb_enable_level_changes; their blobs are marked as such in the
  * header, and a blob whose mark differs from the handle's mode is refused with MWB_ESTATE before anything else is
- * compared). */
+ * compared; the same holds for episode seeds, mwb_enable_episode_seeds). */
 int mwb_snapshot_size(mwb_handle* h, size_t* bytes);
 int mwb_snapshot(mwb_handle* h, void* blob, size_t bytes);
 int mwb_restore(mwb_handle* h, const void* blob, size_t bytes);
@@ -500,6 +540,10 @@ int mwb_debug_camera(mwb_handle* h, float* out /* host [num_envs][16] */);
  * Every _rng must be the float64 difference max - min (numpy's uniform(low, high) is low + (high - low) * random(),
  * with high - low rounded once).  The domain_rand flag stays table data.  A handle whose rows are never written runs
  * exactly as before.  Snapshots carry the table and every env's max_forward_step, and a restore adopts both. */
+/* with episode seeds on (mwb_enable_episode_seeds; MWB_ESTATE otherwise); ids 10 to 15 stay unknown (MWB_EINVAL), free
+ * for further level-table arrays: */
+#define MWB_ARRAY_NEXT_SEED 16      /* int64   [num_envs]  seed of the env's next reset, negative = none           */
+#define MWB_ARRAY_EPISODE_SEED 17   /* int64   [num_envs]  seed the env's current episode started from, or -1    */
 int mwb_state_array(mwb_handle* h, int which, void** dev_ptr, int64_t* count);
 /* 1 when this library keeps the handle's state arrays (mwb_state_array) in host memory -- the CPU build of the kernels
  * used by the test suite -- and 0 for libmwb.so, whose arrays are device memory. */

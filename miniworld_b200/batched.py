@@ -14,7 +14,9 @@ Per-environment semantics are exactly those of the reference's `MiniWorldEnv.res
   * `autoreset=True` gives Gymnasium "next-step" auto-reset: the step after a
     terminated|truncated step resets that env (action ignored, reward 0);
   * with several levels and `dynamic_levels=True`, an env's level can change at its resets:
-    pending assignments (`set_env_level`) and device-side draws from `level_weights`.
+    pending assignments (`set_env_level`) and device-side draws from `level_weights`;
+  * with `episode_seeds=True`, an env's next reset can start from a chosen seed (`next_seed`, `set_env_seed`),
+    seeded on the device as `reset(seed=s)` would, and `info["seed"]` names the seed of each running episode.
 
 Outputs are torch CUDA tensors by default (zero-copy from the kernels); `step_host`
 performs the same step with pinned host buffers for callers that want numpy.
@@ -174,11 +176,17 @@ class BatchedMiniWorld:
 
     A level's params (`level_kwargs` `params=`) are the initial content of a table that `set_level_param` /
     `set_level_params` rewrite while the batch runs (automatic domain randomisation), as the reference's
-    `env.params.set(...)` does: step ranges apply from the next step, the rest from each env's next reset."""
+    `env.params.set(...)` does: step ranges apply from the next step, the rest from each env's next reset.
+
+    `episode_seeds=True` (one level or a table; levels that reset on the device) decides which episode of its level an
+    env plays, for level replay: a seed written to `next_seed[i]` (`set_env_seed`) is consumed by env i's next reset,
+    the auto-reset inside `step` included, which then starts the stream `reset(seed=s)` would, built on the device.
+    `episode_seed` / `info["seed"]` hold the seed each running episode started from, or -1 when the env continued its
+    stream; after a terminating step they still name the episode that just ended."""
 
     def __init__(self, level, num_envs, obs_width=80, obs_height=60, domain_rand=False, autoreset=True,
                  msaa_samples=8, device=0, want_depth=False, level_kwargs=None, obs_format="hwc", env_level=None,
-                 dynamic_levels=False, level_seed=0, env_offset=0, per_env_worlds=False):
+                 dynamic_levels=False, level_seed=0, env_offset=0, per_env_worlds=False, episode_seeds=False):
         self.num_envs = int(num_envs)
         self.obs_width, self.obs_height = int(obs_width), int(obs_height)
         self.domain_rand = bool(domain_rand)
@@ -186,6 +194,7 @@ class BatchedMiniWorld:
         self.device = int(device)
         self.dynamic_levels = bool(dynamic_levels)
         self.per_env_worlds = bool(per_env_worlds)
+        self.episode_seeds = bool(episode_seeds)
         table = isinstance(level, (list, tuple))
         if table:
             defs = self._init_levels(list(level), level_kwargs, env_level)
@@ -203,6 +212,12 @@ class BatchedMiniWorld:
         if self.dynamic_levels:
             self.level_seed, self.env_offset = int(level_seed), int(env_offset)
             self.engine.enable_level_changes(self.level_seed, self.env_offset)
+        self._seed_views = None
+        if self.episode_seeds:
+            if not self.device_reset:
+                self.engine.close()
+                raise TypeError("episode seeds are taken by device resets; host-reset levels keep RNG streams in Python")
+            self.engine.enable_episode_seeds()
         # observation layout written by the render kernel: the reference's PyTorchObsWrapper ("cwh") and
         # GreyscaleWrapper ("grey") are fused into its epilogue instead of running as separate passes
         self.obs_format = obs_format
@@ -360,6 +375,9 @@ class BatchedMiniWorld:
             if self.dynamic_levels:
                 # the level of each env's current episode (after a terminating step still the one that just ended)
                 self._info["level"] = self.level_tensor
+            if self.episode_seeds:
+                # the seed each env's current episode started from (after a terminating step still the ended one's)
+                self._info["seed"] = self.episode_seed
         return self._torch
 
     # ------------------------------------------------------------------ level changes (dynamic_levels=True)
@@ -434,6 +452,74 @@ class BatchedMiniWorld:
             return self._env_level
         view = self.level_tensor
         return np.array(view) if isinstance(view, np.ndarray) else view.cpu().numpy()
+
+    # ------------------------------------------------------------------ episode seeds (episode_seeds=True)
+    def _seeds(self):
+        """next_seed / episode_seed in place, made like `_views`: torch CUDA tensors, or numpy arrays on the kernels'
+        host build."""
+        if not self.episode_seeds:
+            raise RuntimeError("this batch has no episode seeds: construct it with episode_seeds=True")
+        if self._seed_views is None:
+            names = ("next_seed", "episode_seed")
+            if self.engine.host_memory:
+                self._seed_views = {n: self.engine.state_array(n) for n in names}
+            else:
+                import torch
+                dev = torch.device("cuda", self.device)
+                self._seed_views = {n: torch.as_tensor(self.engine.state_array(n), device=dev) for n in names}
+        return self._seed_views
+
+    @property
+    def next_seed(self):
+        """int64 [N] view of the seed each env's next reset starts from; write it in place (stream-ordered, no sync).
+        A negative entry means none: the env continues its stream.  The reset that takes an entry clears it to -1."""
+        return self._seeds()["next_seed"]
+
+    @property
+    def episode_seed(self):
+        """int64 [N] view of the seed each env's current episode started from, -1 when it continued its stream."""
+        return self._seeds()["episode_seed"]
+
+    def set_env_seed(self, env_ids, seeds):
+        """Start the listed envs' next episodes from `seeds` (one seed, or one per env), as `reset(seed=s)` would; envs
+        in mid-episode finish it first.  An env listed more than once takes its last entry.  `seeds` given as a CUDA
+        tensor are written as they are (a negative entry means none); host values must lie in [0, 2**63)."""
+        view = self.next_seed
+        on_device = hasattr(seeds, "is_cuda") and seeds.is_cuda
+        ids = np.atleast_1d(np.asarray(env_ids.cpu() if hasattr(env_ids, "cpu") else env_ids))
+        if not np.issubdtype(ids.dtype, np.integer):
+            raise ValueError("set_env_seed takes integer env ids")
+        if ids.size and (ids.min() < 0 or ids.max() >= self.num_envs):
+            raise ValueError("env ids must lie in [0, %d)" % self.num_envs)
+        if not on_device:
+            seeds = self._host_seeds(seeds.cpu().numpy() if hasattr(seeds, "cpu") else seeds, ids.shape)
+        elif seeds.dim() and tuple(seeds.shape) != ids.shape:
+            raise ValueError("set_env_seed: %d env ids but %d seeds" % (ids.size, seeds.numel()))
+        if ids.size == 0:
+            return
+        last = ids.size - 1 - np.unique(ids[::-1], return_index=True)[1]    # an env listed twice: its last entry wins
+        if isinstance(view, np.ndarray):
+            view[ids[last]] = seeds[last]
+        else:
+            torch = self._ensure_torch()
+            to_dev = lambda a: torch.as_tensor(a, dtype=torch.int64).to(view.device, non_blocking=True)
+            s = seeds.to(torch.int64) if on_device else to_dev(seeds)
+            view[to_dev(ids[last].astype(np.int64))] = s[to_dev(last)] if s.dim() else s
+
+    @staticmethod
+    def _host_seeds(seeds, shape):
+        """Host seeds (an int, or one per env) as int64 of `shape`, checked to lie in [0, 2**63)."""
+        arr = np.asarray(seeds)
+        if arr.dtype.kind not in "iu":
+            arr = np.array([int(v) for v in np.asarray(seeds, object).reshape(-1)], object).reshape(np.shape(seeds))
+        if arr.size and (arr.min() < 0 or arr.max() >= 2 ** 63):
+            raise ValueError("episode seeds must lie in [0, 2**63)")
+        arr = arr.astype(np.int64)
+        if np.ndim(seeds) == 0:
+            return np.broadcast_to(arr.reshape(()), shape)
+        if arr.shape != tuple(shape):
+            raise ValueError("%d env ids but %d seeds" % (int(np.prod(shape)), arr.size))
+        return arr
 
     # ------------------------------------------------------------------ level params at run time
     def _level_params(self):
@@ -547,8 +633,18 @@ class BatchedMiniWorld:
     # ------------------------------------------------------------------ reset
     def reset(self, seed=None, env_ids=None):
         """Reset all (or the listed) envs.  `seed`: int base (env i gets seed + i), a sequence
-        of per-env seeds, or None to continue each env's stream.  Returns (obs, info)."""
+        of per-env seeds, or None to continue each env's stream.  Returns (obs, info).
+        With `episode_seeds=True`, `seed` may also be a CUDA int64 tensor (one seed per reset env): the seeds are
+        queued in `next_seed` and the reset builds the streams on the device, without a sync.  Host seeds in
+        [0, 2**63) go the same way, so that `episode_seed` records them; the streams are the same either way."""
         ids = np.arange(self.num_envs, dtype=np.int32) if env_ids is None else np.asarray(env_ids, np.int32)
+        if self.episode_seeds and hasattr(seed, "is_cuda") and seed.is_cuda:
+            if tuple(seed.shape) != ids.shape:
+                raise ValueError("reset: %d envs but seeds of shape %s" % (ids.size, tuple(seed.shape)))
+            self.set_env_seed(ids, seed)
+            self.engine.reset(None if env_ids is None else ids, stream=self._level_stream())
+            self._seeded = True
+            return self._wrap(self.render()), {}
         if seed is not None:
             seeds = [int(seed) + int(i) for i in ids] if np.isscalar(seed) else [int(s) for s in seed]
             assert len(seeds) == len(ids)
@@ -557,7 +653,9 @@ class BatchedMiniWorld:
             if not self._seeded:
                 seeds = [int(s) for s in np.random.SeedSequence().generate_state(len(ids))]
         if self.device_reset:
-            if seeds is not None:
+            if seeds is not None and self.episode_seeds and all(0 <= s < 2 ** 63 for s in seeds):
+                self.set_env_seed(ids, seeds)
+            elif seeds is not None:
                 states = np.array([rng_state_of(s) for s in seeds], RNG_DTYPE)
                 self.engine.seed(ids, states)
             self.engine.reset(None if env_ids is None else ids, stream=self._level_stream())
@@ -662,9 +760,9 @@ class BatchedMiniWorld:
         self._seeded = True
 
     def _torch_writes(self):
-        """True when torch work may write arrays the kernels read: next_level / level_weights (level changes on) or the
-        params table (once set_level_param has written it)."""
-        return (self.dynamic_levels or self._params_written) and not self.engine.host_memory
+        """True when torch work may write arrays the kernels read: next_level / level_weights (level changes on),
+        next_seed (episode seeds on) or the params table (once set_level_param has written it)."""
+        return (self.dynamic_levels or self.episode_seeds or self._params_written) and not self.engine.host_memory
 
     def _level_stream(self):
         """Stream for a call whose steps and resets read next_level / level_weights or the params table: when torch

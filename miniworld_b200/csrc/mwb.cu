@@ -1337,6 +1337,25 @@ extern "C" int mwb_enable_level_changes(mwb_handle* h, uint64_t seed, int32_t en
   return MWB_OK;
 }
 
+extern "C" int mwb_enable_episode_seeds(mwb_handle* h) {
+  if (!h) return fail(MWB_EINVAL, "null handle");
+  if (h->S.next_seed) return fail(MWB_ESTATE, "episode seeds are already on");
+  if (!h->have_params || !h->S.ops)
+    return fail(MWB_ESTATE, "episode seeds need device resets (params and a reset program: mwb_set_levels, or "
+                            "mwb_set_params and mwb_set_program); host-generated worlds keep their streams on the host");
+  DevState& S = h->S;
+  int rc = drain(h);
+  if (rc) return rc;
+  int64_t* next = nullptr;
+  int64_t* episode = nullptr;
+  if (alloc_arr(h, &next, S.N) || alloc_arr(h, &episode, S.N)) return fail(MWB_ECUDA, "episode-seed state allocation failed");
+  if (dev_memset(next, 0xFF, (size_t)S.N * sizeof(int64_t)) != 0 || dev_memset(episode, 0xFF, (size_t)S.N * sizeof(int64_t)) != 0)
+    return fail(MWB_ECUDA, "memset failed");   // all -1
+  S.next_seed = next;
+  S.episode_seed = episode;
+  return MWB_OK;
+}
+
 // env_level[env] as the kernels see it: the host copy, or the device array once level changes are on
 static int current_level(mwb_handle* h, int env, int32_t* out) {
   if (!h->S.next_level) {
@@ -2021,16 +2040,22 @@ static const uint32_t kSnapMagic = 0x5342574du;               // "MWBS"
 static const uint32_t kSnapMagicLevelChanges = 0x4c42574du;   // "MWBL"
 static const uint32_t kSnapMagicWorlds = 0x5742574du;         // "MWBW": level table with per-env worlds
 static const uint32_t kSnapMagicWorldsLevelChanges = 0x5842574du;   // "MWBX": ... and level changes on
+// a handle with episode seeds on writes the mode letter in lower case ("MWBs", "MWBl", "MWBw", "MWBx") and carries
+// next_seed and episode_seed among its arrays
+static const uint32_t kSnapMagicSeeds = 0x20000000u;
 
 static uint32_t snapshot_magic(const mwb_handle* h) {
-  if (h->level_mazes) return h->S.next_level ? kSnapMagicWorldsLevelChanges : kSnapMagicWorlds;
-  return h->S.next_level ? kSnapMagicLevelChanges : kSnapMagic;
+  const uint32_t seeds = h->S.next_seed ? kSnapMagicSeeds : 0u;
+  if (h->level_mazes) return (h->S.next_level ? kSnapMagicWorldsLevelChanges : kSnapMagicWorlds) | seeds;
+  return (h->S.next_level ? kSnapMagicLevelChanges : kSnapMagic) | seeds;
 }
-static const char* snapshot_mode(uint32_t magic) {
-  return magic == kSnapMagic ? "level changes off, no per-env worlds"
-         : magic == kSnapMagicLevelChanges ? "level changes on, no per-env worlds"
-         : magic == kSnapMagicWorlds ? "level changes off, per-env worlds"
-                                     : "level changes on, per-env worlds";
+static std::string snapshot_mode(uint32_t magic) {
+  const uint32_t base = magic & ~kSnapMagicSeeds;
+  return std::string(base == kSnapMagic ? "level changes off, no per-env worlds"
+                     : base == kSnapMagicLevelChanges ? "level changes on, no per-env worlds"
+                     : base == kSnapMagicWorlds ? "level changes off, per-env worlds"
+                                                : "level changes on, per-env worlds") +
+         (magic & kSnapMagicSeeds ? ", episode seeds on" : ", episode seeds off");
 }
 
 struct SnapHeader {
@@ -2074,6 +2099,7 @@ static void snapshot_arrays(mwb_handle* h, std::vector<std::pair<void*, size_t>>
   SA(rooms, G * S.R); SA(quads, G * S.Q); SA(segs, G * S.S); SA(room_tex, N * S.R * 3);
   // the level ranges are run-time state (MWB_ARRAY_LEVEL_PARAMS), and so is what each env's last reset took from them
   SA(env_mfs, N); SA(level_params, h->levels.size());
+  if (S.next_seed) { SA(next_seed, N); SA(episode_seed, N); }
 #undef SA
 }
 
@@ -2138,8 +2164,9 @@ extern "C" int mwb_restore(mwb_handle* h, const void* blob, size_t bytes) {
   SnapHeader hd;
   if (bytes < sizeof(hd)) return fail(MWB_EINVAL, "not a snapshot");
   memcpy(&hd, blob, sizeof(hd));
-  if ((hd.magic != kSnapMagic && hd.magic != kSnapMagicLevelChanges && hd.magic != kSnapMagicWorlds &&
-       hd.magic != kSnapMagicWorldsLevelChanges) || hd.abi != want.abi)
+  const uint32_t base = hd.magic & ~kSnapMagicSeeds;
+  if ((base != kSnapMagic && base != kSnapMagicLevelChanges && base != kSnapMagicWorlds &&
+       base != kSnapMagicWorldsLevelChanges) || hd.abi != want.abi)
     return fail(MWB_EABI, "snapshot from another ABI version");
   const bool dynamic = h->S.next_level != nullptr;
   if (hd.magic != want.magic)
@@ -2250,6 +2277,11 @@ extern "C" int mwb_state_array(mwb_handle* h, int which, void** dev_ptr, int64_t
       if (which == MWB_ARRAY_ENV_LEVEL) { *dev_ptr = h->S.env_level; *count = N; }                       // int32 [N]
       else if (which == MWB_ARRAY_NEXT_LEVEL) { *dev_ptr = h->S.next_level; *count = N; }                // int32 [N]
       else { *dev_ptr = (void*)h->S.level_weights; *count = h->S.num_levels; }                           // float32 [L]
+      break;
+    case MWB_ARRAY_NEXT_SEED:
+    case MWB_ARRAY_EPISODE_SEED:
+      if (!h->S.next_seed) return fail(MWB_ESTATE, "episode seeds are off (mwb_enable_episode_seeds)");
+      *dev_ptr = which == MWB_ARRAY_NEXT_SEED ? h->S.next_seed : h->S.episode_seed; *count = N;           // int64 [N]
       break;
     case MWB_ARRAY_LEVEL_PARAMS:
       if (!h->have_params || !h->S.ops)

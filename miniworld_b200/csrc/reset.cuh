@@ -74,8 +74,38 @@ MWB_DEV int resolve_level(const DevState& S, int i) {
   return lvl;
 }
 
+// SeedSequence(seed) -> PCG64 into one env's stream.  Out of line: about a hundred dependent integer operations that
+// only a reset with a pending seed runs, kept out of step_kernel's register allocation.  It takes the six addresses
+// rather than the DevState, which is a kernel parameter and would be copied to the stack to be passed on.
+MWB_DEV_NOINLINE void seed_stream(uint64_t seed, uint64_t* s_hi, uint64_t* s_lo, uint64_t* inc_hi, uint64_t* inc_lo,
+                                  int32_t* has32, uint32_t* cache) {
+  const NpRng r = rng_seed(seed);
+  *s_hi = r.s_hi;
+  *s_lo = r.s_lo;
+  *inc_hi = r.inc_hi;
+  *inc_lo = r.inc_lo;
+  *has32 = r.has32;
+  *cache = r.cache;
+}
+
+// The stream env i's reset starts from (mwb_enable_episode_seeds; include/mwb.h states the rule): a pending seed
+// replaces the stream and is consumed, otherwise the env continues its own.  As in resolve_level, every lane computes
+// the same value from the same loads, and warp barriers separate the loads from the stores.
+MWB_DEV void take_seed(const DevState& S, int i) {
+  MWB_WARP_SYNC();
+  const int64_t seed = S.next_seed[i];
+  MWB_WARP_SYNC();
+  S.episode_seed[i] = seed >= 0 ? seed : -1;
+  if (seed != -1) S.next_seed[i] = -1;
+  if (seed >= 0)
+    seed_stream((uint64_t)seed, S.rng_s_hi + i, S.rng_s_lo + i, S.rng_inc_hi + i, S.rng_inc_lo + i, S.rng_has32 + i,
+                S.rng_cache + i);
+  MWB_WARP_SYNC();
+}
+
 MWB_DEV void device_reset(const DevState& S, int i) {
   const size_t N = S.N;
+  if (S.next_seed) take_seed(S, i);
   NpRng rng = load_rng(S, i);
   const int lvl = S.next_level ? resolve_level(S, i) : S.env_level[i];
   // the resolved level decides everything below, its domain_rand included: a reset that switches levels draws by the

@@ -125,6 +125,9 @@ struct DevState {
   const float* level_weights;   // [num_levels] sampling weights, all <= 0 = keep the level
   uint64_t level_seed;
   int32_t level_env_offset;     // global index of env 0 (sharded runs)
+  // episode seeds (mwb_enable_episode_seeds); null on a handle without them
+  int64_t* next_seed;           // [N] seed the env's next reset starts its stream from, negative = none
+  int64_t* episode_seed;        // [N] seed the env's current episode started from, -1 = it continued its stream
   int32_t autoreset;
   // StochasticActionWrapper on the device (reference wrappers.py:49-71): per step one uniform() draw from
   // the env's own stream; below act_prob the chosen action stands, else act_random (< 0: integers(0, 6))

@@ -24,7 +24,9 @@ class ShardedMiniWorld:
     def __init__(self, level, total_envs, dist=None, device=0, env_level=None, **kwargs):
         """`level` may be a sequence of levels as for BatchedMiniWorld; `env_level` is then the assignment of all
         `total_envs` envs (default: contiguous near-equal blocks), and this rank runs its slice of it.  With
-        `dynamic_levels=True` (and `level_seed`) the level draws of global env i are those of the single-process run."""
+        `dynamic_levels=True` (and `level_seed`) the level draws of global env i are those of the single-process run.
+        `episode_seeds=True` is passed on as it is: a seed belongs to an env, so this rank's `local.next_seed` /
+        `local.episode_seed` are its slice of the single-process arrays."""
         from .batched import BatchedMiniWorld, default_env_level
         self.dist = dist
         self.rank = dist.get_rank() if dist is not None else 0

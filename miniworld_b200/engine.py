@@ -135,6 +135,7 @@ EXPORTS = (
     "mwb_snapshot_size", "mwb_snapshot", "mwb_restore", "mwb_set_obs_format",
     "mwb_flag_write", "mwb_flag_wait_geq", "mwb_flag_mode", "mwb_state_array", "mwb_debug_camera", "mwb_set_obs_peer",
     "mwb_set_levels", "mwb_enable_level_changes", "mwb_state_in_host_memory", "mwb_set_level_maze",
+    "mwb_enable_episode_seeds",
 )
 OBS_FORMATS = {"hwc": 0, "cwh": 1, "grey": 2}
 
@@ -173,6 +174,7 @@ def load_library():
     lib.mwb_set_program.argtypes = [vp, vp, C.c_int]
     lib.mwb_set_levels.argtypes = [vp, C.c_int, vp, vp, vp, C.c_int, vp]
     lib.mwb_enable_level_changes.argtypes = [vp, C.c_uint64, C.c_int32]
+    lib.mwb_enable_episode_seeds.argtypes = [vp]
     lib.mwb_state_in_host_memory.argtypes = []
     lib.mwb_seed.argtypes = [vp, vp, C.c_int, vp]
     lib.mwb_reset.argtypes = [vp, vp, C.c_int, vp]
@@ -475,6 +477,11 @@ class Engine:
         draws from "level_weights", keyed by `seed` and the env's global index env_offset + i."""
         self._check(self.lib.mwb_enable_level_changes(self.h, int(seed) & (2 ** 64 - 1), int(env_offset)))
 
+    def enable_episode_seeds(self):
+        """Resets take a pending seed from "next_seed" and record it in "episode_seed" from now on
+        (mwb_enable_episode_seeds); needs device resets."""
+        self._check(self.lib.mwb_enable_episode_seeds(self.h))
+
     # ---- reset
     def seed(self, env_ids, states):
         ids = np.ascontiguousarray(env_ids, np.int32)
@@ -555,13 +562,14 @@ class Engine:
     ARRAYS = {"counter": (0, "<i4", "env"), "step_count": (1, "<i4", "env"), "ent_x": (2, "<f8", "env"),
               "ent_y": (3, "<f8", "env"), "ent_z": (4, "<f8", "env"), "ent_dir": (5, "<f8", "env"),
               "env_level": (6, "<i4", "env"), "next_level": (7, "<i4", "env"), "level_weights": (8, "<f4", "level"),
-              "level_params": (9, "<f8", "params")}
+              "level_params": (9, "<f8", "params"), "next_seed": (16, "<i8", "env"), "episode_seed": (17, "<i8", "env")}
 
     def state_array(self, name):
         """Zero-copy view of a state array (mwb_state_array) as an object with __cuda_array_interface__:
         "counter" / "step_count" int32 [N]; "ent_x|y|z|dir" float64 [max_ents, N]; with level changes on,
         "env_level" / "next_level" int32 [N] and "level_weights" float32 [n_levels]; with device resets,
-        "level_params" float64 [n_levels, PARAMS_DOUBLES] (column of a field: PARAMS_COLUMN).  On the host build of
+        "level_params" float64 [n_levels, PARAMS_DOUBLES] (column of a field: PARAMS_COLUMN); with episode seeds on,
+        "next_seed" / "episode_seed" int64 [N].  On the host build of
         the kernels the arrays live in host memory, and the view is a numpy array over the same memory instead."""
         which, typestr, axis = self.ARRAYS[name]
         ptr, count = C.c_void_p(), C.c_int64()
