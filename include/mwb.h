@@ -387,6 +387,42 @@ typedef struct mwb_maze_desc {
 } mwb_maze_desc;
 int mwb_set_maze(mwb_handle* h, const mwb_maze_desc* maze);
 
+/* Maze layouts (environment design: PAIRED's adversary writes the maze, ACCEL edits the walls of past levels and
+ * replays them).  Valid after mwb_set_maze / mwb_set_level_maze on a handle with device resets; MWB_ESTATE when the
+ * handle has no Maze level, resets on the host, or has the mode on already; MWB_ECAPACITY when some Maze level's
+ * all-open maze does not fit the handle: for c = R C cells and E = R (C - 1) + (R - 1) C inner edges, max_rooms
+ * c + E, max_quads 6c + 2E and max_segs 4c (a tree needs 2c - 1, 8c - 2 and 4c).  K2's per-level triangle capacity and
+ * the HBM triangle lists are sized from the all-open bound from then on.
+ *
+ * A layout is uint8 [maze_rows][maze_cols], the maxima of mwb_maze_desc rows / cols over the handle's Maze levels.  Bit 0 of cell (j, i) opens the
+ * wall to (j, i + 1), bit 1 the wall to (j + 1, i); cells outside a level's grid, bits that point outside it and the
+ * other six bits are ignored.  Loops, isolated cells and unreachable goals are allowed.  Four arrays, all zero (and
+ * the cells -1) at the call, read and written in place through mwb_state_array, stream-ordered, without a sync:
+ *   next_maze uint8 [N][rows][cols]    layout of the env's next reset at a Maze level;
+ *   next_maze_cells int32 [N][2]       (goal cell, agent cell) of that layout, each j * maze_cols + i, or -1 (an index
+ *                                      outside the level's grid counts as -1): where the goal box / agent are placed;
+ *   maze_pending uint8 [N]             nonzero: next_maze waits for the env's next reset at a Maze level;
+ *   episode_maze uint8 [N][rows][cols] layout of each env's running episode, masked to its grid.
+ * At every reset of env i (mwb_reset, and the next-step auto-reset inside mwb_step), after the level is resolved:
+ *   1. at a Maze level with maze_pending[i] set: episode_maze[i] = next_maze[i] masked, maze_pending[i] = 0, and the
+ *      world is built as this host code builds it (Maze._gen_world with options={"maze": ...}): the grid rooms row by
+ *      row; for each cell in row-major order, connect_rooms(cell, cell + x, min_z, max_z) if bit 0 is set, then
+ *      connect_rooms(cell, cell + z, min_x, max_x) if bit 1 is set; place_entity(Box(color="red"), room=goal cell's
+ *      room or none); place_agent(room=agent cell's room or none).  No carve draws are made; textures, sky and light
+ *      and the camera draws follow as at every reset.  The room pick probabilities are the env's own:
+ *      p = areas / np.sum(areas) (numpy's pairwise summation), cdf = p.cumsum() / p.cumsum()[-1];
+ *   2. at a Maze level without a pending layout: the random carve, as before, and episode_maze[i] records its topology
+ *      (a connector from a cell in direction d sets the +x or +z bit of the cell on its -x / -z side).  Replaying such
+ *      a layout builds the same walls but creates the connectors in another order, so the placement draws differ;
+ *   3. at any other level: episode_maze[i] = 0, and a pending layout stays pending.
+ * After a terminating step episode_maze still names the episode that ended, because the reset happens inside the next
+ * step.  With episode seeds on, a layout, its two cells and a seed reproduce an episode exactly.  Handles that never
+ * call this behave exactly as before it existed, and the addition changes no struct, so MWB_ABI_VERSION stays as it
+ * is.  Snapshots of a handle with the mode on carry the four arrays and are marked as such in the header; restoring a
+ * blob into a handle whose layouts are on / off while the blob's were off / on fails with MWB_ESTATE before anything
+ * else is compared. */
+int mwb_enable_maze_layouts(mwb_handle* h);
+
 /* Maze levels in a level table (curricula over maze sizes: MazeS2 -> MazeS3 -> Maze, next to fixed-layout levels).
  * Valid on a shared_geometry = 1 handle after mwb_set_levels (MWB_ESTATE otherwise).  Level `level` (MWB_EINVAL
  * outside [0, L)) becomes a per-env-world level: every reset of an env at that level carves a fresh maze from these
@@ -544,6 +580,11 @@ int mwb_debug_camera(mwb_handle* h, float* out /* host [num_envs][16] */);
  * for further level-table arrays: */
 #define MWB_ARRAY_NEXT_SEED 16      /* int64   [num_envs]  seed of the env's next reset, negative = none           */
 #define MWB_ARRAY_EPISODE_SEED 17   /* int64   [num_envs]  seed the env's current episode started from, or -1    */
+/* with maze layouts on (mwb_enable_maze_layouts; MWB_ESTATE otherwise); count = elements, rows x cols per env: */
+#define MWB_ARRAY_NEXT_MAZE 18        /* uint8 [num_envs][rows][cols]  layout of the env's next reset at a Maze level */
+#define MWB_ARRAY_NEXT_MAZE_CELLS 19  /* int32 [num_envs][2]  goal cell, agent cell of that layout, -1 = random       */
+#define MWB_ARRAY_MAZE_PENDING 20     /* uint8 [num_envs]  nonzero = next_maze waits for a reset at a Maze level       */
+#define MWB_ARRAY_EPISODE_MAZE 21     /* uint8 [num_envs][rows][cols]  layout of the env's running episode            */
 int mwb_state_array(mwb_handle* h, int which, void** dev_ptr, int64_t* count);
 /* 1 when this library keeps the handle's state arrays (mwb_state_array) in host memory -- the CPU build of the kernels
  * used by the test suite -- and 0 for libmwb.so, whose arrays are device memory. */

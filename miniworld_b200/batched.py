@@ -16,7 +16,9 @@ Per-environment semantics are exactly those of the reference's `MiniWorldEnv.res
   * with several levels and `dynamic_levels=True`, an env's level can change at its resets:
     pending assignments (`set_env_level`) and device-side draws from `level_weights`;
   * with `episode_seeds=True`, an env's next reset can start from a chosen seed (`next_seed`, `set_env_seed`),
-    seeded on the device as `reset(seed=s)` would, and `info["seed"]` names the seed of each running episode.
+    seeded on the device as `reset(seed=s)` would, and `info["seed"]` names the seed of each running episode;
+  * with `maze_layouts=True`, an env's next reset at a Maze level can build a maze written into a device tensor
+    (`next_maze`, `set_env_maze`), and `info["maze"]` holds the layout of each running episode.
 
 Outputs are torch CUDA tensors by default (zero-copy from the kernels); `step_host`
 performs the same step with pinned host buffers for callers that want numpy.
@@ -182,11 +184,24 @@ class BatchedMiniWorld:
     env plays, for level replay: a seed written to `next_seed[i]` (`set_env_seed`) is consumed by env i's next reset,
     the auto-reset inside `step` included, which then starts the stream `reset(seed=s)` would, built on the device.
     `episode_seed` / `info["seed"]` hold the seed each running episode started from, or -1 when the env continued its
-    stream; after a terminating step they still name the episode that just ended."""
+    stream; after a terminating step they still name the episode that just ended.
+
+    `maze_layouts=True` (a single Maze-family level, or a table with some) lets torch code design the mazes, for
+    environment design (PAIRED, ACCEL): a layout written to `next_maze[i]` (uint8 [rows, cols], the maxima over the
+    batch's Maze levels; bit 0 of cell (j, i) opens its wall to (j, i + 1), bit 1 its wall to (j + 1, i)) with
+    `maze_pending[i] = 1` is built by env i's next reset at a Maze level, the auto-reset inside `step` included, as
+    `Maze.reset(options={"maze": layout, "goal_cell": g, "agent_cell": a})` builds it on the host; `next_maze_cells[i]`
+    holds (g, a), flat cells j * cols + i where the goal box and the agent are placed, -1 for anywhere.  A reset at a
+    level that is not a Maze leaves the layout pending.  `episode_maze` / `info["maze"]` hold the layout of every
+    running episode, random carves included (zeros at other levels); after a terminating step they still name the
+    episode that just ended.  Replaying a carve's recorded layout builds the same walls, but creates the connector rooms
+    in another order than the carve did, so the episode's placement draws differ.  Each Maze level's capacities are
+    sized for its all-open maze (c cells, E inner edges: c + E rooms, 6c + 2E quads, as against 2c - 1 and 8c - 2)."""
 
     def __init__(self, level, num_envs, obs_width=80, obs_height=60, domain_rand=False, autoreset=True,
                  msaa_samples=8, device=0, want_depth=False, level_kwargs=None, obs_format="hwc", env_level=None,
-                 dynamic_levels=False, level_seed=0, env_offset=0, per_env_worlds=False, episode_seeds=False):
+                 dynamic_levels=False, level_seed=0, env_offset=0, per_env_worlds=False, episode_seeds=False,
+                 maze_layouts=False):
         self.num_envs = int(num_envs)
         self.obs_width, self.obs_height = int(obs_width), int(obs_height)
         self.domain_rand = bool(domain_rand)
@@ -195,6 +210,7 @@ class BatchedMiniWorld:
         self.dynamic_levels = bool(dynamic_levels)
         self.per_env_worlds = bool(per_env_worlds)
         self.episode_seeds = bool(episode_seeds)
+        self.maze_layouts = bool(maze_layouts)
         table = isinstance(level, (list, tuple))
         if table:
             defs = self._init_levels(list(level), level_kwargs, env_level)
@@ -207,6 +223,8 @@ class BatchedMiniWorld:
                 raise ValueError("per_env_worlds lets Maze levels join a level table: pass `level` as a sequence of "
                                  "levels (a single Maze level always has per-env worlds)")
             defs = self._init_level(level, level_kwargs)
+        if self.maze_layouts:
+            self._size_for_layouts(defs)
         self._init_engine(defs, table, msaa_samples, autoreset)
         self._level_views = None
         if self.dynamic_levels:
@@ -218,6 +236,9 @@ class BatchedMiniWorld:
                 self.engine.close()
                 raise TypeError("episode seeds are taken by device resets; host-reset levels keep RNG streams in Python")
             self.engine.enable_episode_seeds()
+        self._maze_views = None
+        if self.maze_layouts:
+            self.engine.enable_maze_layouts()
         # observation layout written by the render kernel: the reference's PyTorchObsWrapper ("cwh") and
         # GreyscaleWrapper ("grey") are fused into its epilogue instead of running as separate passes
         self.obs_format = obs_format
@@ -288,6 +309,26 @@ class BatchedMiniWorld:
         self.max_episode_steps = [d.pe.max_episode_steps for d in defs]     # per level
         self._env_level = env_level.astype(np.int32)
         return defs
+
+    def _size_for_layouts(self, defs):
+        """maze_layouts=True: every Maze level's capacities from its all-open maze (c cells, E inner edges: c + E rooms,
+        6c + 2E quads, 4c segments), and the layout shape from the largest grid."""
+        from .envs.maze import Maze
+        mazes = [d for d in defs if d.uses_maze or issubclass(d.cls, Maze)]
+        if not mazes:
+            raise ValueError("maze_layouts needs a Maze-family level in the batch")
+        for d in mazes:
+            if d.maze is None:
+                raise TypeError("%s: its maze templates do not reproduce host-generated worlds, so it resets on the host, "
+                                "where designed layouts cannot reach it" % d.name) from d.maze_error
+            R, C = d.maze.rows, d.maze.cols
+            try:
+                d.maze.verify_layouts([np.full((R, C), 3, np.uint8)])       # the all-open maze: every connector kind
+            except AssertionError as err:
+                raise TypeError("%s: its maze templates do not reproduce host-built designed layouts" % d.name) from err
+            c, e = R * C, R * (C - 1) + (R - 1) * C
+            d.caps = (max(d.caps[0], c + e), max(d.caps[1], 6 * c + 2 * e), max(d.caps[2], 4 * c))
+        self.maze_shape = (max(d.maze.rows for d in mazes), max(d.maze.cols for d in mazes))
 
     def _init_engine(self, defs, table, msaa_samples, autoreset):
         """Create the handle and program it in one of three ways: a single level that resets on the host (worlds
@@ -378,6 +419,9 @@ class BatchedMiniWorld:
             if self.episode_seeds:
                 # the seed each env's current episode started from (after a terminating step still the ended one's)
                 self._info["seed"] = self.episode_seed
+            if self.maze_layouts:
+                # the layout of each env's current episode (after a terminating step still the ended one's)
+                self._info["maze"] = self.episode_maze
         return self._torch
 
     # ------------------------------------------------------------------ level changes (dynamic_levels=True)
@@ -520,6 +564,94 @@ class BatchedMiniWorld:
         if arr.shape != tuple(shape):
             raise ValueError("%d env ids but %d seeds" % (int(np.prod(shape)), arr.size))
         return arr
+
+    # ------------------------------------------------------------------ maze layouts (maze_layouts=True)
+    def _mazes(self):
+        """next_maze / next_maze_cells / maze_pending / episode_maze in place, made like `_views`: torch CUDA tensors,
+        or numpy arrays on the kernels' host build."""
+        if not self.maze_layouts:
+            raise RuntimeError("this batch has no maze layouts: construct it with maze_layouts=True")
+        if self._maze_views is None:
+            shapes = {"next_maze": (self.num_envs,) + self.maze_shape, "next_maze_cells": (self.num_envs, 2),
+                      "maze_pending": (self.num_envs,), "episode_maze": (self.num_envs,) + self.maze_shape}
+            if self.engine.host_memory:
+                self._maze_views = {n: self.engine.state_array(n).reshape(shp) for n, shp in shapes.items()}
+            else:
+                import torch
+                dev = torch.device("cuda", self.device)
+                self._maze_views = {n: torch.as_tensor(self.engine.state_array(n), device=dev).view(shp)
+                                    for n, shp in shapes.items()}
+        return self._maze_views
+
+    @property
+    def next_maze(self):
+        """uint8 [N, rows, cols] view of the layout each env's next reset at a Maze level builds once `maze_pending` is
+        set; write it in place (stream-ordered, no sync)."""
+        return self._mazes()["next_maze"]
+
+    @property
+    def next_maze_cells(self):
+        """int32 [N, 2] view of (goal cell, agent cell) of each pending layout: j * cols + i, or -1 for anywhere."""
+        return self._mazes()["next_maze_cells"]
+
+    @property
+    def maze_pending(self):
+        """uint8 [N] view: nonzero when next_maze[i] waits for env i's next reset at a Maze level, which clears it."""
+        return self._mazes()["maze_pending"]
+
+    @property
+    def episode_maze(self):
+        """uint8 [N, rows, cols] view of the layout of each env's running episode (zeros at levels that are not Mazes)."""
+        return self._mazes()["episode_maze"]
+
+    def set_env_maze(self, env_ids, layouts, goal_cell=-1, agent_cell=-1):
+        """Build the listed envs' next mazes from `layouts` (one uint8 [rows, cols] layout, or one per env) with the
+        goal box in `goal_cell` and the agent in `agent_cell` (one flat cell j * cols + i, or one per env; -1 for
+        anywhere); envs in mid-episode finish it first.  An env listed more than once takes its last entry.  The input
+        is checked on the host, then written with torch ops on the current stream, without a sync."""
+        views = self._mazes()
+        ids = np.atleast_1d(np.asarray(env_ids.cpu() if hasattr(env_ids, "cpu") else env_ids))
+        if not np.issubdtype(ids.dtype, np.integer) or ids.ndim != 1:
+            raise ValueError("set_env_maze takes a 1-D sequence of integer env ids")
+        if ids.size and (ids.min() < 0 or ids.max() >= self.num_envs):
+            raise ValueError("env ids must lie in [0, %d)" % self.num_envs)
+        host = lambda a: np.asarray(a.cpu() if hasattr(a, "cpu") else a)
+        lay = host(layouts)
+        if not (np.issubdtype(lay.dtype, np.integer) or lay.dtype == np.bool_):
+            raise ValueError("maze layouts are integer arrays (uint8), got %s" % lay.dtype)
+        if lay.shape == self.maze_shape:
+            lay = np.broadcast_to(lay, (ids.size,) + self.maze_shape)
+        if lay.shape != (ids.size,) + self.maze_shape:
+            raise ValueError("maze layouts must have shape %s or %s, got %s" % (self.maze_shape, (ids.size,) + self.maze_shape,
+                                                                              lay.shape))
+        if lay.size and (lay.min() < 0 or lay.max() > 3):
+            raise ValueError("a maze layout sets only bits 0 (+x wall open) and 1 (+z wall open)")
+        n_cells = self.maze_shape[0] * self.maze_shape[1]
+        cells = []
+        for name, c in (("goal_cell", goal_cell), ("agent_cell", agent_cell)):
+            c = host(c)
+            if not np.issubdtype(c.dtype, np.integer) or c.ndim > 1 or (c.ndim == 1 and c.shape != ids.shape):
+                raise ValueError("%s is one integer or one per env id" % name)
+            if c.size and (c.min() < -1 or c.max() >= n_cells):
+                raise ValueError("%s entries must lie in [-1, %d)" % (name, n_cells))
+            cells.append(np.broadcast_to(c, ids.shape))
+        if ids.size == 0:
+            return
+        last = ids.size - 1 - np.unique(ids[::-1], return_index=True)[1]    # an env listed twice: its last entry wins
+        ids, lay = ids[last], np.ascontiguousarray(lay[last], np.uint8)
+        both = np.ascontiguousarray(np.stack([c[last] for c in cells], axis=1), np.int32)
+        if isinstance(views["next_maze"], np.ndarray):
+            views["next_maze"][ids] = lay
+            views["next_maze_cells"][ids] = both
+            views["maze_pending"][ids] = 1
+        else:
+            torch = self._ensure_torch()
+            dev = views["next_maze"].device
+            to_dev = lambda a: torch.as_tensor(a).to(dev, non_blocking=True)
+            idx = to_dev(ids.astype(np.int64))
+            views["next_maze"][idx] = to_dev(lay)
+            views["next_maze_cells"][idx] = to_dev(both)
+            views["maze_pending"][idx] = 1
 
     # ------------------------------------------------------------------ level params at run time
     def _level_params(self):
@@ -761,8 +893,10 @@ class BatchedMiniWorld:
 
     def _torch_writes(self):
         """True when torch work may write arrays the kernels read: next_level / level_weights (level changes on),
-        next_seed (episode seeds on) or the params table (once set_level_param has written it)."""
-        return (self.dynamic_levels or self.episode_seeds or self._params_written) and not self.engine.host_memory
+        next_seed (episode seeds on), the pending maze layouts (maze layouts on) or the params table (once
+        set_level_param has written it)."""
+        return ((self.dynamic_levels or self.episode_seeds or self.maze_layouts or self._params_written)
+                and not self.engine.host_memory)
 
     def _level_stream(self):
         """Stream for a call whose steps and resets read next_level / level_weights or the params table: when torch

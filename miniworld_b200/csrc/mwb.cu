@@ -120,6 +120,7 @@ struct mwb_handle {
   bool level_mazes;               // mwb_set_level_maze succeeded: per-env worlds after the level templates
   std::vector<int32_t> level_quads;   // quads of every level's worlds (per-level K2 planning of a table with mazes)
   std::vector<MazeDev> mazes_h;       // host copies of S.maze / S.maze_cdf, one entry per level
+  MazeLayouts layouts_h;              // host copy of *S.layouts (mwb_enable_maze_layouts)
   std::vector<double> maze_cdf_h;
   bool have_params, have_protos, have_template;
   bool have_level_table;          // mwb_set_levels succeeded (mwb_enable_level_changes needs it)
@@ -1462,6 +1463,57 @@ extern "C" int mwb_set_level_maze(mwb_handle* h, int level, const mwb_maze_desc*
   return MWB_OK;
 }
 
+extern "C" int mwb_enable_maze_layouts(mwb_handle* h) {
+  if (!h) return fail(MWB_EINVAL, "null handle");
+  if (h->S.layouts) return fail(MWB_ESTATE, "maze layouts are already on");
+  if (!h->have_params || !h->S.ops)
+    return fail(MWB_ESTATE, "maze layouts need device resets (mwb_set_maze or mwb_set_level_maze on a handle with a "
+                            "reset program); host-generated worlds are built on the host");
+  DevState& S = h->S;
+  int rows = 0, cols = 0;
+  std::vector<int32_t> quads(h->level_quads);
+  for (size_t l = 0; l < h->levels.size(); ++l) {
+    if (h->levels[l].maze < 0 || !h->levels[l].env_worlds) continue;
+    const MazeDev& m = h->mazes_h[l];
+    const int c = m.rows * m.cols, e = m.rows * (m.cols - 1) + (m.rows - 1) * m.cols;
+    // every layout must fit: the all-open maze has c + E rooms, 6c + 2E quads and 4c segments
+    if (c + e > S.R || 6 * c + 2 * e > h->cfg.max_quads || 4 * c > S.S)
+      return fail(MWB_ECAPACITY, "the handle's room / quad / segment capacities do not fit an all-open maze of level " +
+                                     std::to_string(l) + " (max_rooms c + E, max_quads 6c + 2E, max_segs 4c)");
+    if (l < quads.size()) quads[l] = 6 * c + 2 * e;
+    rows = std::max(rows, m.rows);
+    cols = std::max(cols, m.cols);
+  }
+  if (rows == 0) return fail(MWB_ESTATE, "maze layouts need a Maze level (mwb_set_maze or mwb_set_level_maze)");
+  int rc = drain(h);
+  if (rc) return rc;
+  const size_t N = S.N, cells = (size_t)rows * cols;
+  uint8_t *next = nullptr, *pending = nullptr, *episode = nullptr;
+  int32_t* next_cells = nullptr;
+  if (alloc_arr(h, &next, N * cells) || alloc_arr(h, &next_cells, 2 * N) || alloc_arr(h, &pending, N) ||
+      alloc_arr(h, &episode, N * cells))
+    return fail(MWB_ECUDA, "maze layout state allocation failed");
+  if (dev_memset(next_cells, 0xFF, 2 * N * sizeof(int32_t)) != 0) return fail(MWB_ECUDA, "memset failed");   // all -1
+  if (h->level_mazes) {   // K2's per-level capacity and the HBM lists from the all-open bound
+    h->level_quads = quads;
+    plan_k2(h);
+    if ((rc = ensure_room_tris(h)) != 0 || (rc = upload_levels(h)) != 0) return rc;
+    k2_report(h);
+  }
+  MazeLayouts& Y = h->layouts_h;
+  Y.next = next;
+  Y.cells = next_cells;
+  Y.pending = pending;
+  Y.episode = episode;
+  Y.rows = rows;
+  Y.cols = cols;
+  MazeLayouts* d = nullptr;
+  if (alloc_arr(h, &d, 1)) return fail(MWB_ECUDA, "maze layout state allocation failed");
+  if (h2d(d, &Y, sizeof(Y), h->stream) != 0 || sync_stream(h->stream) != 0) return fail(MWB_ECUDA, "upload failed");
+  S.layouts = d;
+  return MWB_OK;
+}
+
 // geometry block env `env` reads (geom_index in state.h), from the host's view of its level
 static int env_geom_block(mwb_handle* h, int env, size_t* g) {
   int32_t lvl = 0;
@@ -2043,19 +2095,22 @@ static const uint32_t kSnapMagicWorldsLevelChanges = 0x5842574du;   // "MWBX": .
 // a handle with episode seeds on writes the mode letter in lower case ("MWBs", "MWBl", "MWBw", "MWBx") and carries
 // next_seed and episode_seed among its arrays
 static const uint32_t kSnapMagicSeeds = 0x20000000u;
+// one with maze layouts on writes the "B" in lower case ("MWbS", "MWbs", ...) and carries the four layout arrays
+static const uint32_t kSnapMagicMazes = 0x00200000u;
 
 static uint32_t snapshot_magic(const mwb_handle* h) {
-  const uint32_t seeds = h->S.next_seed ? kSnapMagicSeeds : 0u;
+  const uint32_t seeds = (h->S.next_seed ? kSnapMagicSeeds : 0u) | (h->S.layouts ? kSnapMagicMazes : 0u);
   if (h->level_mazes) return (h->S.next_level ? kSnapMagicWorldsLevelChanges : kSnapMagicWorlds) | seeds;
   return (h->S.next_level ? kSnapMagicLevelChanges : kSnapMagic) | seeds;
 }
 static std::string snapshot_mode(uint32_t magic) {
-  const uint32_t base = magic & ~kSnapMagicSeeds;
+  const uint32_t base = magic & ~(kSnapMagicSeeds | kSnapMagicMazes);
   return std::string(base == kSnapMagic ? "level changes off, no per-env worlds"
                      : base == kSnapMagicLevelChanges ? "level changes on, no per-env worlds"
                      : base == kSnapMagicWorlds ? "level changes off, per-env worlds"
                                                 : "level changes on, per-env worlds") +
-         (magic & kSnapMagicSeeds ? ", episode seeds on" : ", episode seeds off");
+         (magic & kSnapMagicSeeds ? ", episode seeds on" : ", episode seeds off") +
+         (magic & kSnapMagicMazes ? ", maze layouts on" : ", maze layouts off");
 }
 
 struct SnapHeader {
@@ -2101,6 +2156,14 @@ static void snapshot_arrays(mwb_handle* h, std::vector<std::pair<void*, size_t>>
   SA(env_mfs, N); SA(level_params, h->levels.size());
   if (S.next_seed) { SA(next_seed, N); SA(episode_seed, N); }
 #undef SA
+  if (S.layouts) {
+    const MazeLayouts& Y = h->layouts_h;
+    const size_t cells = (size_t)Y.rows * Y.cols;
+    v.push_back(std::make_pair((void*)Y.next, N * cells));
+    v.push_back(std::make_pair((void*)Y.cells, 2 * N * sizeof(int32_t)));
+    v.push_back(std::make_pair((void*)Y.pending, N));
+    v.push_back(std::make_pair((void*)Y.episode, N * cells));
+  }
 }
 
 static SnapHeader snapshot_header(mwb_handle* h) {
@@ -2164,7 +2227,7 @@ extern "C" int mwb_restore(mwb_handle* h, const void* blob, size_t bytes) {
   SnapHeader hd;
   if (bytes < sizeof(hd)) return fail(MWB_EINVAL, "not a snapshot");
   memcpy(&hd, blob, sizeof(hd));
-  const uint32_t base = hd.magic & ~kSnapMagicSeeds;
+  const uint32_t base = hd.magic & ~(kSnapMagicSeeds | kSnapMagicMazes);
   if ((base != kSnapMagic && base != kSnapMagicLevelChanges && base != kSnapMagicWorlds &&
        base != kSnapMagicWorldsLevelChanges) || hd.abi != want.abi)
     return fail(MWB_EABI, "snapshot from another ABI version");
@@ -2282,6 +2345,18 @@ extern "C" int mwb_state_array(mwb_handle* h, int which, void** dev_ptr, int64_t
     case MWB_ARRAY_EPISODE_SEED:
       if (!h->S.next_seed) return fail(MWB_ESTATE, "episode seeds are off (mwb_enable_episode_seeds)");
       *dev_ptr = which == MWB_ARRAY_NEXT_SEED ? h->S.next_seed : h->S.episode_seed; *count = N;           // int64 [N]
+      break;
+    case MWB_ARRAY_NEXT_MAZE:
+    case MWB_ARRAY_EPISODE_MAZE:
+      if (!h->S.layouts) return fail(MWB_ESTATE, "maze layouts are off (mwb_enable_maze_layouts)");
+      *dev_ptr = which == MWB_ARRAY_NEXT_MAZE ? h->layouts_h.next : h->layouts_h.episode;                  // uint8
+      *count = N * h->layouts_h.rows * h->layouts_h.cols;                                                 // [N][rows][cols]
+      break;
+    case MWB_ARRAY_NEXT_MAZE_CELLS:
+    case MWB_ARRAY_MAZE_PENDING:
+      if (!h->S.layouts) return fail(MWB_ESTATE, "maze layouts are off (mwb_enable_maze_layouts)");
+      if (which == MWB_ARRAY_NEXT_MAZE_CELLS) { *dev_ptr = h->layouts_h.cells; *count = 2 * N; }          // int32 [N][2]
+      else { *dev_ptr = h->layouts_h.pending; *count = N; }                                               // uint8 [N]
       break;
     case MWB_ARRAY_LEVEL_PARAMS:
       if (!h->have_params || !h->S.ops)

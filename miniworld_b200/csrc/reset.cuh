@@ -9,7 +9,9 @@
 // CHOICE / UNIFORM / PLACE / PUT / IFEQ ops (miniworld_b200/program.py); room layout comes from the
 // static template of the env's level, and the program is that level's slice of the op array.  Maze levels carve a
 // fresh world into the env's own geometry block (maze.cuh) from their level's templates; Maze variants whose
-// templates do not reproduce the host exactly reset on the host and arrive through mwb_set_world instead.
+// templates do not reproduce the host exactly reset on the host and arrive through mwb_set_world instead.  With maze layouts
+// on (mwb_enable_maze_layouts) a Maze reset can instead build a layout written into next_maze (take_maze, maze_design),
+// with the goal box and the agent in the layout's cells.
 #pragma once
 #include "maze.cuh"
 #include "physics.cuh"
@@ -103,6 +105,35 @@ MWB_DEV void take_seed(const DevState& S, int i) {
   MWB_WARP_SYNC();
 }
 
+// Room of flat layout cell f (j * cols_max + i) in a level of R x C cells, -1 when f is outside the grid.
+MWB_DEV int layout_cell_room(int f, int cols_max, int R, int C) {
+  return f >= 0 && f / cols_max < R && f % cols_max < C ? (f / cols_max) * C + f % cols_max : -1;
+}
+
+// The layout env i's reset at a level of R x C cells builds (mwb_enable_maze_layouts; include/mwb.h states the rule; R = 0
+// for a level that is not a Maze).  At a Maze level a pending layout is taken: its copy masked to the grid becomes the
+// episode's layout (episode_maze, which maze_design then reads), and the return value is 1.  Otherwise it returns 0: a
+// Maze level carves (maze_generate records the topology), and any other level writes zeros and leaves a pending layout
+// waiting.  As in take_seed, every lane computes the same values from the same loads, and warp barriers separate the
+// loads from the stores.
+MWB_DEV int take_maze(uint8_t* pending_flag, const uint8_t* next, uint8_t* episode, int rows_max, int cols_max, int R,
+                      int C) {
+  MWB_WARP_SYNC();
+  const bool take = R > 0 && *pending_flag != 0;
+  if (R > 0 && !take) return 0;
+  for (int j = 0; j < rows_max; ++j)
+    for (int ci = 0; ci < cols_max; ++ci) {
+      int b = take && j < R && ci < C ? next[j * cols_max + ci] & 3 : 0;
+      if (ci + 1 >= C) b &= ~1;
+      if (j + 1 >= R) b &= ~2;
+      episode[j * cols_max + ci] = (uint8_t)b;
+    }
+  MWB_WARP_SYNC();
+  if (take) *pending_flag = 0;
+  MWB_WARP_SYNC();
+  return take ? 1 : 0;
+}
+
 MWB_DEV void device_reset(const DevState& S, int i) {
   const size_t N = S.N;
   if (S.next_seed) take_seed(S, i);
@@ -119,6 +150,17 @@ MWB_DEV void device_reset(const DevState& S, int i) {
   const int g = geom_block(S, i, lvl);
   const mwb_room* rooms = S.rooms + (size_t)g * S.R;
   int n_rooms = S.num_rooms[g];
+  // bit 0: the rooms' textures are drawn (_gen_static_data ran); bits 1 / 2: a designed maze's goal / agent cell is
+  // still to be placed (one variable, so that the designed path adds no register to the loop below)
+  int flags = 0;
+  if (S.layouts) {
+    const MazeLayouts& Y = *S.layouts;
+    const size_t cells = (size_t)Y.rows * Y.cols;
+    const bool maze = L.maze >= 0 && L.env_worlds;
+    if (take_maze(Y.pending + i, Y.next + cells * i, Y.episode + cells * i, Y.rows, Y.cols,
+                  maze ? S.maze[L.maze].rows : 0, maze ? S.maze[L.maze].cols : 0))
+      flags = 6;
+  }
 
   S.step_count[i] = 0;
   S.carrying[i] = -1;
@@ -139,14 +181,22 @@ MWB_DEV void device_reset(const DevState& S, int i) {
 
   int ireg[8];
   double freg[8];
-  bool static_done = false;
   int slots = 0;
 
   for (int pc = 0; pc < num_ops; ++pc) {
     const mwb_op& op = ops[pc];
     if (op.op == MWB_OP_END) break;
     if (op.op == MWB_OP_MAZE) {          // per-episode topology: regenerate this env's rooms
-      if (L.maze >= 0 && L.env_worlds && maze_generate(S, S.maze[L.maze], S.maze_cdf + (size_t)L.maze * MWB_MAZE_CDF_STRIDE, g, rng)) {
+      // (a Maze program's first op: flags holds only the designed bits here)
+      const bool built =
+          L.maze >= 0 && L.env_worlds &&
+          (flags ? maze_design(S.maze + L.maze, S.layouts->episode + (size_t)S.layouts->rows * S.layouts->cols * i,
+                               S.layouts->cols, S.rooms + (size_t)g * S.R, S.quads + (size_t)g * S.Q,
+                               S.segs + (size_t)g * S.S, S.R, S.Q, S.S, S.num_rooms + g, S.num_quads + g, S.num_segs + g)
+                 : maze_generate(S, S.maze[L.maze], S.maze_cdf + (size_t)L.maze * MWB_MAZE_CDF_STRIDE, g, rng,
+                                 S.layouts ? S.layouts->episode + (size_t)S.layouts->rows * S.layouts->cols * i : nullptr,
+                                 S.layouts ? S.layouts->rows : 0, S.layouts ? S.layouts->cols : 0));
+      if (built) {
         n_rooms = S.num_rooms[g];
       } else {
         // out of capacity (unreachable when the host sized the handle from a generated maze, mwb_set_maze): placing
@@ -166,9 +216,9 @@ MWB_DEV void device_reset(const DevState& S, int i) {
       continue;
     }
     if (op.op == MWB_OP_PUT) {
-      if (!static_done && op.b == 0) {
+      if (!(flags & 1) && op.b == 0) {
         draw_room_textures(S, i, rooms, n_rooms, L.domain_rand != 0, rng);
-        static_done = true;
+        flags |= 1;
       }
       const mwb_proto& pr = S.protos[op.a];
       const double dir = isnan(op.f[3]) ? rng_uniform(rng, -3.141592653589793, d_sub(3.141592653589793, -3.141592653589793))
@@ -189,9 +239,9 @@ MWB_DEV void device_reset(const DevState& S, int i) {
     } else if (op.op == MWB_OP_UNIFORM) {
       freg[op.a & 7] = rng_uniform(rng, op.f[0], d_sub(op.f[1], op.f[0]));
     } else if (op.op == MWB_OP_PLACE) {
-      if (!static_done) {
+      if (!(flags & 1)) {
         draw_room_textures(S, i, rooms, n_rooms, L.domain_rand != 0, rng);
-        static_done = true;
+        flags |= 1;
       }
       int proto = op.a;
       if (op.ireg_a >= 0) proto += ireg[op.ireg_a & 7] * op.stride_a;
@@ -202,7 +252,14 @@ MWB_DEV void device_reset(const DevState& S, int i) {
       // a Box whose edge length the level drew for this episode (op.b = 1 + freg): Box.__init__'s radius
       const double size = op.b > 0 ? freg[(op.b - 1) & 7] : 0.0;
       const double rad = size > 0.0 ? d_div(d_sqrt(d_add(d_mul(size, size), d_mul(size, size))), 2.0) : pr.radius;
-      place_search(S, i, rng, rooms, n_rooms, op.room, op.f, rad, pr.radius_is_f32 != 0,
+      // a designed maze's cells: the agent's PLACE takes the agent cell, the first other PLACE (the goal box) the goal cell
+      int room = op.room;
+      if (flags & (op.is_agent ? 4 : 2)) {
+        const MazeDev& M = S.maze[L.maze];
+        room = layout_cell_room(S.layouts->cells[2 * (size_t)i + (op.is_agent ? 1 : 0)], S.layouts->cols, M.rows, M.cols);
+        flags &= op.is_agent ? ~4 : ~2;
+      }
+      place_search(S, i, rng, rooms, n_rooms, room, op.f, rad, pr.radius_is_f32 != 0,
                    op.dir_freg >= 0 ? freg[op.dir_freg & 7] : MWB_NAN, x, z, dir);
       int e = slots++;
       S.ent_size[e * N + i] = size;
@@ -244,3 +301,4 @@ MWB_DEV void device_reset(const DevState& S, int i) {
   }
   store_rng(S, i, rng);
 }
+

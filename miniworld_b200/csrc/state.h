@@ -22,6 +22,16 @@
 #define MWB_WARP_SYNC()
 #endif
 
+// The maze layout arrays (mwb_enable_maze_layouts).  A layout is rows x cols bytes (the maxima over the handle's Maze
+// levels), bit 0 of cell (j, i) opening its +x wall, bit 1 its +z wall.
+struct MazeLayouts {
+  uint8_t* next;                // [N][rows][cols] layout the env's next reset at a Maze level builds
+  int32_t* cells;               // [N][2] goal cell, agent cell of that layout (j * cols + i), -1 = random
+  uint8_t* pending;             // [N] 1 = next[i] waits for the env's next reset at a Maze level
+  uint8_t* episode;             // [N][rows][cols] layout of the env's running episode (zeros: no maze)
+  int32_t rows, cols;
+};
+
 struct TriRec;
 struct MeshSegInfo;
 struct MazeDev;
@@ -128,6 +138,9 @@ struct DevState {
   // episode seeds (mwb_enable_episode_seeds); null on a handle without them
   int64_t* next_seed;           // [N] seed the env's next reset starts its stream from, negative = none
   int64_t* episode_seed;        // [N] seed the env's current episode started from, -1 = it continued its stream
+  // maze layouts (mwb_enable_maze_layouts); null on a handle without them.  One pointer to a device-side record rather
+  // than its fields: every byte of DevState is a kernel parameter of every launch
+  const struct MazeLayouts* layouts;
   int32_t autoreset;
   // StochasticActionWrapper on the device (reference wrappers.py:49-71): per step one uniform() draw from
   // the env's own stream; below act_prob the chosen action stands, else act_random (< 0: integers(0, 6))

@@ -135,7 +135,7 @@ EXPORTS = (
     "mwb_snapshot_size", "mwb_snapshot", "mwb_restore", "mwb_set_obs_format",
     "mwb_flag_write", "mwb_flag_wait_geq", "mwb_flag_mode", "mwb_state_array", "mwb_debug_camera", "mwb_set_obs_peer",
     "mwb_set_levels", "mwb_enable_level_changes", "mwb_state_in_host_memory", "mwb_set_level_maze",
-    "mwb_enable_episode_seeds",
+    "mwb_enable_episode_seeds", "mwb_enable_maze_layouts",
 )
 OBS_FORMATS = {"hwc": 0, "cwh": 1, "grey": 2}
 
@@ -175,6 +175,7 @@ def load_library():
     lib.mwb_set_levels.argtypes = [vp, C.c_int, vp, vp, vp, C.c_int, vp]
     lib.mwb_enable_level_changes.argtypes = [vp, C.c_uint64, C.c_int32]
     lib.mwb_enable_episode_seeds.argtypes = [vp]
+    lib.mwb_enable_maze_layouts.argtypes = [vp]
     lib.mwb_state_in_host_memory.argtypes = []
     lib.mwb_seed.argtypes = [vp, vp, C.c_int, vp]
     lib.mwb_reset.argtypes = [vp, vp, C.c_int, vp]
@@ -482,6 +483,12 @@ class Engine:
         (mwb_enable_episode_seeds); needs device resets."""
         self._check(self.lib.mwb_enable_episode_seeds(self.h))
 
+    def enable_maze_layouts(self):
+        """Resets at Maze levels build a pending layout from "next_maze" / "next_maze_cells" / "maze_pending" and record
+        every episode's layout in "episode_maze" from now on (mwb_enable_maze_layouts); needs device resets, a Maze
+        level and capacities that fit its all-open maze."""
+        self._check(self.lib.mwb_enable_maze_layouts(self.h))
+
     # ---- reset
     def seed(self, env_ids, states):
         ids = np.ascontiguousarray(env_ids, np.int32)
@@ -562,20 +569,25 @@ class Engine:
     ARRAYS = {"counter": (0, "<i4", "env"), "step_count": (1, "<i4", "env"), "ent_x": (2, "<f8", "env"),
               "ent_y": (3, "<f8", "env"), "ent_z": (4, "<f8", "env"), "ent_dir": (5, "<f8", "env"),
               "env_level": (6, "<i4", "env"), "next_level": (7, "<i4", "env"), "level_weights": (8, "<f4", "level"),
-              "level_params": (9, "<f8", "params"), "next_seed": (16, "<i8", "env"), "episode_seed": (17, "<i8", "env")}
+              "level_params": (9, "<f8", "params"), "next_seed": (16, "<i8", "env"), "episode_seed": (17, "<i8", "env"),
+              "next_maze": (18, "|u1", "env_rows"), "next_maze_cells": (19, "<i4", "env_rows"),
+              "maze_pending": (20, "|u1", "env"), "episode_maze": (21, "|u1", "env_rows")}
 
     def state_array(self, name):
         """Zero-copy view of a state array (mwb_state_array) as an object with __cuda_array_interface__:
         "counter" / "step_count" int32 [N]; "ent_x|y|z|dir" float64 [max_ents, N]; with level changes on,
         "env_level" / "next_level" int32 [N] and "level_weights" float32 [n_levels]; with device resets,
         "level_params" float64 [n_levels, PARAMS_DOUBLES] (column of a field: PARAMS_COLUMN); with episode seeds on,
-        "next_seed" / "episode_seed" int64 [N].  On the host build of
+        "next_seed" / "episode_seed" int64 [N]; with maze layouts on, "next_maze" / "episode_maze" uint8
+        [N, rows * cols], "next_maze_cells" int32 [N, 2] and "maze_pending" uint8 [N].  On the host build of
         the kernels the arrays live in host memory, and the view is a numpy array over the same memory instead."""
         which, typestr, axis = self.ARRAYS[name]
         ptr, count = C.c_void_p(), C.c_int64()
         self._check(self.lib.mwb_state_array(self.h, which, C.byref(ptr), C.byref(count)))
         if axis == "params":
             shape = (count.value, PARAMS_DOUBLES)
+        elif axis == "env_rows":
+            shape = (self.N, count.value // self.N)
         elif axis == "level" or count.value == self.N:
             shape = (count.value,)
         else:

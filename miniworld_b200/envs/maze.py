@@ -1,4 +1,6 @@
 """MiniWorld-Maze-v0 family: recursive-backtracker maze of 3x3 m cells (reference envs/maze.py)."""
+import numpy as np
+
 from .._gym import spaces, utils
 from ..entity import Box
 from ..params import DEFAULT_PARAMS
@@ -17,6 +19,7 @@ class Maze(GoalBoxRule, MiniWorldEnv, utils.EzPickle):
         self.action_space = spaces.Discrete(self.actions.move_forward + 1)
 
     def _gen_world(self):
+        """The recursive-backtracker carve, or with reset(options={"maze": ...}) a designed layout (_build_layout)."""
         pitch = self.room_size + self.gap_size
         grid = []
         for j in range(self.num_rows):
@@ -27,6 +30,10 @@ class Maze(GoalBoxRule, MiniWorldEnv, utils.EzPickle):
                                               min_z=min_z, max_z=min_z + self.room_size,
                                               wall_tex="brick_wall"))
             grid.append(row)
+        options = getattr(self, "reset_options", None) or {}
+        if "maze" in options:
+            self._build_layout(grid, options)
+            return
         seen = set()
 
         def carve(i, j):
@@ -54,6 +61,28 @@ class Maze(GoalBoxRule, MiniWorldEnv, utils.EzPickle):
         carve(0, 0)
         self.box = self.place_entity(Box(color="red"))
         self.place_agent()
+
+    def _build_layout(self, grid, options):
+        """The maze of a designed layout (options "maze": uint8 [rows, cols] or larger, bit 0 of cell (j, i) opening the
+        wall to (j, i + 1), bit 1 the wall to (j + 1, i); cells and bits outside the grid are ignored) with the goal box
+        in cell "goal_cell" and the agent in cell "agent_cell" (flat j * layout_cols + i; -1, absent or outside the grid:
+        anywhere).  No carve draws; loops, isolated cells and unreachable goals are allowed."""
+        layout = np.asarray(options["maze"])
+        R, C = self.num_rows, self.num_cols
+        for j in range(R):
+            for i in range(C):
+                cell, bits = grid[j][i], int(layout[j, i]) if j < layout.shape[0] and i < layout.shape[1] else 0
+                if bits & 1 and i + 1 < C:
+                    self.connect_rooms(cell, grid[j][i + 1], min_z=cell.min_z, max_z=cell.max_z)
+                if bits & 2 and j + 1 < R:
+                    self.connect_rooms(cell, grid[j + 1][i], min_x=cell.min_x, max_x=cell.max_x)
+
+        def room_of(key):
+            f = int(options.get(key, -1))
+            j, i = divmod(f, layout.shape[1])
+            return grid[j][i] if f >= 0 and j < R and i < C else None
+        self.box = self.place_entity(Box(color="red"), room=room_of("goal_cell"))
+        self.place_agent(room=room_of("agent_cell"))
 
     def device_program(self, prog):
         """Topology is random per episode: the carving itself is lowered (csrc/maze.cuh), using

@@ -162,6 +162,47 @@ class MazeTemplate:
             out.append(best)
         return out
 
+    def layout_of(self, connections):
+        """uint8 [rows, cols] layout (bit 0: wall to (j, i + 1) open, bit 1: wall to (j + 1, i) open) of connections
+        (i, j, dir): a connector in direction d opens the +x or +z bit of the cell on its -x / -z side."""
+        out = np.zeros((self.rows, self.cols), np.uint8)
+        for i, j, d in connections:
+            dj, di = DIRS[d]
+            if dj == 0:
+                out[j, min(i, i + di)] |= 1
+            else:
+                out[min(j, j + dj), i] |= 2
+        return out
+
+    def layout_connections(self, layout):
+        """The connections a designed reset creates from `layout`, in its order: per cell in row-major order, +x
+        (template direction 0), then +z (direction 3); bits that point outside the grid are ignored."""
+        out = []
+        for j in range(self.rows):
+            for i in range(self.cols):
+                bits = int(layout[j, i])
+                if bits & 1 and i + 1 < self.cols:
+                    out.append((i, j, 0))
+                if bits & 2 and j + 1 < self.rows:
+                    out.append((i, j, 3))
+        return out
+
+    def verify_layouts(self, layouts):
+        """Assembling the canonical connections of each layout reproduces the world the host builds from it
+        (Maze.reset(options={"maze": layout})) field for field."""
+        for layout in layouts:
+            env = self.level_cls(device=None, **self.kwargs)
+            env.reset(seed=0, options={"maze": layout})
+            want = pack.pack_geometry(env)
+            got = self.assemble(self.layout_connections(layout))
+            for w, g, name in zip(want, got, ("rooms", "quads", "segs")):
+                assert len(w) == len(g), (name, len(w), len(g))
+                for field in w.dtype.names:
+                    if field in ("cdf", "reserved"):
+                        continue
+                    assert np.array_equal(w[field], g[field]), (name, field)
+        return True
+
     def verify(self, seeds=(0, 1, 2)):
         """Translating the templates reproduces host-generated mazes field for field."""
         for seed in seeds:

@@ -211,6 +211,7 @@ class MiniWorldEnv(gym.Env):
         self.entities = []
         self.rooms = []
         self.wall_segs = []
+        self.reset_options = options        # what the level's _gen_world may read (Maze: a designed layout)
         self._gen_world()
 
         rand = self.np_random if self.domain_rand else None
