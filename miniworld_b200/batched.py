@@ -159,6 +159,44 @@ def default_env_level(num_envs, n_levels):
     return np.repeat(np.arange(n_levels, dtype=np.int32), [base + (1 if k < extra else 0) for k in range(n_levels)])
 
 
+# the flag a run-time array needs, and what its accessor raises on a batch built without it
+_NEEDS = {**dict.fromkeys(("env_level", "next_level", "level_weights"), (
+              "dynamic_levels", RuntimeError, "levels are fixed in this batch: construct it with dynamic_levels=True")),
+          **dict.fromkeys(("next_seed", "episode_seed"), (
+              "episode_seeds", RuntimeError, "this batch has no episode seeds: construct it with episode_seeds=True")),
+          **dict.fromkeys(("next_maze", "next_maze_cells", "maze_pending", "episode_maze"), (
+              "maze_layouts", RuntimeError, "this batch has no maze layouts: construct it with maze_layouts=True")),
+          "level_params": ("device_reset", TypeError, "level params change at device resets; host-reset levels draw "
+                           "theirs in Python (set them on the level's own DomainParams)")}
+
+
+class _Views(dict):
+    """Array name -> in-place view of one handle's state array (Engine.ARRAYS) in its final shape: a torch CUDA tensor,
+    or a numpy array on the kernels' host build (whose state lives in host memory).  A view is made at the first lookup
+    of its name, which raises as _NEEDS says when the batch lacks the array's mode; later lookups are dict lookups."""
+
+    def __init__(self, engine, device, flags, maze_shape):
+        super().__init__()
+        self._engine, self._device, self._flags, self._maze_shape = engine, device, flags, maze_shape
+
+    def __missing__(self, name):
+        need = _NEEDS.get(name)
+        if need is not None and not self._flags[need[0]]:
+            raise need[1](need[2])
+        shape = (self._engine.N,) + self._maze_shape if name in ("next_maze", "episode_maze") else None
+        view = self._engine.state_array(name, shape)
+        if not self._engine.host_memory:
+            import torch
+            view = torch.as_tensor(view, device=torch.device("cuda", self._device))
+        self[name] = view
+        return view
+
+
+def _host(a):
+    """`a` as a numpy array, copied from a torch tensor first when it is one."""
+    return np.asarray(a.cpu() if hasattr(a, "cpu") else a)
+
+
 class BatchedMiniWorld:
     """`level`: a level id or class, or a sequence of them to run several levels side by side in one batch (multi-task
     or curriculum training; env i runs level `env_level[i]`).  With a sequence, `level_kwargs` may be a sequence
@@ -226,17 +264,17 @@ class BatchedMiniWorld:
         if self.maze_layouts:
             self._size_for_layouts(defs)
         self._init_engine(defs, table, msaa_samples, autoreset)
-        self._level_views = None
+        self._view_map = _Views(self.engine, self.device, dict(
+            dynamic_levels=self.dynamic_levels, episode_seeds=self.episode_seeds, maze_layouts=self.maze_layouts,
+            device_reset=self.device_reset), getattr(self, "maze_shape", None))
         if self.dynamic_levels:
             self.level_seed, self.env_offset = int(level_seed), int(env_offset)
             self.engine.enable_level_changes(self.level_seed, self.env_offset)
-        self._seed_views = None
         if self.episode_seeds:
             if not self.device_reset:
                 self.engine.close()
                 raise TypeError("episode seeds are taken by device resets; host-reset levels keep RNG streams in Python")
             self.engine.enable_episode_seeds()
-        self._maze_views = None
         if self.maze_layouts:
             self.engine.enable_maze_layouts()
         # observation layout written by the render kernel: the reference's PyTorchObsWrapper ("cwh") and
@@ -250,7 +288,6 @@ class BatchedMiniWorld:
         self._seeded = False
         self._torch = None
         self._bufs = None
-        self._params_view = None
         self._params_written = False
 
     def _init_level(self, level, level_kwargs):
@@ -404,14 +441,12 @@ class BatchedMiniWorld:
             self._bufs["trunc_view"] = self._bufs["truncated"].view(torch.bool)
             self._info = {"depth": self._bufs["depth"]} if self.want_depth else {}
             # what the level's step() puts into `info` / the observation, read in place from the device state
-            eng = self.engine
             self._info_views = {}
             for key, spec in self._device_info.items():
                 if spec[0] == "counter":                   # CollectHealth: info["health"] (collecthealth.py:100)
-                    self._info[key] = torch.as_tensor(eng.state_array("counter"), device=dev)
+                    self._info[key] = self._views()["counter"]
                 elif spec[0] == "entity_pos":              # TMaze: info["goal_pos"] = self.box.pos (tmaze.py:89)
-                    self._info_views[key] = (int(spec[1]), [torch.as_tensor(eng.state_array(n), device=dev)
-                                                            for n in ("ent_x", "ent_y", "ent_z")])
+                    self._info_views[key] = (int(spec[1]), [self._views()[n] for n in ("ent_x", "ent_y", "ent_z")])
             self._obs_dict = dict(self._device_obs_extra)
             if self.dynamic_levels:
                 # the level of each env's current episode (after a terminating step still the one that just ended)
@@ -424,22 +459,38 @@ class BatchedMiniWorld:
                 self._info["maze"] = self.episode_maze
         return self._torch
 
-    # ------------------------------------------------------------------ level changes (dynamic_levels=True)
+    # ------------------------------------------------------------------ run-time arrays
     def _views(self):
-        """env_level / next_level / level_weights in place: torch CUDA tensors, or numpy arrays on the kernels' host
-        build (whose state lives in host memory)."""
-        if not self.dynamic_levels:
-            raise RuntimeError("levels are fixed in this batch: construct it with dynamic_levels=True")
-        if self._level_views is None:
-            names = ("env_level", "next_level", "level_weights")
-            if self.engine.host_memory:
-                self._level_views = {n: self.engine.state_array(n) for n in names}
-            else:
-                import torch
-                dev = torch.device("cuda", self.device)
-                self._level_views = {n: torch.as_tensor(self.engine.state_array(n), device=dev) for n in names}
-        return self._level_views
+        """The batch's state arrays by name, in place and in their final shapes (_Views)."""
+        return self._view_map
 
+    def _write_pending(self, what, ids, arrays):
+        """The part set_env_level / set_env_seed / set_env_maze share: check the env ids `ids` (1-D integers in [0, N)),
+        then write each (array name, values) of `arrays` at those envs -- values one per id (a numpy array, or a CUDA
+        tensor) or one for all -- an env listed more than once taking its last entry.  On the host build the write is
+        numpy's; on the device it is torch ops on the current stream, without a sync."""
+        if not np.issubdtype(ids.dtype, np.integer) or ids.ndim != 1:
+            raise ValueError("%s takes a 1-D sequence of integer env ids" % what)
+        if ids.size and (ids.min() < 0 or ids.max() >= self.num_envs):
+            raise ValueError("env ids must lie in [0, %d)" % self.num_envs)
+        if ids.size == 0:
+            return
+        last = ids.size - 1 - np.unique(ids[::-1], return_index=True)[1]    # an env listed twice: its last entry wins
+        if self.engine.host_memory:
+            for name, vals in arrays:
+                self._views()[name][ids[last]] = vals[last] if np.ndim(vals) else vals
+            return
+        import torch
+        to_dev = lambda a: torch.as_tensor(a).to(torch.device("cuda", self.device), non_blocking=True)
+        idx = to_dev(ids[last].astype(np.int64))
+        for name, vals in arrays:
+            if torch.is_tensor(vals):
+                vals = vals[to_dev(last)] if vals.dim() else vals
+            elif np.ndim(vals):
+                vals = to_dev(np.ascontiguousarray(vals[last]))
+            self._views()[name][idx] = vals
+
+    # ------------------------------------------------------------------ level changes (dynamic_levels=True)
     @property
     def level_tensor(self):
         """int32 [N] view of each env's current level (changes only at the env's resets)."""
@@ -472,21 +523,11 @@ class BatchedMiniWorld:
             raise ValueError("set_env_level: %d env ids but %d levels" % (ids.size, lv.size))
         if ids.size == 0:
             return
-        if not (np.issubdtype(ids.dtype, np.integer) and np.issubdtype(lv.dtype, np.integer)):
+        if not np.issubdtype(lv.dtype, np.integer):
             raise ValueError("set_env_level takes integer env ids and levels")
-        if ids.min() < 0 or ids.max() >= self.num_envs:
-            raise ValueError("env ids must lie in [0, %d)" % self.num_envs)
         if lv.min() < 0 or lv.max() >= len(self.level_ids):
             raise ValueError("levels must lie in [0, %d)" % len(self.level_ids))
-        last = ids.size - 1 - np.unique(ids[::-1], return_index=True)[1]    # an env listed twice: its last entry wins
-        ids, lv = ids[last], lv[last]
-        view = self._views()["next_level"]
-        if isinstance(view, np.ndarray):
-            view[ids] = lv.astype(np.int32)
-        else:
-            import torch
-            view[torch.as_tensor(ids.astype(np.int64), device=view.device)] = torch.as_tensor(
-                lv.astype(np.int32), device=view.device)
+        self._write_pending("set_env_level", ids, [("next_level", lv.astype(np.int32))])
 
     @property
     def env_level(self):
@@ -498,57 +539,30 @@ class BatchedMiniWorld:
         return np.array(view) if isinstance(view, np.ndarray) else view.cpu().numpy()
 
     # ------------------------------------------------------------------ episode seeds (episode_seeds=True)
-    def _seeds(self):
-        """next_seed / episode_seed in place, made like `_views`: torch CUDA tensors, or numpy arrays on the kernels'
-        host build."""
-        if not self.episode_seeds:
-            raise RuntimeError("this batch has no episode seeds: construct it with episode_seeds=True")
-        if self._seed_views is None:
-            names = ("next_seed", "episode_seed")
-            if self.engine.host_memory:
-                self._seed_views = {n: self.engine.state_array(n) for n in names}
-            else:
-                import torch
-                dev = torch.device("cuda", self.device)
-                self._seed_views = {n: torch.as_tensor(self.engine.state_array(n), device=dev) for n in names}
-        return self._seed_views
-
     @property
     def next_seed(self):
         """int64 [N] view of the seed each env's next reset starts from; write it in place (stream-ordered, no sync).
         A negative entry means none: the env continues its stream.  The reset that takes an entry clears it to -1."""
-        return self._seeds()["next_seed"]
+        return self._views()["next_seed"]
 
     @property
     def episode_seed(self):
         """int64 [N] view of the seed each env's current episode started from, -1 when it continued its stream."""
-        return self._seeds()["episode_seed"]
+        return self._views()["episode_seed"]
 
     def set_env_seed(self, env_ids, seeds):
         """Start the listed envs' next episodes from `seeds` (one seed, or one per env), as `reset(seed=s)` would; envs
         in mid-episode finish it first.  An env listed more than once takes its last entry.  `seeds` given as a CUDA
         tensor are written as they are (a negative entry means none); host values must lie in [0, 2**63)."""
-        view = self.next_seed
-        on_device = hasattr(seeds, "is_cuda") and seeds.is_cuda
-        ids = np.atleast_1d(np.asarray(env_ids.cpu() if hasattr(env_ids, "cpu") else env_ids))
-        if not np.issubdtype(ids.dtype, np.integer):
-            raise ValueError("set_env_seed takes integer env ids")
-        if ids.size and (ids.min() < 0 or ids.max() >= self.num_envs):
-            raise ValueError("env ids must lie in [0, %d)" % self.num_envs)
-        if not on_device:
+        self._views()["next_seed"]                   # a batch without the mode raises before any input check
+        ids = np.atleast_1d(_host(env_ids))
+        if not (hasattr(seeds, "is_cuda") and seeds.is_cuda):
             seeds = self._host_seeds(seeds.cpu().numpy() if hasattr(seeds, "cpu") else seeds, ids.shape)
         elif seeds.dim() and tuple(seeds.shape) != ids.shape:
             raise ValueError("set_env_seed: %d env ids but %d seeds" % (ids.size, seeds.numel()))
-        if ids.size == 0:
-            return
-        last = ids.size - 1 - np.unique(ids[::-1], return_index=True)[1]    # an env listed twice: its last entry wins
-        if isinstance(view, np.ndarray):
-            view[ids[last]] = seeds[last]
         else:
-            torch = self._ensure_torch()
-            to_dev = lambda a: torch.as_tensor(a, dtype=torch.int64).to(view.device, non_blocking=True)
-            s = seeds.to(torch.int64) if on_device else to_dev(seeds)
-            view[to_dev(ids[last].astype(np.int64))] = s[to_dev(last)] if s.dim() else s
+            seeds = seeds.long()
+        self._write_pending("set_env_seed", ids, [("next_seed", seeds)])
 
     @staticmethod
     def _host_seeds(seeds, shape):
@@ -566,57 +580,35 @@ class BatchedMiniWorld:
         return arr
 
     # ------------------------------------------------------------------ maze layouts (maze_layouts=True)
-    def _mazes(self):
-        """next_maze / next_maze_cells / maze_pending / episode_maze in place, made like `_views`: torch CUDA tensors,
-        or numpy arrays on the kernels' host build."""
-        if not self.maze_layouts:
-            raise RuntimeError("this batch has no maze layouts: construct it with maze_layouts=True")
-        if self._maze_views is None:
-            shapes = {"next_maze": (self.num_envs,) + self.maze_shape, "next_maze_cells": (self.num_envs, 2),
-                      "maze_pending": (self.num_envs,), "episode_maze": (self.num_envs,) + self.maze_shape}
-            if self.engine.host_memory:
-                self._maze_views = {n: self.engine.state_array(n).reshape(shp) for n, shp in shapes.items()}
-            else:
-                import torch
-                dev = torch.device("cuda", self.device)
-                self._maze_views = {n: torch.as_tensor(self.engine.state_array(n), device=dev).view(shp)
-                                    for n, shp in shapes.items()}
-        return self._maze_views
-
     @property
     def next_maze(self):
         """uint8 [N, rows, cols] view of the layout each env's next reset at a Maze level builds once `maze_pending` is
         set; write it in place (stream-ordered, no sync)."""
-        return self._mazes()["next_maze"]
+        return self._views()["next_maze"]
 
     @property
     def next_maze_cells(self):
         """int32 [N, 2] view of (goal cell, agent cell) of each pending layout: j * cols + i, or -1 for anywhere."""
-        return self._mazes()["next_maze_cells"]
+        return self._views()["next_maze_cells"]
 
     @property
     def maze_pending(self):
         """uint8 [N] view: nonzero when next_maze[i] waits for env i's next reset at a Maze level, which clears it."""
-        return self._mazes()["maze_pending"]
+        return self._views()["maze_pending"]
 
     @property
     def episode_maze(self):
         """uint8 [N, rows, cols] view of the layout of each env's running episode (zeros at levels that are not Mazes)."""
-        return self._mazes()["episode_maze"]
+        return self._views()["episode_maze"]
 
     def set_env_maze(self, env_ids, layouts, goal_cell=-1, agent_cell=-1):
         """Build the listed envs' next mazes from `layouts` (one uint8 [rows, cols] layout, or one per env) with the
         goal box in `goal_cell` and the agent in `agent_cell` (one flat cell j * cols + i, or one per env; -1 for
         anywhere); envs in mid-episode finish it first.  An env listed more than once takes its last entry.  The input
         is checked on the host, then written with torch ops on the current stream, without a sync."""
-        views = self._mazes()
-        ids = np.atleast_1d(np.asarray(env_ids.cpu() if hasattr(env_ids, "cpu") else env_ids))
-        if not np.issubdtype(ids.dtype, np.integer) or ids.ndim != 1:
-            raise ValueError("set_env_maze takes a 1-D sequence of integer env ids")
-        if ids.size and (ids.min() < 0 or ids.max() >= self.num_envs):
-            raise ValueError("env ids must lie in [0, %d)" % self.num_envs)
-        host = lambda a: np.asarray(a.cpu() if hasattr(a, "cpu") else a)
-        lay = host(layouts)
+        self._views()["next_maze"]                   # a batch without the mode raises before any input check
+        ids = np.atleast_1d(_host(env_ids))
+        lay = _host(layouts)
         if not (np.issubdtype(lay.dtype, np.integer) or lay.dtype == np.bool_):
             raise ValueError("maze layouts are integer arrays (uint8), got %s" % lay.dtype)
         if lay.shape == self.maze_shape:
@@ -629,45 +621,17 @@ class BatchedMiniWorld:
         n_cells = self.maze_shape[0] * self.maze_shape[1]
         cells = []
         for name, c in (("goal_cell", goal_cell), ("agent_cell", agent_cell)):
-            c = host(c)
+            c = _host(c)
             if not np.issubdtype(c.dtype, np.integer) or c.ndim > 1 or (c.ndim == 1 and c.shape != ids.shape):
                 raise ValueError("%s is one integer or one per env id" % name)
             if c.size and (c.min() < -1 or c.max() >= n_cells):
                 raise ValueError("%s entries must lie in [-1, %d)" % (name, n_cells))
             cells.append(np.broadcast_to(c, ids.shape))
-        if ids.size == 0:
-            return
-        last = ids.size - 1 - np.unique(ids[::-1], return_index=True)[1]    # an env listed twice: its last entry wins
-        ids, lay = ids[last], np.ascontiguousarray(lay[last], np.uint8)
-        both = np.ascontiguousarray(np.stack([c[last] for c in cells], axis=1), np.int32)
-        if isinstance(views["next_maze"], np.ndarray):
-            views["next_maze"][ids] = lay
-            views["next_maze_cells"][ids] = both
-            views["maze_pending"][ids] = 1
-        else:
-            torch = self._ensure_torch()
-            dev = views["next_maze"].device
-            to_dev = lambda a: torch.as_tensor(a).to(dev, non_blocking=True)
-            idx = to_dev(ids.astype(np.int64))
-            views["next_maze"][idx] = to_dev(lay)
-            views["next_maze_cells"][idx] = to_dev(both)
-            views["maze_pending"][idx] = 1
+        both = np.stack(cells, axis=1).astype(np.int32)
+        self._write_pending("set_env_maze", ids, [("next_maze", lay.astype(np.uint8, copy=False)),
+                                                  ("next_maze_cells", both), ("maze_pending", 1)])
 
     # ------------------------------------------------------------------ level params at run time
-    def _level_params(self):
-        """The device's params table as float64 [n_levels, words] (mwb_params records): a torch CUDA tensor, or a
-        numpy array on the kernels' host build."""
-        if not self.device_reset:
-            raise TypeError("level params change at device resets; host-reset levels draw theirs in Python "
-                            "(set them on the level's own DomainParams)")
-        if self._params_view is None:
-            view = self.engine.state_array("level_params")
-            if not self.engine.host_memory:
-                torch = self._ensure_torch()
-                view = torch.as_tensor(view, device=torch.device("cuda", self.device))
-            self._params_view = view
-        return self._params_view
-
     def set_level_param(self, level, name, default=None, min=None, max=None):
         """Change one DomainParams entry of level `level` while the batch runs (automatic domain randomisation).
         `name` is one of the twelve params the engine reads (engine.LOWERED_PARAMS) and must be a float param.  As
@@ -685,7 +649,7 @@ class BatchedMiniWorld:
         if isinstance(level, bool) or not (isinstance(level, (int, np.integer)) and 0 <= int(level) < n_levels):
             raise ValueError("level must be an int in [0, %d), got %r" % (n_levels, level))
         level = int(level)
-        view = self._level_params()
+        view = self._views()["level_params"]
         p = self.proto_envs[level].params.params[name]
         if p.type != "float":
             raise TypeError("%r of level %d is a %s param; only float params can be set" % (name, level, p.type))
@@ -712,7 +676,7 @@ class BatchedMiniWorld:
                     for key, v in given.items()}
             sub = np.subtract
         else:
-            torch = self._torch
+            torch = self._ensure_torch()
             vals = {key: torch.as_tensor(v, dtype=torch.float64).to(view.device, non_blocking=True).reshape(k)
                     for key, v in given.items()}
             sub = torch.sub
@@ -738,7 +702,7 @@ class BatchedMiniWorld:
         """Level `level`'s params as the device has them now, as a DomainParams (synchronises with the device).  The
         table holds min and max - min, so `max` is read back as min + (max - min), except forward_step's, which is
         max_forward_step.  The entries the engine does not read are the level's construction values."""
-        view = self._level_params()
+        view = self._views()["level_params"]
         row = np.array(view[level] if isinstance(view, np.ndarray) else view[level].cpu().numpy())
         out = DomainParams()
         out.params = dict(self.proto_envs[level].params.params)

@@ -14,6 +14,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <initializer_list>
 #include <string>
 #include <vector>
 
@@ -1316,23 +1317,39 @@ extern "C" int mwb_set_levels(mwb_handle* h, int n_levels, const mwb_level* leve
   return MWB_OK;
 }
 
+// The run-time control arrays a mode's enable call adds: with the handle drained, each of `bytes` bytes, zeros or, where
+// `minus_one`, all -1 (0xFF bytes).  `what` names the mode in the allocation error.
+struct ControlArray {
+  void** out;
+  size_t bytes;
+  bool minus_one;
+};
+static int alloc_control_arrays(mwb_handle* h, const char* what, std::initializer_list<ControlArray> arrays) {
+  int rc = drain(h);
+  if (rc) return rc;
+  for (const ControlArray& a : arrays) {
+    uint8_t* p = nullptr;
+    if (alloc_arr(h, &p, a.bytes)) return fail(MWB_ECUDA, std::string(what) + " state allocation failed");
+    if (a.minus_one && dev_memset(p, 0xFF, a.bytes) != 0) return fail(MWB_ECUDA, "memset failed");
+    *a.out = p;
+  }
+  return MWB_OK;
+}
+
 extern "C" int mwb_enable_level_changes(mwb_handle* h, uint64_t seed, int32_t env_offset) {
   if (!h) return fail(MWB_EINVAL, "null handle");
   if (!h->have_level_table) return fail(MWB_ESTATE, "level changes need a level table (mwb_set_levels first)");
   if (h->S.next_level) return fail(MWB_ESTATE, "level changes are already on");
   if (env_offset < 0) return fail(MWB_EINVAL, "env_offset must not be negative");
   DevState& S = h->S;
-  int rc = drain(h);
+  void *next, *draws, *weights;
+  int rc = alloc_control_arrays(h, "level-change", {{&next, S.N * sizeof(int32_t), true},
+                                                    {&draws, S.N * sizeof(uint32_t), false},
+                                                    {&weights, S.num_levels * sizeof(float), false}});
   if (rc) return rc;
-  int32_t* next = nullptr;
-  uint32_t* draws = nullptr;
-  float* weights = nullptr;
-  if (alloc_arr(h, &next, S.N) || alloc_arr(h, &draws, S.N) || alloc_arr(h, &weights, (size_t)S.num_levels))
-    return fail(MWB_ECUDA, "level-change state allocation failed");
-  if (dev_memset(next, 0xFF, (size_t)S.N * sizeof(int32_t)) != 0) return fail(MWB_ECUDA, "memset failed");   // all -1
-  S.next_level = next;
-  S.level_draws = draws;
-  S.level_weights = weights;       // zeros: no draws until weights are set
+  S.next_level = (int32_t*)next;
+  S.level_draws = (uint32_t*)draws;
+  S.level_weights = (float*)weights;       // zeros: no draws until weights are set
   S.level_seed = seed;
   S.level_env_offset = env_offset;
   return MWB_OK;
@@ -1345,15 +1362,12 @@ extern "C" int mwb_enable_episode_seeds(mwb_handle* h) {
     return fail(MWB_ESTATE, "episode seeds need device resets (params and a reset program: mwb_set_levels, or "
                             "mwb_set_params and mwb_set_program); host-generated worlds keep their streams on the host");
   DevState& S = h->S;
-  int rc = drain(h);
+  void *next, *episode;
+  int rc = alloc_control_arrays(h, "episode-seed", {{&next, S.N * sizeof(int64_t), true},
+                                                    {&episode, S.N * sizeof(int64_t), true}});
   if (rc) return rc;
-  int64_t* next = nullptr;
-  int64_t* episode = nullptr;
-  if (alloc_arr(h, &next, S.N) || alloc_arr(h, &episode, S.N)) return fail(MWB_ECUDA, "episode-seed state allocation failed");
-  if (dev_memset(next, 0xFF, (size_t)S.N * sizeof(int64_t)) != 0 || dev_memset(episode, 0xFF, (size_t)S.N * sizeof(int64_t)) != 0)
-    return fail(MWB_ECUDA, "memset failed");   // all -1
-  S.next_seed = next;
-  S.episode_seed = episode;
+  S.next_seed = (int64_t*)next;
+  S.episode_seed = (int64_t*)episode;
   return MWB_OK;
 }
 
@@ -1485,15 +1499,11 @@ extern "C" int mwb_enable_maze_layouts(mwb_handle* h) {
     cols = std::max(cols, m.cols);
   }
   if (rows == 0) return fail(MWB_ESTATE, "maze layouts need a Maze level (mwb_set_maze or mwb_set_level_maze)");
-  int rc = drain(h);
-  if (rc) return rc;
   const size_t N = S.N, cells = (size_t)rows * cols;
-  uint8_t *next = nullptr, *pending = nullptr, *episode = nullptr;
-  int32_t* next_cells = nullptr;
-  if (alloc_arr(h, &next, N * cells) || alloc_arr(h, &next_cells, 2 * N) || alloc_arr(h, &pending, N) ||
-      alloc_arr(h, &episode, N * cells))
-    return fail(MWB_ECUDA, "maze layout state allocation failed");
-  if (dev_memset(next_cells, 0xFF, 2 * N * sizeof(int32_t)) != 0) return fail(MWB_ECUDA, "memset failed");   // all -1
+  void *next, *next_cells, *pending, *episode;
+  int rc = alloc_control_arrays(h, "maze layout", {{&next, N * cells, false}, {&next_cells, 2 * N * sizeof(int32_t), true},
+                                                   {&pending, N, false}, {&episode, N * cells, false}});
+  if (rc) return rc;
   if (h->level_mazes) {   // K2's per-level capacity and the HBM lists from the all-open bound
     h->level_quads = quads;
     plan_k2(h);
@@ -1501,10 +1511,10 @@ extern "C" int mwb_enable_maze_layouts(mwb_handle* h) {
     k2_report(h);
   }
   MazeLayouts& Y = h->layouts_h;
-  Y.next = next;
-  Y.cells = next_cells;
-  Y.pending = pending;
-  Y.episode = episode;
+  Y.next = (uint8_t*)next;
+  Y.cells = (int32_t*)next_cells;
+  Y.pending = (uint8_t*)pending;
+  Y.episode = (uint8_t*)episode;
   Y.rows = rows;
   Y.cols = cols;
   MazeLayouts* d = nullptr;
@@ -2084,10 +2094,9 @@ extern "C" int mwb_visible_ents(mwb_handle* h, uint32_t* mask, void* stream) {
 }
 
 // ------------------------------------------------------------------ ABI: snapshot / restore
-// Every array that changes while episodes run (entity lists, counters, camera / lighting parameters, RNG
-// streams, pending-reset flags) plus the geometry currently on the device, in one fixed order.
-// the magic names the blob's mode: a handle with level changes on writes (and needs) the level-change section, and a
-// level table with Maze levels carries the per-env worlds after the templates
+// A header, then the sections of snapshot_sections in one fixed order.  The magic names the blob's mode: a handle
+// with level changes on writes (and needs) the level-change section, and a level table with Maze levels carries the
+// per-env worlds after the templates
 static const uint32_t kSnapMagic = 0x5342574du;               // "MWBS"
 static const uint32_t kSnapMagicLevelChanges = 0x4c42574du;   // "MWBL"
 static const uint32_t kSnapMagicWorlds = 0x5742574du;         // "MWBW": level table with per-env worlds
@@ -2124,27 +2133,31 @@ static size_t snapshot_blocks(const mwb_handle* h) {
   return h->cfg.shared_geometry && !h->level_mazes ? h->levels.size() : (size_t)h->S.env_geom + h->S.N;
 }
 
-// the level-change section of a snapshot: next_level [N], level_draws [N], level_weights [L], then this
+// the level-change section of a snapshot ends with this
 struct LevelChangeTail {
   uint64_t seed;
   int32_t env_offset, reserved;
 };
 
-// a handle with several levels appends its env_level [N] to the blob (checked on restore, never overwritten); one with
-// level changes on always does, followed by the level-change section (adopted on restore: the assignment is state)
-static size_t level_change_bytes(const mwb_handle* h) {
-  return (size_t)h->S.N * (sizeof(int32_t) + sizeof(uint32_t)) + (size_t)h->S.num_levels * sizeof(float) + sizeof(LevelChangeTail);
-}
-static size_t snapshot_level_bytes(const mwb_handle* h) {
-  const bool level_changes = h->S.next_level != nullptr;
-  const size_t assignment = h->levels.size() > 1 || level_changes ? h->env_level.size() * sizeof(int32_t) : 0;
-  return assignment + (level_changes ? level_change_bytes(h) : 0);
-}
+// One section of a snapshot blob: `bytes` bytes of device memory at `dev`, or of host memory at `host`.
+struct SnapSection {
+  void* dev;
+  void* host;
+  size_t bytes;
+};
 
-static void snapshot_arrays(mwb_handle* h, std::vector<std::pair<void*, size_t>>& v) {
+// The sections of a blob after its header, in blob order: every array that changes while episodes run (entity lists,
+// counters, camera / lighting parameters, RNG streams, pending-reset flags), the geometry currently on the device and
+// the level ranges, then the episode-seed and maze-layout arrays of handles with those modes on.  A handle with level
+// changes on closes the blob with its level-change section: env_level, next_level, level_draws, level_weights and
+// `tail` (adopted on restore: the assignment is state).  A static table of several levels closes it with the host's
+// env_level (checked on restore, never overwritten).
+static std::vector<SnapSection> snapshot_sections(mwb_handle* h, LevelChangeTail* tail) {
   const DevState& S = h->S;
   const size_t N = S.N, E = S.E, G = snapshot_blocks(h);
-#define SA(field, count) v.push_back(std::make_pair((void*)S.field, (size_t)(count) * sizeof(*S.field)))
+  std::vector<SnapSection> v;
+  auto dev = [&](const void* p, size_t bytes) { v.push_back(SnapSection{(void*)p, nullptr, bytes}); };
+#define SA(field, count) dev(S.field, (size_t)(count) * sizeof(*S.field))
   SA(ent_proto, E * N); SA(ent_px, E * N); SA(ent_py, E * N); SA(ent_pz, E * N); SA(ent_dir, E * N);
   SA(ent_col, E * 3 * N); SA(ent_size, E * N); SA(num_slots, N); SA(agent_slot, N); SA(carrying, N); SA(step_count, N);
   SA(num_picked, N); SA(needs_reset, N); SA(episodes_done, 1); SA(cam, 4 * N); SA(envp, 12 * N);
@@ -2155,75 +2168,66 @@ static void snapshot_arrays(mwb_handle* h, std::vector<std::pair<void*, size_t>>
   // the level ranges are run-time state (MWB_ARRAY_LEVEL_PARAMS), and so is what each env's last reset took from them
   SA(env_mfs, N); SA(level_params, h->levels.size());
   if (S.next_seed) { SA(next_seed, N); SA(episode_seed, N); }
-#undef SA
   if (S.layouts) {
     const MazeLayouts& Y = h->layouts_h;
     const size_t cells = (size_t)Y.rows * Y.cols;
-    v.push_back(std::make_pair((void*)Y.next, N * cells));
-    v.push_back(std::make_pair((void*)Y.cells, 2 * N * sizeof(int32_t)));
-    v.push_back(std::make_pair((void*)Y.pending, N));
-    v.push_back(std::make_pair((void*)Y.episode, N * cells));
+    dev(Y.next, N * cells); dev(Y.cells, 2 * N * sizeof(int32_t)); dev(Y.pending, N); dev(Y.episode, N * cells);
   }
+  if (S.next_level) {
+    SA(env_level, N); SA(next_level, N); SA(level_draws, N); SA(level_weights, S.num_levels);
+    v.push_back(SnapSection{nullptr, tail, sizeof(*tail)});
+  } else if (h->levels.size() > 1) {
+    v.push_back(SnapSection{nullptr, h->env_level.data(), h->env_level.size() * sizeof(int32_t)});
+  }
+#undef SA
+  return v;
 }
 
-static SnapHeader snapshot_header(mwb_handle* h) {
-  std::vector<std::pair<void*, size_t>> v;
-  snapshot_arrays(h, v);
+static SnapHeader snapshot_header(mwb_handle* h, const std::vector<SnapSection>& v) {
   SnapHeader hd;
   hd.magic = snapshot_magic(h);
   hd.abi = MWB_ABI_VERSION;
   hd.N = h->S.N; hd.E = h->S.E; hd.R = h->S.R; hd.Q = h->S.Q; hd.S = h->S.S;
   hd.G = (int32_t)snapshot_blocks(h);
-  hd.bytes = sizeof(SnapHeader) + snapshot_level_bytes(h);
-  for (size_t k = 0; k < v.size(); ++k) hd.bytes += v[k].second;
+  hd.bytes = sizeof(SnapHeader);
+  for (const SnapSection& s : v) hd.bytes += s.bytes;
   return hd;
 }
 
 extern "C" int mwb_snapshot_size(mwb_handle* h, size_t* bytes) {
   if (!h || !bytes) return fail(MWB_EINVAL, "null argument");
-  *bytes = (size_t)snapshot_header(h).bytes;
+  LevelChangeTail tail;
+  *bytes = (size_t)snapshot_header(h, snapshot_sections(h, &tail)).bytes;
   return MWB_OK;
 }
 
 extern "C" int mwb_snapshot(mwb_handle* h, void* blob, size_t bytes) {
   if (!h || !blob) return fail(MWB_EINVAL, "null argument");
-  const SnapHeader hd = snapshot_header(h);
+  LevelChangeTail tail;
+  memset(&tail, 0, sizeof(tail));
+  tail.seed = h->S.level_seed;
+  tail.env_offset = h->S.level_env_offset;
+  const std::vector<SnapSection> v = snapshot_sections(h, &tail);
+  const SnapHeader hd = snapshot_header(h, v);
   if (bytes < hd.bytes) return fail(MWB_ECAPACITY, "snapshot buffer too small");
-  std::vector<std::pair<void*, size_t>> v;
-  snapshot_arrays(h, v);
   unsigned char* p = (unsigned char*)blob;
   memcpy(p, &hd, sizeof(hd));
   p += sizeof(hd);
   if (stream_enter(h, h->stream)) return MWB_ECUDA;
-  for (size_t k = 0; k < v.size(); ++k) {
-    if (d2h(p, v[k].first, v[k].second, h->stream) != 0) return fail(MWB_ECUDA, "readback failed");
-    p += v[k].second;
-  }
-  if (h->S.next_level) {
-    const DevState& S = h->S;
-    int rc = d2h(p, S.env_level, (size_t)S.N * sizeof(int32_t), h->stream);
-    p += (size_t)S.N * sizeof(int32_t);
-    rc |= d2h(p, S.next_level, (size_t)S.N * sizeof(int32_t), h->stream);
-    p += (size_t)S.N * sizeof(int32_t);
-    rc |= d2h(p, S.level_draws, (size_t)S.N * sizeof(uint32_t), h->stream);
-    p += (size_t)S.N * sizeof(uint32_t);
-    rc |= d2h(p, S.level_weights, (size_t)S.num_levels * sizeof(float), h->stream);
-    p += (size_t)S.num_levels * sizeof(float);
-    LevelChangeTail tail;
-    memset(&tail, 0, sizeof(tail));
-    tail.seed = S.level_seed;
-    tail.env_offset = S.level_env_offset;
-    memcpy(p, &tail, sizeof(tail));
-    if (rc) return fail(MWB_ECUDA, "readback failed");
+  for (const SnapSection& s : v) {
+    if (!s.dev) memcpy(p, s.host, s.bytes);
+    else if (d2h(p, s.dev, s.bytes, h->stream) != 0) return fail(MWB_ECUDA, "readback failed");
+    p += s.bytes;
   }
   if (sync_stream(h->stream) != 0) return fail(MWB_ECUDA, "sync failed");
-  if (!h->S.next_level && snapshot_level_bytes(h)) memcpy(p, h->env_level.data(), snapshot_level_bytes(h));
   return MWB_OK;
 }
 
 extern "C" int mwb_restore(mwb_handle* h, const void* blob, size_t bytes) {
   if (!h || !blob) return fail(MWB_EINVAL, "null argument");
-  const SnapHeader want = snapshot_header(h);
+  LevelChangeTail tail;
+  const std::vector<SnapSection> v = snapshot_sections(h, &tail);
+  const SnapHeader want = snapshot_header(h, v);
   SnapHeader hd;
   if (bytes < sizeof(hd)) return fail(MWB_EINVAL, "not a snapshot");
   memcpy(&hd, blob, sizeof(hd));
@@ -2231,7 +2235,6 @@ extern "C" int mwb_restore(mwb_handle* h, const void* blob, size_t bytes) {
   if ((base != kSnapMagic && base != kSnapMagicLevelChanges && base != kSnapMagicWorlds &&
        base != kSnapMagicWorldsLevelChanges) || hd.abi != want.abi)
     return fail(MWB_EABI, "snapshot from another ABI version");
-  const bool dynamic = h->S.next_level != nullptr;
   if (hd.magic != want.magic)
     return fail(MWB_ESTATE, std::string("snapshot of a handle with ") + snapshot_mode(hd.magic) + " (this one has " +
                                 snapshot_mode(want.magic) + ")");
@@ -2242,42 +2245,35 @@ extern "C" int mwb_restore(mwb_handle* h, const void* blob, size_t bytes) {
     return fail(shared ? MWB_ESTATE : MWB_EINVAL, shared ? "snapshot of a handle with another number of levels"
                                                          : "snapshot does not match this handle's configuration");
   if (bytes < hd.bytes) return fail(MWB_EINVAL, "snapshot truncated");
-  std::vector<std::pair<void*, size_t>> v;
-  snapshot_arrays(h, v);
-  const size_t lb = snapshot_level_bytes(h);
-  if (!dynamic && lb && memcmp((const unsigned char*)blob + hd.bytes - lb, h->env_level.data(), lb) != 0)
-    return fail(MWB_ESTATE, "snapshot assigns envs to other levels than this handle");
+  // the blob's level assignment and tail, checked before anything is uploaded: a static table's must equal this
+  // handle's, and with level changes the kernels index the level table with the blob's (pending entries outside
+  // [-1, L) are ignored anyway)
+  const DevState& S = h->S;
   const unsigned char* p = (const unsigned char*)blob + sizeof(hd);
-  LevelChangeTail tail;
-  if (dynamic) {
-    // the kernels index the level table with the blob's assignment (pending entries outside [-1, L) are ignored anyway)
-    const DevState& S = h->S;
-    const unsigned char* q = p;
-    for (size_t k = 0; k < v.size(); ++k) q += v[k].second;
-    std::vector<int32_t> lv((size_t)S.N);
-    memcpy(lv.data(), q, lv.size() * sizeof(int32_t));
-    for (size_t k = 0; k < lv.size(); ++k)
-      if (lv[k] < 0 || lv[k] >= S.num_levels) return fail(MWB_EINVAL, "snapshot assigns an env to a level this handle does not have");
-    memcpy(&tail, (const unsigned char*)blob + hd.bytes - sizeof(tail), sizeof(tail));
-    if (tail.env_offset < 0) return fail(MWB_EINVAL, "snapshot has a negative env offset");
+  for (const SnapSection& s : v) {
+    if (!s.dev && s.host == h->env_level.data() && memcmp(p, s.host, s.bytes) != 0)
+      return fail(MWB_ESTATE, "snapshot assigns envs to other levels than this handle");
+    if (s.dev && s.dev == S.env_level) {
+      std::vector<int32_t> lv((size_t)S.N);
+      memcpy(lv.data(), p, lv.size() * sizeof(int32_t));
+      for (size_t k = 0; k < lv.size(); ++k)
+        if (lv[k] < 0 || lv[k] >= S.num_levels) return fail(MWB_EINVAL, "snapshot assigns an env to a level this handle does not have");
+    }
+    if (s.host == &tail) {
+      memcpy(&tail, p, sizeof(tail));
+      if (tail.env_offset < 0) return fail(MWB_EINVAL, "snapshot has a negative env offset");
+    }
+    p += s.bytes;
   }
   if (stream_enter(h, h->stream)) return MWB_ECUDA;
-  for (size_t k = 0; k < v.size(); ++k) {
-    if (h2d(v[k].first, p, v[k].second, h->stream) != 0) return fail(MWB_ECUDA, "upload failed");
-    p += v[k].second;
+  p = (const unsigned char*)blob + sizeof(hd);
+  for (const SnapSection& s : v) {
+    if (s.dev && h2d(s.dev, p, s.bytes, h->stream) != 0) return fail(MWB_ECUDA, "upload failed");
+    p += s.bytes;
   }
-  if (dynamic) {
-    DevState& S = h->S;
-    int rc = h2d(S.env_level, p, (size_t)S.N * sizeof(int32_t), h->stream);
-    p += (size_t)S.N * sizeof(int32_t);
-    rc |= h2d(S.next_level, p, (size_t)S.N * sizeof(int32_t), h->stream);
-    p += (size_t)S.N * sizeof(int32_t);
-    rc |= h2d(S.level_draws, p, (size_t)S.N * sizeof(uint32_t), h->stream);
-    p += (size_t)S.N * sizeof(uint32_t);
-    rc |= h2d((void*)S.level_weights, p, (size_t)S.num_levels * sizeof(float), h->stream);
-    if (rc) return fail(MWB_ECUDA, "upload failed");
-    S.level_seed = tail.seed;
-    S.level_env_offset = tail.env_offset;
+  if (S.next_level) {
+    h->S.level_seed = tail.seed;
+    h->S.level_env_offset = tail.env_offset;
   }
   if (sync_stream(h->stream) != 0) return fail(MWB_ECUDA, "sync failed");
   return MWB_OK;
@@ -2325,47 +2321,41 @@ extern "C" int mwb_debug_camera(mwb_handle* h, float* out) {
 // info["health"] (collecthealth.py:100) is the per-env counter, info["goal_pos"] (tmaze.py:89) three entity-pose rows.
 extern "C" int mwb_state_array(mwb_handle* h, int which, void** dev_ptr, int64_t* count) {
   if (!h || !dev_ptr || !count) return fail(MWB_EINVAL, "null argument");
-  const int64_t N = h->S.N, E = h->S.E;
+  const DevState& S = h->S;
+  const MazeLayouts& Y = h->layouts_h;
+  const int64_t N = S.N, E = S.E;
+  // why the arrays of a mode are missing, naming the call that adds them; null while the mode is on
+  const char* levels_off = S.next_level ? nullptr : "level changes are off (mwb_enable_level_changes)";
+  const char* seeds_off = S.next_seed ? nullptr : "episode seeds are off (mwb_enable_episode_seeds)";
+  const char* mazes_off = S.layouts ? nullptr : "maze layouts are off (mwb_enable_maze_layouts)";
+  const char* params_off = h->have_params && S.ops ? nullptr
+                           : "the handle has no device resets (params and a reset program: mwb_set_levels, or "
+                             "mwb_set_params and mwb_set_program); host-generated worlds carry their own draws";
+  const char* off = nullptr;
+  void* p = nullptr;
+  int64_t n = N;
   switch (which) {
-    case MWB_ARRAY_COUNTER: *dev_ptr = h->S.num_picked; *count = N; break;       // int32 [N]
-    case MWB_ARRAY_STEP_COUNT: *dev_ptr = h->S.step_count; *count = N; break;    // int32 [N]
-    case MWB_ARRAY_ENT_X: *dev_ptr = h->S.ent_px; *count = E * N; break;         // float64 [E][N]
-    case MWB_ARRAY_ENT_Y: *dev_ptr = h->S.ent_py; *count = E * N; break;
-    case MWB_ARRAY_ENT_Z: *dev_ptr = h->S.ent_pz; *count = E * N; break;
-    case MWB_ARRAY_ENT_DIR: *dev_ptr = h->S.ent_dir; *count = E * N; break;
-    case MWB_ARRAY_ENV_LEVEL:
-    case MWB_ARRAY_NEXT_LEVEL:
-    case MWB_ARRAY_LEVEL_WEIGHTS:
-      if (!h->S.next_level) return fail(MWB_ESTATE, "level changes are off (mwb_enable_level_changes)");
-      if (which == MWB_ARRAY_ENV_LEVEL) { *dev_ptr = h->S.env_level; *count = N; }                       // int32 [N]
-      else if (which == MWB_ARRAY_NEXT_LEVEL) { *dev_ptr = h->S.next_level; *count = N; }                // int32 [N]
-      else { *dev_ptr = (void*)h->S.level_weights; *count = h->S.num_levels; }                           // float32 [L]
-      break;
-    case MWB_ARRAY_NEXT_SEED:
-    case MWB_ARRAY_EPISODE_SEED:
-      if (!h->S.next_seed) return fail(MWB_ESTATE, "episode seeds are off (mwb_enable_episode_seeds)");
-      *dev_ptr = which == MWB_ARRAY_NEXT_SEED ? h->S.next_seed : h->S.episode_seed; *count = N;           // int64 [N]
-      break;
-    case MWB_ARRAY_NEXT_MAZE:
-    case MWB_ARRAY_EPISODE_MAZE:
-      if (!h->S.layouts) return fail(MWB_ESTATE, "maze layouts are off (mwb_enable_maze_layouts)");
-      *dev_ptr = which == MWB_ARRAY_NEXT_MAZE ? h->layouts_h.next : h->layouts_h.episode;                  // uint8
-      *count = N * h->layouts_h.rows * h->layouts_h.cols;                                                 // [N][rows][cols]
-      break;
-    case MWB_ARRAY_NEXT_MAZE_CELLS:
-    case MWB_ARRAY_MAZE_PENDING:
-      if (!h->S.layouts) return fail(MWB_ESTATE, "maze layouts are off (mwb_enable_maze_layouts)");
-      if (which == MWB_ARRAY_NEXT_MAZE_CELLS) { *dev_ptr = h->layouts_h.cells; *count = 2 * N; }          // int32 [N][2]
-      else { *dev_ptr = h->layouts_h.pending; *count = N; }                                               // uint8 [N]
-      break;
-    case MWB_ARRAY_LEVEL_PARAMS:
-      if (!h->have_params || !h->S.ops)
-        return fail(MWB_ESTATE, "the handle has no device resets (params and a reset program: mwb_set_levels, or "
-                                "mwb_set_params and mwb_set_program); host-generated worlds carry their own draws");
-      *dev_ptr = (void*)h->S.level_params; *count = (int64_t)h->levels.size();                            // mwb_params [L]
-      break;
+    case MWB_ARRAY_COUNTER: p = S.num_picked; break;                                              // int32 [N]
+    case MWB_ARRAY_STEP_COUNT: p = S.step_count; break;                                           // int32 [N]
+    case MWB_ARRAY_ENT_X: p = S.ent_px; n = E * N; break;                                         // float64 [E][N]
+    case MWB_ARRAY_ENT_Y: p = S.ent_py; n = E * N; break;
+    case MWB_ARRAY_ENT_Z: p = S.ent_pz; n = E * N; break;
+    case MWB_ARRAY_ENT_DIR: p = S.ent_dir; n = E * N; break;
+    case MWB_ARRAY_ENV_LEVEL: p = S.env_level; off = levels_off; break;                           // int32 [N]
+    case MWB_ARRAY_NEXT_LEVEL: p = S.next_level; off = levels_off; break;                         // int32 [N]
+    case MWB_ARRAY_LEVEL_WEIGHTS: p = (void*)S.level_weights; n = S.num_levels; off = levels_off; break;   // float32 [L]
+    case MWB_ARRAY_NEXT_SEED: p = S.next_seed; off = seeds_off; break;                            // int64 [N]
+    case MWB_ARRAY_EPISODE_SEED: p = S.episode_seed; off = seeds_off; break;                      // int64 [N]
+    case MWB_ARRAY_NEXT_MAZE: p = Y.next; n = N * Y.rows * Y.cols; off = mazes_off; break;        // uint8 [N][rows][cols]
+    case MWB_ARRAY_EPISODE_MAZE: p = Y.episode; n = N * Y.rows * Y.cols; off = mazes_off; break;  // uint8 [N][rows][cols]
+    case MWB_ARRAY_NEXT_MAZE_CELLS: p = Y.cells; n = 2 * N; off = mazes_off; break;               // int32 [N][2]
+    case MWB_ARRAY_MAZE_PENDING: p = Y.pending; off = mazes_off; break;                           // uint8 [N]
+    case MWB_ARRAY_LEVEL_PARAMS: p = (void*)S.level_params; n = (int64_t)h->levels.size(); off = params_off; break;  // mwb_params [L]
     default: return fail(MWB_EINVAL, "unknown array");
   }
+  if (off) return fail(MWB_ESTATE, off);
+  *dev_ptr = p;
+  *count = n;
   return MWB_OK;
 }
 

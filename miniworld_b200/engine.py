@@ -564,34 +564,32 @@ class Engine:
         """uint32[N] (numpy or CUDA tensor): bit e = entity slot e passes the reference's occlusion query."""
         self._check(self.lib.mwb_visible_ents(self.h, _dev_or_host_ptr(mask), stream))
 
-    # name -> (mwb_state_array id, element type, leading axis: "env" = [N] or [k, N], "level" = [n_levels],
-    # "params" = [n_levels, PARAMS_DOUBLES] mwb_params records as float64 words)
-    ARRAYS = {"counter": (0, "<i4", "env"), "step_count": (1, "<i4", "env"), "ent_x": (2, "<f8", "env"),
-              "ent_y": (3, "<f8", "env"), "ent_z": (4, "<f8", "env"), "ent_dir": (5, "<f8", "env"),
+    # name -> (mwb_state_array id, element type, shape): "env" = [N], "ents" = [max_ents, N], "level" = [n_levels],
+    # "params" = [n_levels, PARAMS_DOUBLES] (mwb_params records as float64 words), "env_rows" = [N, count / N]
+    ARRAYS = {"counter": (0, "<i4", "env"), "step_count": (1, "<i4", "env"), "ent_x": (2, "<f8", "ents"),
+              "ent_y": (3, "<f8", "ents"), "ent_z": (4, "<f8", "ents"), "ent_dir": (5, "<f8", "ents"),
               "env_level": (6, "<i4", "env"), "next_level": (7, "<i4", "env"), "level_weights": (8, "<f4", "level"),
               "level_params": (9, "<f8", "params"), "next_seed": (16, "<i8", "env"), "episode_seed": (17, "<i8", "env"),
               "next_maze": (18, "|u1", "env_rows"), "next_maze_cells": (19, "<i4", "env_rows"),
               "maze_pending": (20, "|u1", "env"), "episode_maze": (21, "|u1", "env_rows")}
 
-    def state_array(self, name):
+    def state_array(self, name, shape=None):
         """Zero-copy view of a state array (mwb_state_array) as an object with __cuda_array_interface__:
         "counter" / "step_count" int32 [N]; "ent_x|y|z|dir" float64 [max_ents, N]; with level changes on,
         "env_level" / "next_level" int32 [N] and "level_weights" float32 [n_levels]; with device resets,
         "level_params" float64 [n_levels, PARAMS_DOUBLES] (column of a field: PARAMS_COLUMN); with episode seeds on,
         "next_seed" / "episode_seed" int64 [N]; with maze layouts on, "next_maze" / "episode_maze" uint8
-        [N, rows * cols], "next_maze_cells" int32 [N, 2] and "maze_pending" uint8 [N].  On the host build of
-        the kernels the arrays live in host memory, and the view is a numpy array over the same memory instead."""
+        [N, rows * cols], "next_maze_cells" int32 [N, 2] and "maze_pending" uint8 [N].  `shape` gives the view
+        another shape of the same size (the maze layouts as [N, rows, cols]).  On the host build of the kernels the
+        arrays live in host memory, and the view is a numpy array over the same memory instead."""
         which, typestr, axis = self.ARRAYS[name]
         ptr, count = C.c_void_p(), C.c_int64()
         self._check(self.lib.mwb_state_array(self.h, which, C.byref(ptr), C.byref(count)))
-        if axis == "params":
-            shape = (count.value, PARAMS_DOUBLES)
-        elif axis == "env_rows":
-            shape = (self.N, count.value // self.N)
-        elif axis == "level" or count.value == self.N:
-            shape = (count.value,)
-        else:
-            shape = (count.value // self.N, self.N)
+        n = count.value
+        shape = tuple(shape or {"env": (self.N,), "ents": (n // self.N, self.N), "level": (n,),
+                                "params": (n, PARAMS_DOUBLES), "env_rows": (self.N, n // self.N)}[axis])
+        if int(np.prod(shape)) != (n * PARAMS_DOUBLES if axis == "params" else n):
+            raise ValueError("%s has %d entries, not shape %s" % (name, n, shape))
         if self.host_memory:
             dt = np.dtype(typestr)
             buf = (C.c_char * (int(np.prod(shape)) * dt.itemsize)).from_address(ptr.value)
