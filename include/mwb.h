@@ -423,6 +423,36 @@ int mwb_set_maze(mwb_handle* h, const mwb_maze_desc* maze);
  * else is compared. */
 int mwb_enable_maze_layouts(mwb_handle* h);
 
+/* Start poses (reverse curricula, start-state curricula, goal-placement environment design).  Valid on a handle with
+ * device resets (params and a reset program); MWB_ESTATE when the handle resets on the host or has the mode on already.
+ * A pose is (x, z, dir) in float64.  Four arrays, read and written in place through mwb_state_array, stream-ordered,
+ * without a sync; the designed rows are all NaN and the rest zero at the call:
+ *   next_pose float64 [N][max_ents][3]   designed pose of each entity-list slot at the env's next reset;
+ *   next_agent_pose float64 [N][3]       designed pose of the agent at the env's next reset;
+ *   pose_pending uint8 [N]               nonzero: the rows wait for the env's next reset;
+ *   episode_start float64 [N][3]         the agent's (x, z, dir) at the start of the env's running episode.
+ * At every reset of env i (mwb_reset, and the next-step auto-reset inside mwb_step) with pose_pending[i] set, at any
+ * level, pose_pending[i] = 0 and the level's program runs with these placements replaced (the rows stay as written):
+ *   - the place_entity call that fills entity-list slot e (a PLACE op, or a PUT op that is not append-only) takes
+ *     next_pose[i][e] when its x and z are finite; the agent's call (place_agent) takes next_agent_pose[i] when its x
+ *     and z are finite, and otherwise its slot's row as any other call.  In a level table a slot is a slot of the
+ *     level the reset runs; next_agent_pose is the agent at every level;
+ *   - a designed call runs the reference's place_entity(pos=[x, y, z], dir=...) branch: y is the y of the pos the
+ *     level passed (0 for a searched placement), dir is the designed dir when finite, else the dir the level passed,
+ *     else uniform(-pi, pi) drawn from the env's stream.  No room is picked, no position searched and no collision
+ *     checked, as in the reference; a pose outside the floor plan is kept as written.  A design that leaves a later
+ *     searched placement of the same reset no free spot makes that search run forever, as it would in the reference;
+ *   - every other draw (choices, sizes, other slots' searches, textures, sky and light, colours, camera) happens as
+ *     before and in order, so with episode seeds on a seed and a design reproduce an episode;
+ *   - a designed pose wins over the goal or agent cell of a designed maze (mwb_enable_maze_layouts) for that call.
+ * Every reset writes the agent's pose into episode_start[i], designed or drawn; after a terminating step it still names
+ * the episode that ended, because the reset happens inside the next step.  Handles that never call this behave
+ * exactly as before it existed, and the addition changes no struct, so MWB_ABI_VERSION stays as it is.  Snapshots of
+ * a handle with the mode on carry the four arrays and are marked as such in the header; restoring a blob into a handle
+ * whose start poses are on / off while the blob's were off / on fails with MWB_ESTATE before anything else is
+ * compared. */
+int mwb_enable_start_poses(mwb_handle* h);
+
 /* Maze levels in a level table (curricula over maze sizes: MazeS2 -> MazeS3 -> Maze, next to fixed-layout levels).
  * Valid on a shared_geometry = 1 handle after mwb_set_levels (MWB_ESTATE otherwise).  Level `level` (MWB_EINVAL
  * outside [0, L)) becomes a per-env-world level: every reset of an env at that level carves a fresh maze from these
@@ -585,6 +615,11 @@ int mwb_debug_camera(mwb_handle* h, float* out /* host [num_envs][16] */);
 #define MWB_ARRAY_NEXT_MAZE_CELLS 19  /* int32 [num_envs][2]  goal cell, agent cell of that layout, -1 = random       */
 #define MWB_ARRAY_MAZE_PENDING 20     /* uint8 [num_envs]  nonzero = next_maze waits for a reset at a Maze level       */
 #define MWB_ARRAY_EPISODE_MAZE 21     /* uint8 [num_envs][rows][cols]  layout of the env's running episode            */
+/* with start poses on (mwb_enable_start_poses; MWB_ESTATE otherwise); count = elements: */
+#define MWB_ARRAY_NEXT_POSE 22        /* float64 [num_envs][max_ents][3]  designed (x, z, dir) per slot, next reset   */
+#define MWB_ARRAY_NEXT_AGENT_POSE 23  /* float64 [num_envs][3]  designed (x, z, dir) of the agent, next reset         */
+#define MWB_ARRAY_POSE_PENDING 24     /* uint8 [num_envs]  nonzero = the designed poses wait for the next reset       */
+#define MWB_ARRAY_EPISODE_START 25    /* float64 [num_envs][3]  the agent's (x, z, dir) when the episode started      */
 int mwb_state_array(mwb_handle* h, int which, void** dev_ptr, int64_t* count);
 /* 1 when this library keeps the handle's state arrays (mwb_state_array) in host memory -- the CPU build of the kernels
  * used by the test suite -- and 0 for libmwb.so, whose arrays are device memory. */

@@ -18,7 +18,9 @@ Per-environment semantics are exactly those of the reference's `MiniWorldEnv.res
   * with `episode_seeds=True`, an env's next reset can start from a chosen seed (`next_seed`, `set_env_seed`),
     seeded on the device as `reset(seed=s)` would, and `info["seed"]` names the seed of each running episode;
   * with `maze_layouts=True`, an env's next reset at a Maze level can build a maze written into a device tensor
-    (`next_maze`, `set_env_maze`), and `info["maze"]` holds the layout of each running episode.
+    (`next_maze`, `set_env_maze`), and `info["maze"]` holds the layout of each running episode;
+  * with `start_poses=True`, an env's next reset can place the agent and the entities at poses written into device
+    tensors (`next_pose`, `set_env_pose`), and `info["start"]` holds where each running episode's agent started.
 
 Outputs are torch CUDA tensors by default (zero-copy from the kernels); `step_host`
 performs the same step with pinned host buffers for callers that want numpy.
@@ -166,6 +168,8 @@ _NEEDS = {**dict.fromkeys(("env_level", "next_level", "level_weights"), (
               "episode_seeds", RuntimeError, "this batch has no episode seeds: construct it with episode_seeds=True")),
           **dict.fromkeys(("next_maze", "next_maze_cells", "maze_pending", "episode_maze"), (
               "maze_layouts", RuntimeError, "this batch has no maze layouts: construct it with maze_layouts=True")),
+          **dict.fromkeys(("next_pose", "next_agent_pose", "pose_pending", "episode_start"), (
+              "start_poses", RuntimeError, "this batch has no start poses: construct it with start_poses=True")),
           "level_params": ("device_reset", TypeError, "level params change at device resets; host-reset levels draw "
                            "theirs in Python (set them on the level's own DomainParams)")}
 
@@ -234,12 +238,24 @@ class BatchedMiniWorld:
     running episode, random carves included (zeros at other levels); after a terminating step they still name the
     episode that just ended.  Replaying a carve's recorded layout builds the same walls, but creates the connector rooms
     in another order than the carve did, so the episode's placement draws differ.  Each Maze level's capacities are
-    sized for its all-open maze (c cells, E inner edges: c + E rooms, 6c + 2E quads, as against 2c - 1 and 8c - 2)."""
+    sized for its all-open maze (c cells, E inner edges: c + E rooms, 6c + 2E quads, as against 2c - 1 and 8c - 2).
+
+    `start_poses=True` (one level or a table; levels that reset on the device) decides where episodes start, for reverse
+    and start-state curricula and goal placement: with `pose_pending[i]` set, env i's next reset at any level, the
+    auto-reset inside `step` included, places the entity that fills slot e at `next_pose[i, e]` = (x, z, dir) and the
+    agent at `next_agent_pose[i]`, as `reset(options={"poses": {e: (x, z, dir)}, "agent_pose": (x, z, dir)})` does on
+    the host: the reference's `place_entity(pos=..., dir=...)` branch, without a search or a collision check.  A row
+    applies when its x and z are finite (the rows start as NaN), its dir when that is finite (otherwise the level's dir,
+    or a uniform draw).  The agent's row wins over the agent's slot row.  The reset clears `pose_pending` and leaves the
+    rows as written.  A design that leaves a later searched placement of the same reset no free spot makes that search
+    run forever, as it would in the reference.  `level_slots` names the slots each level fills.  `episode_start` / `info["start"]` hold the
+    agent's (x, z, dir) at the start of every running episode, designed or drawn; after a terminating step they still
+    name the episode that just ended."""
 
     def __init__(self, level, num_envs, obs_width=80, obs_height=60, domain_rand=False, autoreset=True,
                  msaa_samples=8, device=0, want_depth=False, level_kwargs=None, obs_format="hwc", env_level=None,
                  dynamic_levels=False, level_seed=0, env_offset=0, per_env_worlds=False, episode_seeds=False,
-                 maze_layouts=False):
+                 maze_layouts=False, start_poses=False):
         self.num_envs = int(num_envs)
         self.obs_width, self.obs_height = int(obs_width), int(obs_height)
         self.domain_rand = bool(domain_rand)
@@ -249,6 +265,7 @@ class BatchedMiniWorld:
         self.per_env_worlds = bool(per_env_worlds)
         self.episode_seeds = bool(episode_seeds)
         self.maze_layouts = bool(maze_layouts)
+        self.start_poses = bool(start_poses)
         table = isinstance(level, (list, tuple))
         if table:
             defs = self._init_levels(list(level), level_kwargs, env_level)
@@ -266,7 +283,7 @@ class BatchedMiniWorld:
         self._init_engine(defs, table, msaa_samples, autoreset)
         self._view_map = _Views(self.engine, self.device, dict(
             dynamic_levels=self.dynamic_levels, episode_seeds=self.episode_seeds, maze_layouts=self.maze_layouts,
-            device_reset=self.device_reset), getattr(self, "maze_shape", None))
+            start_poses=self.start_poses, device_reset=self.device_reset), getattr(self, "maze_shape", None))
         if self.dynamic_levels:
             self.level_seed, self.env_offset = int(level_seed), int(env_offset)
             self.engine.enable_level_changes(self.level_seed, self.env_offset)
@@ -277,6 +294,12 @@ class BatchedMiniWorld:
             self.engine.enable_episode_seeds()
         if self.maze_layouts:
             self.engine.enable_maze_layouts()
+        if self.start_poses:
+            if not self.device_reset:
+                self.engine.close()
+                raise TypeError("start poses are taken by device resets; host-reset levels place entities in Python "
+                                "(reset(options={\"poses\": ...}) of the level itself)")
+            self.engine.enable_start_poses()
         # observation layout written by the render kernel: the reference's PyTorchObsWrapper ("cwh") and
         # GreyscaleWrapper ("grey") are fused into its epilogue instead of running as separate passes
         self.obs_format = obs_format
@@ -378,6 +401,9 @@ class BatchedMiniWorld:
         self.action_space = self.single_action_space = largest.action_space
         self.single_observation_space = d0.pe.observation_space
         self.device_reset = all(d.program is not None for d in defs)
+        # the entity-list slots each level's reset fills: kind, whether it is the agent, whether it takes a design
+        self.level_slots = [[dict(slot=e, kind=k, agent=a, designable=ds) for e, (k, a, ds) in enumerate(d.program.slots)]
+                            if d.program is not None else None for d in defs]
         self.program, self.maze_template = (None, None) if table else (d0.program, d0.maze)
         self.autoreset = bool(autoreset)
         if self.device_reset:
@@ -457,6 +483,10 @@ class BatchedMiniWorld:
             if self.maze_layouts:
                 # the layout of each env's current episode (after a terminating step still the ended one's)
                 self._info["maze"] = self.episode_maze
+            if self.start_poses:
+                # the agent's (x, z, dir) at the start of each env's current episode (after a terminating step still
+                # the ended one's)
+                self._info["start"] = self.episode_start
         return self._torch
 
     # ------------------------------------------------------------------ run-time arrays
@@ -465,9 +495,9 @@ class BatchedMiniWorld:
         return self._view_map
 
     def _write_pending(self, what, ids, arrays):
-        """The part set_env_level / set_env_seed / set_env_maze share: check the env ids `ids` (1-D integers in [0, N)),
-        then write each (array name, values) of `arrays` at those envs -- values one per id (a numpy array, or a CUDA
-        tensor) or one for all -- an env listed more than once taking its last entry.  On the host build the write is
+        """The part set_env_level / set_env_seed / set_env_maze / set_env_pose share: check the env ids `ids` (1-D
+        integers in [0, N)), then write each (array name or view, values) of `arrays` at those envs -- values one per id
+        (a numpy array, or a CUDA tensor) or one for all -- an env listed more than once taking its last entry.  On the host build the write is
         numpy's; on the device it is torch ops on the current stream, without a sync."""
         if not np.issubdtype(ids.dtype, np.integer) or ids.ndim != 1:
             raise ValueError("%s takes a 1-D sequence of integer env ids" % what)
@@ -478,7 +508,7 @@ class BatchedMiniWorld:
         last = ids.size - 1 - np.unique(ids[::-1], return_index=True)[1]    # an env listed twice: its last entry wins
         if self.engine.host_memory:
             for name, vals in arrays:
-                self._views()[name][ids[last]] = vals[last] if np.ndim(vals) else vals
+                self._target(name)[ids[last]] = vals[last] if np.ndim(vals) else vals
             return
         import torch
         to_dev = lambda a: torch.as_tensor(a).to(torch.device("cuda", self.device), non_blocking=True)
@@ -488,7 +518,10 @@ class BatchedMiniWorld:
                 vals = vals[to_dev(last)] if vals.dim() else vals
             elif np.ndim(vals):
                 vals = to_dev(np.ascontiguousarray(vals[last]))
-            self._views()[name][idx] = vals
+            self._target(name)[idx] = vals
+
+    def _target(self, name):
+        return self._views()[name] if isinstance(name, str) else name
 
     # ------------------------------------------------------------------ level changes (dynamic_levels=True)
     @property
@@ -630,6 +663,65 @@ class BatchedMiniWorld:
         both = np.stack(cells, axis=1).astype(np.int32)
         self._write_pending("set_env_maze", ids, [("next_maze", lay.astype(np.uint8, copy=False)),
                                                   ("next_maze_cells", both), ("maze_pending", 1)])
+
+    # ------------------------------------------------------------------ start poses (start_poses=True)
+    @property
+    def next_pose(self):
+        """float64 [N, max_ents, 3] view of the designed (x, z, dir) of each entity-list slot at each env's next reset
+        with `pose_pending` set; write it in place (stream-ordered, no sync).  A row applies when x and z are finite."""
+        return self._views()["next_pose"]
+
+    @property
+    def next_agent_pose(self):
+        """float64 [N, 3] view of the designed (x, z, dir) of the agent at each env's next reset with `pose_pending`
+        set, at every level; it wins over the agent's slot row of `next_pose`."""
+        return self._views()["next_agent_pose"]
+
+    @property
+    def pose_pending(self):
+        """uint8 [N] view: nonzero when the designed rows wait for env i's next reset, which clears it."""
+        return self._views()["pose_pending"]
+
+    @property
+    def episode_start(self):
+        """float64 [N, 3] view of the agent's (x, z, dir) at the start of each env's running episode."""
+        return self._views()["episode_start"]
+
+    def set_env_pose(self, env_ids, slot, x, z, dir=None):
+        """Start the listed envs' next episodes with entity-list slot `slot` (an int in [0, max_ents), or "agent") at
+        (x, z) facing `dir` (None: the level's dir, or a uniform draw); envs in mid-episode finish it first.  Values are
+        one for all or one per env; an env listed more than once takes its last entry.  Sets `pose_pending`; rows
+        written earlier stay.  Host values are checked (x and z finite); CUDA tensors are written as they are.  The
+        write is numpy's on the host build, torch ops on the current stream without a sync on the device."""
+        self._views()["next_pose"]                   # a batch without the mode raises before any input check
+        ids = np.atleast_1d(_host(env_ids))
+        if isinstance(slot, str) and slot == "agent":
+            target = self.next_agent_pose
+        elif isinstance(slot, (int, np.integer)) and not isinstance(slot, bool) and 0 <= slot < self.engine.max_ents:
+            target = self.next_pose[:, int(slot)]
+        else:
+            raise ValueError("slot must be \"agent\" or an int in [0, %d), got %r" % (self.engine.max_ents, slot))
+        comps, on_device = [], False
+        for name, v in (("x", x), ("z", z), ("dir", np.nan if dir is None else dir)):
+            if hasattr(v, "is_cuda") and v.is_cuda:
+                on_device = True
+                got = tuple(v.shape)
+            else:
+                v = np.asarray(_host(v), np.float64)
+                got = v.shape
+                if name != "dir" and not np.isfinite(v).all():
+                    raise ValueError("set_env_pose: %s must be finite" % name)
+            if got not in ((), ids.shape):
+                raise ValueError("set_env_pose: %s is one value or one per env id (%d), got shape %s" % (name, ids.size, got))
+            comps.append(v)
+        if on_device:
+            torch = self._ensure_torch()
+            dev = torch.device("cuda", self.device)
+            rows = torch.stack([torch.as_tensor(c, dtype=torch.float64).to(dev, non_blocking=True).expand(ids.shape)
+                                for c in comps], dim=1)
+        else:
+            rows = np.stack([np.broadcast_to(c, ids.shape) for c in comps], axis=1)
+        self._write_pending("set_env_pose", ids, [(target, rows), ("pose_pending", 1)])
 
     # ------------------------------------------------------------------ level params at run time
     def set_level_param(self, level, name, default=None, min=None, max=None):
@@ -857,9 +949,10 @@ class BatchedMiniWorld:
 
     def _torch_writes(self):
         """True when torch work may write arrays the kernels read: next_level / level_weights (level changes on),
-        next_seed (episode seeds on), the pending maze layouts (maze layouts on) or the params table (once
-        set_level_param has written it)."""
-        return ((self.dynamic_levels or self.episode_seeds or self.maze_layouts or self._params_written)
+        next_seed (episode seeds on), the pending maze layouts (maze layouts on), the designed start poses (start poses
+        on) or the params table (once set_level_param has written it)."""
+        return ((self.dynamic_levels or self.episode_seeds or self.maze_layouts or self.start_poses
+                 or self._params_written)
                 and not self.engine.host_memory)
 
     def _level_stream(self):

@@ -122,6 +122,7 @@ struct mwb_handle {
   std::vector<int32_t> level_quads;   // quads of every level's worlds (per-level K2 planning of a table with mazes)
   std::vector<MazeDev> mazes_h;       // host copies of S.maze / S.maze_cdf, one entry per level
   MazeLayouts layouts_h;              // host copy of *S.layouts (mwb_enable_maze_layouts)
+  StartPoses poses_h;                 // host copy of *S.poses (mwb_enable_start_poses)
   std::vector<double> maze_cdf_h;
   bool have_params, have_protos, have_template;
   bool have_level_table;          // mwb_set_levels succeeded (mwb_enable_level_changes needs it)
@@ -1524,6 +1525,32 @@ extern "C" int mwb_enable_maze_layouts(mwb_handle* h) {
   return MWB_OK;
 }
 
+extern "C" int mwb_enable_start_poses(mwb_handle* h) {
+  if (!h) return fail(MWB_EINVAL, "null handle");
+  if (h->S.poses) return fail(MWB_ESTATE, "start poses are already on");
+  if (!h->have_params || !h->S.ops)
+    return fail(MWB_ESTATE, "start poses need device resets (params and a reset program: mwb_set_levels, or "
+                            "mwb_set_params and mwb_set_program); host-generated worlds are placed on the host");
+  DevState& S = h->S;
+  const size_t N = S.N, E = S.E;
+  void *next, *next_agent, *pending, *episode;
+  // NaN rows (0xFF bytes): no design until one is written
+  int rc = alloc_control_arrays(h, "start pose", {{&next, N * E * 3 * sizeof(double), true},
+                                                  {&next_agent, N * 3 * sizeof(double), true},
+                                                  {&pending, N, false}, {&episode, N * 3 * sizeof(double), false}});
+  if (rc) return rc;
+  StartPoses& P = h->poses_h;
+  P.next = (double*)next;
+  P.next_agent = (double*)next_agent;
+  P.pending = (uint8_t*)pending;
+  P.episode = (double*)episode;
+  StartPoses* d = nullptr;
+  if (alloc_arr(h, &d, 1)) return fail(MWB_ECUDA, "start pose state allocation failed");
+  if (h2d(d, &P, sizeof(P), h->stream) != 0 || sync_stream(h->stream) != 0) return fail(MWB_ECUDA, "upload failed");
+  S.poses = d;
+  return MWB_OK;
+}
+
 // geometry block env `env` reads (geom_index in state.h), from the host's view of its level
 static int env_geom_block(mwb_handle* h, int env, size_t* g) {
   int32_t lvl = 0;
@@ -2106,20 +2133,25 @@ static const uint32_t kSnapMagicWorldsLevelChanges = 0x5842574du;   // "MWBX": .
 static const uint32_t kSnapMagicSeeds = 0x20000000u;
 // one with maze layouts on writes the "B" in lower case ("MWbS", "MWbs", ...) and carries the four layout arrays
 static const uint32_t kSnapMagicMazes = 0x00200000u;
+// one with start poses on writes the "W" in lower case ("MwBS", "MwbS", ...) and carries the four start pose arrays
+static const uint32_t kSnapMagicPoses = 0x00002000u;
+static const uint32_t kSnapMagicModes = kSnapMagicSeeds | kSnapMagicMazes | kSnapMagicPoses;
 
 static uint32_t snapshot_magic(const mwb_handle* h) {
-  const uint32_t seeds = (h->S.next_seed ? kSnapMagicSeeds : 0u) | (h->S.layouts ? kSnapMagicMazes : 0u);
+  const uint32_t seeds = (h->S.next_seed ? kSnapMagicSeeds : 0u) | (h->S.layouts ? kSnapMagicMazes : 0u) |
+                         (h->S.poses ? kSnapMagicPoses : 0u);
   if (h->level_mazes) return (h->S.next_level ? kSnapMagicWorldsLevelChanges : kSnapMagicWorlds) | seeds;
   return (h->S.next_level ? kSnapMagicLevelChanges : kSnapMagic) | seeds;
 }
 static std::string snapshot_mode(uint32_t magic) {
-  const uint32_t base = magic & ~(kSnapMagicSeeds | kSnapMagicMazes);
+  const uint32_t base = magic & ~kSnapMagicModes;
   return std::string(base == kSnapMagic ? "level changes off, no per-env worlds"
                      : base == kSnapMagicLevelChanges ? "level changes on, no per-env worlds"
                      : base == kSnapMagicWorlds ? "level changes off, per-env worlds"
                                                 : "level changes on, per-env worlds") +
          (magic & kSnapMagicSeeds ? ", episode seeds on" : ", episode seeds off") +
-         (magic & kSnapMagicMazes ? ", maze layouts on" : ", maze layouts off");
+         (magic & kSnapMagicMazes ? ", maze layouts on" : ", maze layouts off") +
+         (magic & kSnapMagicPoses ? ", start poses on" : ", start poses off");
 }
 
 struct SnapHeader {
@@ -2148,7 +2180,7 @@ struct SnapSection {
 
 // The sections of a blob after its header, in blob order: every array that changes while episodes run (entity lists,
 // counters, camera / lighting parameters, RNG streams, pending-reset flags), the geometry currently on the device and
-// the level ranges, then the episode-seed and maze-layout arrays of handles with those modes on.  A handle with level
+// the level ranges, then the episode-seed, maze-layout and start-pose arrays of handles with those modes on.  A handle with level
 // changes on closes the blob with its level-change section: env_level, next_level, level_draws, level_weights and
 // `tail` (adopted on restore: the assignment is state).  A static table of several levels closes it with the host's
 // env_level (checked on restore, never overwritten).
@@ -2172,6 +2204,11 @@ static std::vector<SnapSection> snapshot_sections(mwb_handle* h, LevelChangeTail
     const MazeLayouts& Y = h->layouts_h;
     const size_t cells = (size_t)Y.rows * Y.cols;
     dev(Y.next, N * cells); dev(Y.cells, 2 * N * sizeof(int32_t)); dev(Y.pending, N); dev(Y.episode, N * cells);
+  }
+  if (S.poses) {
+    const StartPoses& P = h->poses_h;
+    dev(P.next, N * E * 3 * sizeof(double)); dev(P.next_agent, N * 3 * sizeof(double)); dev(P.pending, N);
+    dev(P.episode, N * 3 * sizeof(double));
   }
   if (S.next_level) {
     SA(env_level, N); SA(next_level, N); SA(level_draws, N); SA(level_weights, S.num_levels);
@@ -2231,7 +2268,7 @@ extern "C" int mwb_restore(mwb_handle* h, const void* blob, size_t bytes) {
   SnapHeader hd;
   if (bytes < sizeof(hd)) return fail(MWB_EINVAL, "not a snapshot");
   memcpy(&hd, blob, sizeof(hd));
-  const uint32_t base = hd.magic & ~(kSnapMagicSeeds | kSnapMagicMazes);
+  const uint32_t base = hd.magic & ~kSnapMagicModes;
   if ((base != kSnapMagic && base != kSnapMagicLevelChanges && base != kSnapMagicWorlds &&
        base != kSnapMagicWorldsLevelChanges) || hd.abi != want.abi)
     return fail(MWB_EABI, "snapshot from another ABI version");
@@ -2323,11 +2360,13 @@ extern "C" int mwb_state_array(mwb_handle* h, int which, void** dev_ptr, int64_t
   if (!h || !dev_ptr || !count) return fail(MWB_EINVAL, "null argument");
   const DevState& S = h->S;
   const MazeLayouts& Y = h->layouts_h;
+  const StartPoses& P = h->poses_h;
   const int64_t N = S.N, E = S.E;
   // why the arrays of a mode are missing, naming the call that adds them; null while the mode is on
   const char* levels_off = S.next_level ? nullptr : "level changes are off (mwb_enable_level_changes)";
   const char* seeds_off = S.next_seed ? nullptr : "episode seeds are off (mwb_enable_episode_seeds)";
   const char* mazes_off = S.layouts ? nullptr : "maze layouts are off (mwb_enable_maze_layouts)";
+  const char* poses_off = S.poses ? nullptr : "start poses are off (mwb_enable_start_poses)";
   const char* params_off = h->have_params && S.ops ? nullptr
                            : "the handle has no device resets (params and a reset program: mwb_set_levels, or "
                              "mwb_set_params and mwb_set_program); host-generated worlds carry their own draws";
@@ -2350,6 +2389,10 @@ extern "C" int mwb_state_array(mwb_handle* h, int which, void** dev_ptr, int64_t
     case MWB_ARRAY_EPISODE_MAZE: p = Y.episode; n = N * Y.rows * Y.cols; off = mazes_off; break;  // uint8 [N][rows][cols]
     case MWB_ARRAY_NEXT_MAZE_CELLS: p = Y.cells; n = 2 * N; off = mazes_off; break;               // int32 [N][2]
     case MWB_ARRAY_MAZE_PENDING: p = Y.pending; off = mazes_off; break;                           // uint8 [N]
+    case MWB_ARRAY_NEXT_POSE: p = P.next; n = N * E * 3; off = poses_off; break;                  // float64 [N][E][3]
+    case MWB_ARRAY_NEXT_AGENT_POSE: p = P.next_agent; n = N * 3; off = poses_off; break;          // float64 [N][3]
+    case MWB_ARRAY_POSE_PENDING: p = P.pending; off = poses_off; break;                           // uint8 [N]
+    case MWB_ARRAY_EPISODE_START: p = P.episode; n = N * 3; off = poses_off; break;               // float64 [N][3]
     case MWB_ARRAY_LEVEL_PARAMS: p = (void*)S.level_params; n = (int64_t)h->levels.size(); off = params_off; break;  // mwb_params [L]
     default: return fail(MWB_EINVAL, "unknown array");
   }

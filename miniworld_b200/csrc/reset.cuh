@@ -11,7 +11,8 @@
 // fresh world into the env's own geometry block (maze.cuh) from their level's templates; Maze variants whose
 // templates do not reproduce the host exactly reset on the host and arrive through mwb_set_world instead.  With maze layouts
 // on (mwb_enable_maze_layouts) a Maze reset can instead build a layout written into next_maze (take_maze, maze_design),
-// with the goal box and the agent in the layout's cells.
+// with the goal box and the agent in the layout's cells.  With start poses on (mwb_enable_start_poses) a reset can take
+// designed poses for the agent and the placed entities (take_poses, designed_pose), as place_entity(pos=..., dir=...).
 #pragma once
 #include "maze.cuh"
 #include "physics.cuh"
@@ -134,6 +135,28 @@ MWB_DEV int take_maze(uint8_t* pending_flag, const uint8_t* next, uint8_t* episo
   return take ? 1 : 0;
 }
 
+// Whether env i's reset takes the designed start poses (mwb_enable_start_poses; include/mwb.h states the rule): a pending
+// flag is consumed by the next reset at any level, and the rows stay as written.  As in take_seed, every lane computes
+// the same value from the same load, and warp barriers separate the load from the store.
+MWB_DEV bool take_poses(uint8_t* pending_flag) {
+  MWB_WARP_SYNC();
+  const bool take = *pending_flag != 0;
+  MWB_WARP_SYNC();
+  if (take) *pending_flag = 0;
+  MWB_WARP_SYNC();
+  return take;
+}
+
+// The designed (x, z, dir) row of the placement that fills slot e of env i, or null when the placement runs as the
+// level wrote it: the agent's call takes next_agent when its x and z are finite, then (any call) the slot's row when
+// its x and z are finite.  Out of line, like seed_stream, so that handles without the mode keep their registers.
+MWB_DEV_NOINLINE const double* designed_pose(const StartPoses* P, int i, int e, int E, int is_agent) {
+  const double* a = P->next_agent + (size_t)3 * i;
+  if (is_agent && isfinite(a[0]) && isfinite(a[1])) return a;
+  const double* r = P->next + ((size_t)i * E + e) * 3;
+  return isfinite(r[0]) && isfinite(r[1]) ? r : nullptr;
+}
+
 MWB_DEV void device_reset(const DevState& S, int i) {
   const size_t N = S.N;
   if (S.next_seed) take_seed(S, i);
@@ -151,15 +174,17 @@ MWB_DEV void device_reset(const DevState& S, int i) {
   const mwb_room* rooms = S.rooms + (size_t)g * S.R;
   int n_rooms = S.num_rooms[g];
   // bit 0: the rooms' textures are drawn (_gen_static_data ran); bits 1 / 2: a designed maze's goal / agent cell is
-  // still to be placed (one variable, so that the designed path adds no register to the loop below)
+  // still to be placed; bit 3: this reset takes designed start poses (one variable, so that the designed paths add no
+  // register to the loop below)
   int flags = 0;
+  if (S.poses && take_poses(S.poses->pending + i)) flags = 8;
   if (S.layouts) {
     const MazeLayouts& Y = *S.layouts;
     const size_t cells = (size_t)Y.rows * Y.cols;
     const bool maze = L.maze >= 0 && L.env_worlds;
     if (take_maze(Y.pending + i, Y.next + cells * i, Y.episode + cells * i, Y.rows, Y.cols,
                   maze ? S.maze[L.maze].rows : 0, maze ? S.maze[L.maze].cols : 0))
-      flags = 6;
+      flags |= 6;
   }
 
   S.step_count[i] = 0;
@@ -190,7 +215,7 @@ MWB_DEV void device_reset(const DevState& S, int i) {
       // (a Maze program's first op: flags holds only the designed bits here)
       const bool built =
           L.maze >= 0 && L.env_worlds &&
-          (flags ? maze_design(S.maze + L.maze, S.layouts->episode + (size_t)S.layouts->rows * S.layouts->cols * i,
+          ((flags & 6) ? maze_design(S.maze + L.maze, S.layouts->episode + (size_t)S.layouts->rows * S.layouts->cols * i,
                                S.layouts->cols, S.rooms + (size_t)g * S.R, S.quads + (size_t)g * S.Q,
                                S.segs + (size_t)g * S.S, S.R, S.Q, S.S, S.num_rooms + g, S.num_quads + g, S.num_segs + g)
                  : maze_generate(S, S.maze[L.maze], S.maze_cdf + (size_t)L.maze * MWB_MAZE_CDF_STRIDE, g, rng,
@@ -221,13 +246,17 @@ MWB_DEV void device_reset(const DevState& S, int i) {
         flags |= 1;
       }
       const mwb_proto& pr = S.protos[op.a];
-      const double dir = isnan(op.f[3]) ? rng_uniform(rng, -3.141592653589793, d_sub(3.141592653589793, -3.141592653589793))
-                                        : op.f[3];
+      // a designed pose replaces x and z (the level's y stays), and its dir when that is finite; append-only
+      // entities are not placed, so they keep the level's pose
+      const double* d = (flags & 8) && op.b == 0 ? designed_pose(S.poses, i, slots, S.E, 0) : nullptr;
+      const double dir = d && isfinite(d[2]) ? d[2]
+                         : isnan(op.f[3]) ? rng_uniform(rng, -3.141592653589793, d_sub(3.141592653589793, -3.141592653589793))
+                                          : op.f[3];
       const int e = slots++;
       S.ent_proto[e * N + i] = op.a;
-      S.ent_px[e * N + i] = op.f[0];
+      S.ent_px[e * N + i] = d ? d[0] : op.f[0];
       S.ent_py[e * N + i] = op.f[1];
-      S.ent_pz[e * N + i] = op.f[2];
+      S.ent_pz[e * N + i] = d ? d[1] : op.f[2];
       S.ent_dir[e * N + i] = dir;
       S.ent_size[e * N + i] = 0.0;
       for (int k = 0; k < 3; ++k) S.ent_col[((size_t)e * 3 + k) * N + i] = pr.color[k];
@@ -259,8 +288,19 @@ MWB_DEV void device_reset(const DevState& S, int i) {
         room = layout_cell_room(S.layouts->cells[2 * (size_t)i + (op.is_agent ? 1 : 0)], S.layouts->cols, M.rows, M.cols);
         flags &= op.is_agent ? ~4 : ~2;
       }
-      place_search(S, i, rng, rooms, n_rooms, room, op.f, rad, pr.radius_is_f32 != 0,
-                   op.dir_freg >= 0 ? freg[op.dir_freg & 7] : MWB_NAN, x, z, dir);
+      // a designed pose: place_entity(pos=...)'s branch (reference miniworld.py:861-867), no room, search or
+      // collision check; dir is the designed one when finite, else the level's, else uniform(-pi, pi)
+      const double* d = (flags & 8) ? designed_pose(S.poses, i, slots, S.E, op.is_agent) : nullptr;
+      if (d) {
+        x = d[0];
+        z = d[1];
+        dir = isfinite(d[2]) ? d[2]
+              : op.dir_freg >= 0 ? freg[op.dir_freg & 7]
+                                 : rng_uniform(rng, -3.141592653589793, d_sub(3.141592653589793, -3.141592653589793));
+      } else {
+        place_search(S, i, rng, rooms, n_rooms, room, op.f, rad, pr.radius_is_f32 != 0,
+                     op.dir_freg >= 0 ? freg[op.dir_freg & 7] : MWB_NAN, x, z, dir);
+      }
       int e = slots++;
       S.ent_size[e * N + i] = size;
       S.ent_proto[e * N + i] = proto;
@@ -272,6 +312,13 @@ MWB_DEV void device_reset(const DevState& S, int i) {
       if (op.is_agent) S.agent_slot[i] = e;
       S.num_slots[i] = slots;
     }
+  }
+  if (S.poses) {   // where this episode starts, designed or drawn
+    const int a = S.agent_slot[i];
+    double* st = S.poses->episode + (size_t)3 * i;
+    st[0] = S.ent_px[a * N + i];
+    st[1] = S.ent_pz[a * N + i];
+    st[2] = S.ent_dir[a * N + i];
   }
 
   // params.sample_many(rand, self, [sky_color, light_pos, light_color, light_ambient])

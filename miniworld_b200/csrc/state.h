@@ -32,6 +32,15 @@ struct MazeLayouts {
   int32_t rows, cols;
 };
 
+// The start pose arrays (mwb_enable_start_poses).  A pose is (x, z, dir); a row applies when its x and z are finite,
+// and its dir when that is finite too.
+struct StartPoses {
+  double* next;                 // [N][E][3] designed pose of each entity-list slot at the env's next reset
+  double* next_agent;           // [N][3] designed pose of the agent at the env's next reset (wins over its slot's row)
+  uint8_t* pending;             // [N] 1 = the rows wait for the env's next reset
+  double* episode;              // [N][3] the agent's pose at the start of the env's running episode
+};
+
 struct TriRec;
 struct MeshSegInfo;
 struct MazeDev;
@@ -141,6 +150,8 @@ struct DevState {
   // maze layouts (mwb_enable_maze_layouts); null on a handle without them.  One pointer to a device-side record rather
   // than its fields: every byte of DevState is a kernel parameter of every launch
   const struct MazeLayouts* layouts;
+  // start poses (mwb_enable_start_poses); null on a handle without them, one pointer for the same reason
+  const struct StartPoses* poses;
   int32_t autoreset;
   // StochasticActionWrapper on the device (reference wrappers.py:49-71): per step one uniform() draw from
   // the env's own stream; below act_prob the chosen action stands, else act_random (< 0: integers(0, 6))

@@ -26,7 +26,8 @@ class ShardedMiniWorld:
         `total_envs` envs (default: contiguous near-equal blocks), and this rank runs its slice of it.  With
         `dynamic_levels=True` (and `level_seed`) the level draws of global env i are those of the single-process run.
         `episode_seeds=True` is passed on as it is: a seed belongs to an env, so this rank's `local.next_seed` /
-        `local.episode_seed` are its slice of the single-process arrays, and so are the maze layout arrays of `maze_layouts=True`."""
+        `local.episode_seed` are its slice of the single-process arrays, and so are the maze layout arrays of `maze_layouts=True`
+        and the start pose arrays of `start_poses=True`."""
         from .batched import BatchedMiniWorld, default_env_level
         self.dist = dist
         self.rank = dist.get_rank() if dist is not None else 0

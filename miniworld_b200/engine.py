@@ -135,7 +135,7 @@ EXPORTS = (
     "mwb_snapshot_size", "mwb_snapshot", "mwb_restore", "mwb_set_obs_format",
     "mwb_flag_write", "mwb_flag_wait_geq", "mwb_flag_mode", "mwb_state_array", "mwb_debug_camera", "mwb_set_obs_peer",
     "mwb_set_levels", "mwb_enable_level_changes", "mwb_state_in_host_memory", "mwb_set_level_maze",
-    "mwb_enable_episode_seeds", "mwb_enable_maze_layouts",
+    "mwb_enable_episode_seeds", "mwb_enable_maze_layouts", "mwb_enable_start_poses",
 )
 OBS_FORMATS = {"hwc": 0, "cwh": 1, "grey": 2}
 
@@ -176,6 +176,7 @@ def load_library():
     lib.mwb_enable_level_changes.argtypes = [vp, C.c_uint64, C.c_int32]
     lib.mwb_enable_episode_seeds.argtypes = [vp]
     lib.mwb_enable_maze_layouts.argtypes = [vp]
+    lib.mwb_enable_start_poses.argtypes = [vp]
     lib.mwb_state_in_host_memory.argtypes = []
     lib.mwb_seed.argtypes = [vp, vp, C.c_int, vp]
     lib.mwb_reset.argtypes = [vp, vp, C.c_int, vp]
@@ -489,6 +490,12 @@ class Engine:
         level and capacities that fit its all-open maze."""
         self._check(self.lib.mwb_enable_maze_layouts(self.h))
 
+    def enable_start_poses(self):
+        """Resets with "pose_pending" set place the agent and the entities at the designed poses of "next_pose" /
+        "next_agent_pose", and every reset records the agent's start pose in "episode_start" from now on
+        (mwb_enable_start_poses); needs device resets."""
+        self._check(self.lib.mwb_enable_start_poses(self.h))
+
     # ---- reset
     def seed(self, env_ids, states):
         ids = np.ascontiguousarray(env_ids, np.int32)
@@ -565,13 +572,16 @@ class Engine:
         self._check(self.lib.mwb_visible_ents(self.h, _dev_or_host_ptr(mask), stream))
 
     # name -> (mwb_state_array id, element type, shape): "env" = [N], "ents" = [max_ents, N], "level" = [n_levels],
-    # "params" = [n_levels, PARAMS_DOUBLES] (mwb_params records as float64 words), "env_rows" = [N, count / N]
+    # "params" = [n_levels, PARAMS_DOUBLES] (mwb_params records as float64 words), "env_rows" = [N, count / N],
+    # "env_slots" = [N, max_ents, 3]
     ARRAYS = {"counter": (0, "<i4", "env"), "step_count": (1, "<i4", "env"), "ent_x": (2, "<f8", "ents"),
               "ent_y": (3, "<f8", "ents"), "ent_z": (4, "<f8", "ents"), "ent_dir": (5, "<f8", "ents"),
               "env_level": (6, "<i4", "env"), "next_level": (7, "<i4", "env"), "level_weights": (8, "<f4", "level"),
               "level_params": (9, "<f8", "params"), "next_seed": (16, "<i8", "env"), "episode_seed": (17, "<i8", "env"),
               "next_maze": (18, "|u1", "env_rows"), "next_maze_cells": (19, "<i4", "env_rows"),
-              "maze_pending": (20, "|u1", "env"), "episode_maze": (21, "|u1", "env_rows")}
+              "maze_pending": (20, "|u1", "env"), "episode_maze": (21, "|u1", "env_rows"),
+              "next_pose": (22, "<f8", "env_slots"), "next_agent_pose": (23, "<f8", "env_rows"),
+              "pose_pending": (24, "|u1", "env"), "episode_start": (25, "<f8", "env_rows")}
 
     def state_array(self, name, shape=None):
         """Zero-copy view of a state array (mwb_state_array) as an object with __cuda_array_interface__:
@@ -579,7 +589,9 @@ class Engine:
         "env_level" / "next_level" int32 [N] and "level_weights" float32 [n_levels]; with device resets,
         "level_params" float64 [n_levels, PARAMS_DOUBLES] (column of a field: PARAMS_COLUMN); with episode seeds on,
         "next_seed" / "episode_seed" int64 [N]; with maze layouts on, "next_maze" / "episode_maze" uint8
-        [N, rows * cols], "next_maze_cells" int32 [N, 2] and "maze_pending" uint8 [N].  `shape` gives the view
+        [N, rows * cols], "next_maze_cells" int32 [N, 2] and "maze_pending" uint8 [N]; with start poses on,
+        "next_pose" float64 [N, max_ents, 3], "next_agent_pose" / "episode_start" float64 [N, 3] and "pose_pending"
+        uint8 [N].  `shape` gives the view
         another shape of the same size (the maze layouts as [N, rows, cols]).  On the host build of the kernels the
         arrays live in host memory, and the view is a numpy array over the same memory instead."""
         which, typestr, axis = self.ARRAYS[name]
@@ -587,7 +599,8 @@ class Engine:
         self._check(self.lib.mwb_state_array(self.h, which, C.byref(ptr), C.byref(count)))
         n = count.value
         shape = tuple(shape or {"env": (self.N,), "ents": (n // self.N, self.N), "level": (n,),
-                                "params": (n, PARAMS_DOUBLES), "env_rows": (self.N, n // self.N)}[axis])
+                                "params": (n, PARAMS_DOUBLES), "env_rows": (self.N, n // self.N),
+                                "env_slots": (self.N, n // (3 * self.N), 3)}[axis])
         if int(np.prod(shape)) != (n * PARAMS_DOUBLES if axis == "params" else n):
             raise ValueError("%s has %d entries, not shape %s" % (name, n, shape))
         if self.host_memory:

@@ -21,14 +21,16 @@ class _Reg:
 
 
 class ProtoTable:
-    def __init__(self, base, strides):
-        self.base, self.strides = base, strides
+    def __init__(self, base, strides, size):
+        self.base, self.strides, self.size = base, strides, size
 
 
 class ResetProgram:
     def __init__(self):
         self.ops = []
         self.protos = []
+        self.proto_kinds = []          # class name of each prototype's entity
+        self.slots = []                # (kind, is_agent, takes a designed pose) of each entity-list slot the reset fills
         self._ireg = 0
         self._freg = 0
         self.agent_proto = self.proto(Agent())
@@ -38,7 +40,18 @@ class ResetProgram:
     # ---- prototypes
     def proto(self, ent):
         self.protos.append(proto_record(ent))
+        self.proto_kinds.append(type(ent).__name__)
         return len(self.protos) - 1
+
+    def _fill_slot(self, proto, agent, designable):
+        """Record the slot the next placement fills (the branches of one `if` fill one slot: recorded once)."""
+        if self.num_placed < len(self.slots):
+            return
+        if isinstance(proto, ProtoTable):
+            kind = "/".join(sorted(set(self.proto_kinds[proto.base:proto.base + proto.size])))
+        else:
+            kind = self.proto_kinds[int(proto)]
+        self.slots.append((kind, bool(agent), bool(designable)))
 
     def set_agent(self, agent):
         """The level changes the agent's physical constants (RoomObjects: `self.agent.radius = 1.5`)."""
@@ -49,7 +62,7 @@ class ResetProgram:
         base = len(self.protos)
         for ent in ents:
             self.proto(ent)
-        return ProtoTable(base, (1, 0))
+        return ProtoTable(base, (1, 0), len(ents))
 
     def proto_table(self, nested):
         """2-D table of entities indexed by two CHOICE results."""
@@ -59,7 +72,7 @@ class ResetProgram:
             assert len(row) == cols
             for ent in row:
                 self.proto(ent)
-        return ProtoTable(base, (cols, 1))
+        return ProtoTable(base, (cols, 1), rows * cols)
 
     # ---- per-episode topology
     def maze(self):
@@ -95,6 +108,7 @@ class ResetProgram:
         op["op"], op["a"], op["b"] = OP_PUT, int(proto), int(append_only)
         op["f"] = [float(pos[0]), float(pos[1]), float(pos[2]), math.nan if dir is None else float(dir)]
         self.ops.append(op)
+        self._fill_slot(proto, False, not append_only)
         self.num_placed += 1
         return self.num_placed - 1
 
@@ -109,6 +123,7 @@ class ResetProgram:
             self.ops.append(cond)
         if same_slot:
             self.num_placed -= 1
+        self._fill_slot(proto, _agent, True)
         op = np.zeros((), OP_DTYPE)
         op["op"] = OP_PLACE
         op["ireg_a"] = op["ireg_b"] = -1

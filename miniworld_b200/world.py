@@ -204,7 +204,9 @@ class MiniWorldEnv(gym.Env):
     # ------------------------------------------------------------------ episode control
 
     def reset(self, *, seed=None, options=None):
-        """New episode: regenerate the world (host), push it to the engine, render."""
+        """New episode: regenerate the world (host), push it to the engine, render.  `options` may hold designed start
+        poses: "poses" {slot: (x, z, dir)} for the place_entity calls that fill those entity-list slots and
+        "agent_pose" (x, z, dir) for place_agent (see place_entity); Maze levels also read a designed layout."""
         super().reset(seed=seed)
         self.step_count = 0
         self.agent = Agent()
@@ -212,7 +214,9 @@ class MiniWorldEnv(gym.Env):
         self.rooms = []
         self.wall_segs = []
         self.reset_options = options        # what the level's _gen_world may read (Maze: a designed layout)
+        self._start_design = options if options and ("poses" in options or "agent_pose" in options) else None
         self._gen_world()
+        self._start_design = None           # placements after the reset (CollectHealth's respawns) run as written
 
         rand = self.np_random if self.domain_rand else None
         self.params.sample_many(rand, self, ["sky_color", "light_pos", "light_color", "light_ambient"])
@@ -294,11 +298,20 @@ class MiniWorldEnv(gym.Env):
         link.add_portal(3, start_pos=0, end_pos=len_b)
 
     def place_entity(self, ent, room=None, pos=None, dir=None, min_x=None, max_x=None, min_z=None, max_z=None):
-        """Rejection-sample a free spot for `ent` (RNG order as reference :839-909)."""
+        """Rejection-sample a free spot for `ent` (RNG order as reference :839-909).
+        During a reset with designed start poses, the call that fills entity-list slot e = len(self.entities) takes
+        options["poses"][e], and the call for the agent takes options["agent_pose"] first, when its x and z are finite:
+        it then runs the `pos=` branch with pos = [x, y, z] (y of the level's own pos, else 0) and the designed dir
+        when finite, else the level's dir, else a uniform draw -- no room, search or collision check."""
         assert len(self.rooms) > 0, "create rooms before calling place_entity"
         assert ent.radius is not None, "entity must have physical size defined"
         if len(self.wall_segs) == 0:
             self._gen_static_data()
+        design = self._designed_pose(ent)
+        if design is not None:
+            x, z, d = design
+            pos = np.array([x, 0.0 if pos is None else float(pos[1]), z])
+            dir = d if math.isfinite(d) else dir
         if pos is not None:
             ent.dir = dir if dir is not None else self.np_random.uniform(-math.pi, math.pi)
             ent.pos = pos
@@ -321,6 +334,21 @@ class MiniWorldEnv(gym.Env):
             break
         self.entities.append(ent)
         return ent
+
+    def _designed_pose(self, ent):
+        """(x, z, dir) of the designed start pose that applies to placing `ent` now, or None."""
+        design = getattr(self, "_start_design", None)
+        if design is None:
+            return None
+        rows = [design.get("agent_pose")] if ent is self.agent else []
+        rows.append((design.get("poses") or {}).get(len(self.entities)))
+        for row in rows:
+            if row is not None:
+                x, z = float(row[0]), float(row[1])
+                d = float(row[2]) if len(row) > 2 and row[2] is not None else math.nan
+                if math.isfinite(x) and math.isfinite(z):
+                    return x, z, d
+        return None
 
     def place_agent(self, room=None, pos=None, dir=None, min_x=None, max_x=None, min_z=None, max_z=None):
         return self.place_entity(self.agent, room=room, pos=pos, dir=dir,
