@@ -453,6 +453,41 @@ int mwb_enable_maze_layouts(mwb_handle* h);
  * compared. */
 int mwb_enable_start_poses(mwb_handle* h);
 
+/* State bank (Go-Explore, backplay and demonstration-start curricula, branching rollouts): save env states into device
+ * records and start an env's next episode from one.  Valid on a handle with device resets, after the level table, any
+ * Maze levels and the other modes are set up: MWB_ESTATE when the handle resets on the host or has the bank on already,
+ * and every later mwb_enable_* / mwb_set_levels / mwb_set_maze / mwb_set_level_maze call fails with MWB_ESTATE, because
+ * the record layout depends on them.  MWB_EINVAL for slots < 1.  Allocates `slots` records and three int32 arrays,
+ * read and written in place through mwb_state_array, stream-ordered, without a sync:
+ *   next_state [N]         slot env i's next reset loads, -1 = none (all -1 at the call);
+ *   episode_state [N]      slot the running episode was loaded from, -1 = it ran the level's program; after a
+ *                          terminating step it still names the episode that ended;
+ *   bank_level [slots]     level of the state each slot holds, -1 = empty (all -1 at the call; treat as read-only).
+ * A record is everything a running episode is: the entity list (proto, pose, colour, size), num_slots, agent_slot,
+ * carrying, step_count, the counter (CollectHealth's health), the camera, sky and light parameters, max_forward_step,
+ * the ghost entity, the RNG stream, the env's room texture variants, env_level, the episode_seed / episode_maze /
+ * episode_start records of the modes that are on and, when the saved env's level has per-env worlds, its world block
+ * (the rooms, quads and segments in use).  Not in a record: needs_reset, the pending inputs (next_level, level_draws,
+ * next_seed, the pending layout, cells and poses), next_state, episode_state, episodes_done, the level table and its
+ * params.
+ * At every reset of env i (mwb_reset, and the next-step auto-reset inside mwb_step) with next_state[i] = s >= 0, before
+ * anything else, next_state[i] = -1; then, when slot s exists and is filled and its level is the env's level or level
+ * changes are on, env i becomes the record bit for bit (env_level included), episode_state[i] = s, and no program runs
+ * and nothing is drawn: every other pending input stays pending for the next reset that runs a program.  Otherwise the
+ * entry is dropped, the reset runs as it would have, and episode_state[i] = -1.  So a loaded env's future under the
+ * same actions is the saved env's, its auto-resets included; the level's current params apply to its per-step draws,
+ * and its step_count is the saved one.  Handles that never call this behave exactly as before it existed, and the
+ * addition changes no struct, so MWB_ABI_VERSION stays as it is.  Snapshots of a handle with the bank carry the
+ * records and the three arrays and are marked as such in the header; restoring across the mode fails with MWB_ESTATE,
+ * and into a bank of another size with MWB_EINVAL. */
+int mwb_enable_state_bank(mwb_handle* h, int32_t slots);
+/* Copy env env_ids[t] into slot slots[t] for t in [0, n) and set bank_level[slots[t]] to the env's level.  A slot
+ * named more than once takes its last entry.  Both arrays are host memory, checked here (MWB_EINVAL for an env or slot
+ * out of range), or both device memory: then the call enqueues on `stream` (null: the handle's stream, and the call
+ * returns finished) without a check on the host, and entries with an env or slot out of range are skipped on the
+ * device.  MWB_ESTATE without the bank. */
+int mwb_save_states(mwb_handle* h, const int32_t* env_ids, const int32_t* slots, int n, void* stream);
+
 /* Maze levels in a level table (curricula over maze sizes: MazeS2 -> MazeS3 -> Maze, next to fixed-layout levels).
  * Valid on a shared_geometry = 1 handle after mwb_set_levels (MWB_ESTATE otherwise).  Level `level` (MWB_EINVAL
  * outside [0, L)) becomes a per-env-world level: every reset of an env at that level carves a fresh maze from these
@@ -620,6 +655,10 @@ int mwb_debug_camera(mwb_handle* h, float* out /* host [num_envs][16] */);
 #define MWB_ARRAY_NEXT_AGENT_POSE 23  /* float64 [num_envs][3]  designed (x, z, dir) of the agent, next reset         */
 #define MWB_ARRAY_POSE_PENDING 24     /* uint8 [num_envs]  nonzero = the designed poses wait for the next reset       */
 #define MWB_ARRAY_EPISODE_START 25    /* float64 [num_envs][3]  the agent's (x, z, dir) when the episode started      */
+/* with the state bank on (mwb_enable_state_bank; MWB_ESTATE otherwise): */
+#define MWB_ARRAY_NEXT_STATE 26       /* int32 [num_envs]  slot the env's next reset loads, -1 = none                  */
+#define MWB_ARRAY_EPISODE_STATE 27    /* int32 [num_envs]  slot the running episode was loaded from, -1 = none         */
+#define MWB_ARRAY_BANK_LEVEL 28       /* int32 [slots]  level of the state each slot holds, -1 = empty                 */
 int mwb_state_array(mwb_handle* h, int which, void** dev_ptr, int64_t* count);
 /* 1 when this library keeps the handle's state arrays (mwb_state_array) in host memory -- the CPU build of the kernels
  * used by the test suite -- and 0 for libmwb.so, whose arrays are device memory. */

@@ -20,7 +20,9 @@ Per-environment semantics are exactly those of the reference's `MiniWorldEnv.res
   * with `maze_layouts=True`, an env's next reset at a Maze level can build a maze written into a device tensor
     (`next_maze`, `set_env_maze`), and `info["maze"]` holds the layout of each running episode;
   * with `start_poses=True`, an env's next reset can place the agent and the entities at poses written into device
-    tensors (`next_pose`, `set_env_pose`), and `info["start"]` holds where each running episode's agent started.
+    tensors (`next_pose`, `set_env_pose`), and `info["start"]` holds where each running episode's agent started;
+  * with `state_bank=K`, envs can be saved into K device-side records (`save_states`) and an env's next reset can load
+    one (`next_state`, `set_env_state`), and `info["state"]` names the record each running episode was loaded from.
 
 Outputs are torch CUDA tensors by default (zero-copy from the kernels); `step_host`
 performs the same step with pinned host buffers for callers that want numpy.
@@ -170,6 +172,8 @@ _NEEDS = {**dict.fromkeys(("env_level", "next_level", "level_weights"), (
               "maze_layouts", RuntimeError, "this batch has no maze layouts: construct it with maze_layouts=True")),
           **dict.fromkeys(("next_pose", "next_agent_pose", "pose_pending", "episode_start"), (
               "start_poses", RuntimeError, "this batch has no start poses: construct it with start_poses=True")),
+          **dict.fromkeys(("next_state", "episode_state", "bank_level"), (
+              "state_bank", RuntimeError, "this batch has no state bank: construct it with state_bank=K")),
           "level_params": ("device_reset", TypeError, "level params change at device resets; host-reset levels draw "
                            "theirs in Python (set them on the level's own DomainParams)")}
 
@@ -250,12 +254,25 @@ class BatchedMiniWorld:
     rows as written.  A design that leaves a later searched placement of the same reset no free spot makes that search
     run forever, as it would in the reference.  `level_slots` names the slots each level fills.  `episode_start` / `info["start"]` hold the
     agent's (x, z, dir) at the start of every running episode, designed or drawn; after a terminating step they still
-    name the episode that just ended."""
+    name the episode that just ended.
+
+    `state_bank=K` (one level or a table; levels that reset on the device) keeps K records of env states on the device,
+    for Go-Explore, backplay and branching rollouts: `save_states(env_ids, slots)` copies env env_ids[t] into slot
+    slots[t] (entity list, counters, health, camera, lighting, colours, textures, the RNG stream, the level, the mode
+    records and, at levels with per-env worlds, the world in use).  With `next_state[i] = s` (`set_env_state`), env i's
+    next reset, the auto-reset inside `step` included, becomes slot s bit for bit instead of running the level's program,
+    when the slot is filled and holds the env's level (any level with `dynamic_levels=True`); otherwise the entry is
+    dropped and the reset runs as it would have.  The load consumes only `next_state`: a pending level, seed, layout or
+    pose waits for the next reset that runs a program.  A loaded env continues exactly as the saved env would have,
+    `step_count` included.  `episode_state` / `info["state"]` name the slot each running episode was loaded from, or -1;
+    after a terminating step they still name the episode that just ended.  `bank_level` holds each slot's level (-1 =
+    empty).  A record takes about 264 B + 68 B per entity slot + 12 B per room; at levels with per-env worlds it has
+    room for one world block as well (about 123 KB for an 8 x 8 Maze), so 4096 slots of such a batch take over 0.5 GB."""
 
     def __init__(self, level, num_envs, obs_width=80, obs_height=60, domain_rand=False, autoreset=True,
                  msaa_samples=8, device=0, want_depth=False, level_kwargs=None, obs_format="hwc", env_level=None,
                  dynamic_levels=False, level_seed=0, env_offset=0, per_env_worlds=False, episode_seeds=False,
-                 maze_layouts=False, start_poses=False):
+                 maze_layouts=False, start_poses=False, state_bank=None):
         self.num_envs = int(num_envs)
         self.obs_width, self.obs_height = int(obs_width), int(obs_height)
         self.domain_rand = bool(domain_rand)
@@ -266,6 +283,11 @@ class BatchedMiniWorld:
         self.episode_seeds = bool(episode_seeds)
         self.maze_layouts = bool(maze_layouts)
         self.start_poses = bool(start_poses)
+        if state_bank is not None and (isinstance(state_bank, bool) or not isinstance(state_bank, (int, np.integer))
+                                       or state_bank < 1):
+            raise ValueError("state_bank is a number of slots >= 1, got %r" % (state_bank,))
+        self.bank_slots = int(state_bank or 0)
+        self.state_bank = self.bank_slots > 0
         table = isinstance(level, (list, tuple))
         if table:
             defs = self._init_levels(list(level), level_kwargs, env_level)
@@ -283,7 +305,8 @@ class BatchedMiniWorld:
         self._init_engine(defs, table, msaa_samples, autoreset)
         self._view_map = _Views(self.engine, self.device, dict(
             dynamic_levels=self.dynamic_levels, episode_seeds=self.episode_seeds, maze_layouts=self.maze_layouts,
-            start_poses=self.start_poses, device_reset=self.device_reset), getattr(self, "maze_shape", None))
+            start_poses=self.start_poses, state_bank=self.state_bank, device_reset=self.device_reset),
+            getattr(self, "maze_shape", None))
         if self.dynamic_levels:
             self.level_seed, self.env_offset = int(level_seed), int(env_offset)
             self.engine.enable_level_changes(self.level_seed, self.env_offset)
@@ -300,6 +323,12 @@ class BatchedMiniWorld:
                 raise TypeError("start poses are taken by device resets; host-reset levels place entities in Python "
                                 "(reset(options={\"poses\": ...}) of the level itself)")
             self.engine.enable_start_poses()
+        if self.state_bank:
+            if not self.device_reset:
+                self.engine.close()
+                raise TypeError("the state bank loads states at device resets; host-reset levels keep their worlds and "
+                                "RNG streams in Python")
+            self.engine.enable_state_bank(self.bank_slots)     # last: the record layout depends on the other modes
         # observation layout written by the render kernel: the reference's PyTorchObsWrapper ("cwh") and
         # GreyscaleWrapper ("grey") are fused into its epilogue instead of running as separate passes
         self.obs_format = obs_format
@@ -487,6 +516,10 @@ class BatchedMiniWorld:
                 # the agent's (x, z, dir) at the start of each env's current episode (after a terminating step still
                 # the ended one's)
                 self._info["start"] = self.episode_start
+            if self.state_bank:
+                # the slot each env's current episode was loaded from, -1 for none (after a terminating step still the
+                # ended one's)
+                self._info["state"] = self.episode_state
         return self._torch
 
     # ------------------------------------------------------------------ run-time arrays
@@ -495,7 +528,7 @@ class BatchedMiniWorld:
         return self._view_map
 
     def _write_pending(self, what, ids, arrays):
-        """The part set_env_level / set_env_seed / set_env_maze / set_env_pose share: check the env ids `ids` (1-D
+        """The part set_env_level / set_env_seed / set_env_maze / set_env_pose / set_env_state share: check the env ids `ids` (1-D
         integers in [0, N)), then write each (array name or view, values) of `arrays` at those envs -- values one per id
         (a numpy array, or a CUDA tensor) or one for all -- an env listed more than once taking its last entry.  On the host build the write is
         numpy's; on the device it is torch ops on the current stream, without a sync."""
@@ -722,6 +755,87 @@ class BatchedMiniWorld:
         else:
             rows = np.stack([np.broadcast_to(c, ids.shape) for c in comps], axis=1)
         self._write_pending("set_env_pose", ids, [(target, rows), ("pose_pending", 1)])
+
+    # ------------------------------------------------------------------ state bank (state_bank=K)
+    @property
+    def next_state(self):
+        """int32 [N] view of the slot each env's next reset loads, -1 for none; write it in place (stream-ordered, no
+        sync).  The reset that takes an entry clears it to -1, loaded or not."""
+        return self._views()["next_state"]
+
+    @property
+    def episode_state(self):
+        """int32 [N] view of the slot each env's running episode was loaded from, -1 when it ran the level's program."""
+        return self._views()["episode_state"]
+
+    @property
+    def bank_level(self):
+        """int32 [K] view of the level of the state each slot holds, -1 for an empty slot (read-only)."""
+        return self._views()["bank_level"]
+
+    def entity_xz(self, slot):
+        """float64 [N, 2]: the (x, z) floor position of entity-list slot `slot` of every env, read from the device
+        state by torch ops without a sync (a numpy array on the host build).  `level_slots` names each level's agent
+        slot (FourRooms: 1)."""
+        x, z = self._views()["ent_x"][slot], self._views()["ent_z"][slot]
+        return np.stack([x, z], 1) if isinstance(x, np.ndarray) else self._ensure_torch().stack([x, z], 1)
+
+    def _bank_ids(self, what, env_ids, slots, lo):
+        """(env ids, slots) of save_states / set_env_state: host values as 1-D int64 numpy arrays, checked (env ids in
+        [0, N), slots in [lo, K)); a CUDA tensor stays on the device, unchecked."""
+        self._views()["next_state"]                  # a batch without the bank raises before any input check
+        out = []
+        for name, v, bound in (("env ids", env_ids, (0, self.num_envs)), ("slots", slots, (lo, self.bank_slots))):
+            if hasattr(v, "is_cuda") and v.is_cuda:
+                if v.dim() > 1 or v.dtype.is_floating_point or v.dtype == self._ensure_torch().bool:
+                    raise ValueError("%s: %s are a 1-D integer tensor" % (what, name))
+                out.append(v)
+                continue
+            a = np.atleast_1d(_host(v))
+            if a.ndim != 1 or not (np.issubdtype(a.dtype, np.integer) or a.size == 0):
+                raise ValueError("%s: %s are integers, one or a 1-D sequence" % (what, name))
+            if a.size and (a.min() < bound[0] or a.max() >= bound[1]):
+                raise ValueError("%s: %s must lie in [%d, %d)" % (what, name, bound[0], bound[1]))
+            out.append(a.astype(np.int64))
+        return out
+
+    def save_states(self, env_ids, slots):
+        """Copy env env_ids[t] into slot slots[t] (ints, numpy arrays or CUDA tensors of one length).  A slot named more
+        than once keeps its last entry.  Host values are checked; CUDA tensors are taken as they are, entries out of
+        range skipped on the device.  The copy is enqueued on torch's current stream without a sync (on the host build
+        of the kernels it runs in the call)."""
+        ids, sl = self._bank_ids("save_states", env_ids, slots, 0)
+        if ids.shape[0] != sl.shape[0]:
+            raise ValueError("save_states: %d env ids but %d slots" % (ids.shape[0], sl.shape[0]))
+        if ids.shape[0] == 0:
+            return
+        if self.engine.host_memory:
+            self.engine.save_states(ids.astype(np.int32), sl.astype(np.int32))
+            return
+        torch = self._ensure_torch()
+        dev = torch.device("cuda", self.device)
+        ids, sl = (torch.as_tensor(a).to(dev, torch.int32, non_blocking=True).contiguous() for a in (ids, sl))
+        self.engine.save_states(ids, sl, stream=_torch_stream(torch, self.device))
+
+    def set_env_state(self, env_ids, slots):
+        """Start the listed envs' next episodes from `slots` (one slot, or one per env; -1 cancels a pending entry);
+        envs in mid-episode finish it first.  An env listed more than once takes its last entry.  Host slots must lie
+        in [-1, K); CUDA tensors are written as they are.  The write is numpy's on the host build, torch ops on the
+        current stream without a sync on the device."""
+        ids, sl = self._bank_ids("set_env_state", env_ids, slots, -1)
+        if hasattr(ids, "is_cuda"):
+            raise ValueError("set_env_state takes host env ids (write next_state in place for device ones)")
+        if not hasattr(sl, "is_cuda"):
+            if np.ndim(slots) == 0:
+                sl = np.broadcast_to(sl, ids.shape)
+            if sl.shape != ids.shape:
+                raise ValueError("set_env_state: %d env ids but %d slots" % (ids.size, sl.size))
+            sl = sl.astype(np.int32)
+        elif sl.dim() and tuple(sl.shape) != ids.shape:
+            raise ValueError("set_env_state: %d env ids but %d slots" % (ids.size, sl.numel()))
+        else:
+            sl = sl.to(self._ensure_torch().int32)
+        self._write_pending("set_env_state", ids, [("next_state", sl)])
 
     # ------------------------------------------------------------------ level params at run time
     def set_level_param(self, level, name, default=None, min=None, max=None):
@@ -950,9 +1064,9 @@ class BatchedMiniWorld:
     def _torch_writes(self):
         """True when torch work may write arrays the kernels read: next_level / level_weights (level changes on),
         next_seed (episode seeds on), the pending maze layouts (maze layouts on), the designed start poses (start poses
-        on) or the params table (once set_level_param has written it)."""
+        on), the pending slots (state bank on) or the params table (once set_level_param has written it)."""
         return ((self.dynamic_levels or self.episode_seeds or self.maze_layouts or self.start_poses
-                 or self._params_written)
+                 or self.state_bank or self._params_written)
                 and not self.engine.host_memory)
 
     def _level_stream(self):

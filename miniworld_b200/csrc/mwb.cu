@@ -123,6 +123,9 @@ struct mwb_handle {
   std::vector<MazeDev> mazes_h;       // host copies of S.maze / S.maze_cdf, one entry per level
   MazeLayouts layouts_h;              // host copy of *S.layouts (mwb_enable_maze_layouts)
   StartPoses poses_h;                 // host copy of *S.poses (mwb_enable_start_poses)
+  StateBank bank_h;                   // host copy of *S.bank (mwb_enable_state_bank)
+  int32_t* d_bank_pairs;              // [2][slots] staging of a host mwb_save_states call (env ids, then slots)
+  int32_t* d_bank_winner;             // [slots] per-call scratch: the last entry of each slot
   std::vector<double> maze_cdf_h;
   bool have_params, have_protos, have_template;
   bool have_level_table;          // mwb_set_levels succeeded (mwb_enable_level_changes needs it)
@@ -358,6 +361,21 @@ __global__ void reset_kernel(DevState S, const int32_t* ids, int n) {
   int i = ids ? ids[t] : t;
   device_reset(S, i);
   S.needs_reset[i] = 0;
+}
+// mwb_save_states: the winning entry of every slot (the last one naming it), then one warp per entry that won.  Entries
+// with an env or slot out of range take no part and are never indexed.
+__global__ void bank_mark_kernel(const int32_t* envs, const int32_t* slots, int n, int N, int nslots, int32_t* winner) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= n) return;
+  const int e = envs[t], s = slots[t];
+  if (e >= 0 && e < N && s >= 0 && s < nslots) atomicMax(winner + s, t);
+}
+__global__ void bank_save_kernel(DevState S, const int32_t* envs, const int32_t* slots, int n, const int32_t* winner) {
+  const int t = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (t >= n) return;
+  const int e = envs[t], s = slots[t];
+  if (e < 0 || e >= S.N || s < 0 || s >= S.bank->slots || winner[s] != t) return;
+  bank_save(S.bank, S.env_level, S.levels, e, s);
 }
 __global__ void scatter_kernel(DevState S, const WorldUpload* u, int n) {
   int t = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1263,6 +1281,7 @@ extern "C" int mwb_set_levels(mwb_handle* h, int n_levels, const mwb_level* leve
   if (!h || !levels || !templates || !ops || !env_level) return fail(MWB_EINVAL, "null argument");
   if (!h->cfg.shared_geometry) return fail(MWB_EINVAL, "a level table needs shared_geometry = 1 (per-env worlds have no templates)");
   if (h->S.next_level) return fail(MWB_ESTATE, "the level table is fixed once level changes are on");
+  if (h->S.bank) return fail(MWB_ESTATE, "the level table is fixed once the state bank is on (its record layout depends on it)");
   if (h->level_mazes) return fail(MWB_ESTATE, "the level table is fixed once it has Maze levels (mwb_set_level_maze)");
   if (n_levels <= 0) return fail(MWB_EINVAL, "n_levels must be positive");
   if (n_levels > MWB_LEVEL_CAP) return fail(MWB_ECAPACITY, "more than MWB_LEVEL_CAP levels");
@@ -1341,6 +1360,7 @@ extern "C" int mwb_enable_level_changes(mwb_handle* h, uint64_t seed, int32_t en
   if (!h) return fail(MWB_EINVAL, "null handle");
   if (!h->have_level_table) return fail(MWB_ESTATE, "level changes need a level table (mwb_set_levels first)");
   if (h->S.next_level) return fail(MWB_ESTATE, "level changes are already on");
+  if (h->S.bank) return fail(MWB_ESTATE, "level changes cannot be turned on once the state bank is on (its record layout depends on it)");
   if (env_offset < 0) return fail(MWB_EINVAL, "env_offset must not be negative");
   DevState& S = h->S;
   void *next, *draws, *weights;
@@ -1359,6 +1379,7 @@ extern "C" int mwb_enable_level_changes(mwb_handle* h, uint64_t seed, int32_t en
 extern "C" int mwb_enable_episode_seeds(mwb_handle* h) {
   if (!h) return fail(MWB_EINVAL, "null handle");
   if (h->S.next_seed) return fail(MWB_ESTATE, "episode seeds are already on");
+  if (h->S.bank) return fail(MWB_ESTATE, "episode seeds cannot be turned on once the state bank is on (its record layout depends on it)");
   if (!h->have_params || !h->S.ops)
     return fail(MWB_ESTATE, "episode seeds need device resets (params and a reset program: mwb_set_levels, or "
                             "mwb_set_params and mwb_set_program); host-generated worlds keep their streams on the host");
@@ -1418,6 +1439,7 @@ static int put_maze(mwb_handle* h, int level, const mwb_maze_desc* mz) {
 extern "C" int mwb_set_maze(mwb_handle* h, const mwb_maze_desc* mz) {
   if (!h || !mz || !mz->cdf) return fail(MWB_EINVAL, "null argument");
   if (h->cfg.shared_geometry) return fail(MWB_ESTATE, "Maze needs per-env geometry (shared_geometry = 0)");
+  if (h->S.bank) return fail(MWB_ESTATE, "the Maze templates are fixed once the state bank is on (its record layout depends on it)");
   const int cells = mz->rows * mz->cols;
   if (cells <= 0 || cells > MWB_MAZE_MAX_CELLS) return fail(MWB_ECAPACITY, "maze too large");
   if (2 * cells - 1 > h->S.R) return fail(MWB_ECAPACITY, "max_rooms too small for this maze");
@@ -1462,6 +1484,7 @@ extern "C" int mwb_set_level_maze(mwb_handle* h, int level, const mwb_maze_desc*
   if (!h->cfg.shared_geometry || !h->have_level_table)
     return fail(MWB_ESTATE, "Maze levels in a table need a shared_geometry = 1 handle and mwb_set_levels first");
   if (level < 0 || level >= (int)h->levels.size()) return fail(MWB_EINVAL, "level out of range");
+  if (h->S.bank) return fail(MWB_ESTATE, "Maze levels cannot be added once the state bank is on (its record layout depends on it)");
   const int cells = mz->rows * mz->cols;
   if (cells <= 0 || cells > MWB_MAZE_MAX_CELLS) return fail(MWB_ECAPACITY, "maze too large");
   // a maze of c cells is a spanning tree: 2c - 1 rooms, 8c - 2 quads and 4c segments, whatever the episode draws
@@ -1481,6 +1504,7 @@ extern "C" int mwb_set_level_maze(mwb_handle* h, int level, const mwb_maze_desc*
 extern "C" int mwb_enable_maze_layouts(mwb_handle* h) {
   if (!h) return fail(MWB_EINVAL, "null handle");
   if (h->S.layouts) return fail(MWB_ESTATE, "maze layouts are already on");
+  if (h->S.bank) return fail(MWB_ESTATE, "maze layouts cannot be turned on once the state bank is on (its record layout depends on it)");
   if (!h->have_params || !h->S.ops)
     return fail(MWB_ESTATE, "maze layouts need device resets (mwb_set_maze or mwb_set_level_maze on a handle with a "
                             "reset program); host-generated worlds are built on the host");
@@ -1528,6 +1552,7 @@ extern "C" int mwb_enable_maze_layouts(mwb_handle* h) {
 extern "C" int mwb_enable_start_poses(mwb_handle* h) {
   if (!h) return fail(MWB_EINVAL, "null handle");
   if (h->S.poses) return fail(MWB_ESTATE, "start poses are already on");
+  if (h->S.bank) return fail(MWB_ESTATE, "start poses cannot be turned on once the state bank is on (its record layout depends on it)");
   if (!h->have_params || !h->S.ops)
     return fail(MWB_ESTATE, "start poses need device resets (params and a reset program: mwb_set_levels, or "
                             "mwb_set_params and mwb_set_program); host-generated worlds are placed on the host");
@@ -1548,6 +1573,155 @@ extern "C" int mwb_enable_start_poses(mwb_handle* h) {
   if (alloc_arr(h, &d, 1)) return fail(MWB_ECUDA, "start pose state allocation failed");
   if (h2d(d, &P, sizeof(P), h->stream) != 0 || sync_stream(h->stream) != 0) return fail(MWB_ECUDA, "upload failed");
   S.poses = d;
+  return MWB_OK;
+}
+
+// The record layout of the handle as it stands (StateBank in state.h): the scalars of one env, widest first so that
+// each lands aligned, then the world section on handles with per-env worlds.
+static void bank_layout(const mwb_handle* h, std::vector<BankCol>& cols, StateBank& B) {
+  const DevState& S = h->S;
+  const size_t N = S.N, E = S.E;
+  int32_t off = 0;
+  // k components of a structure-of-arrays row ([k][N]) or of an [N][k] array (`rows`)
+  auto add = [&](const void* p, int bytes, size_t k, bool rows) {
+    for (size_t c = 0; c < k; ++c) {
+      BankCol col;
+      col.base = (uint8_t*)p + (rows ? c : c * N) * bytes;
+      col.env_stride = rows ? (int32_t)(k * bytes) : bytes;
+      col.rec_off = off;
+      col.bytes = bytes;
+      col.pad_ = 0;
+      cols.push_back(col);
+      off += bytes;
+    }
+  };
+  add(S.ent_px, 8, E, false); add(S.ent_py, 8, E, false); add(S.ent_pz, 8, E, false); add(S.ent_dir, 8, E, false);
+  add(S.ent_col, 8, 3 * E, false); add(S.ent_size, 8, E, false);
+  add(S.cam, 8, 4, false); add(S.envp, 8, 12, false); add(S.env_mfs, 8, 1, false);
+  add(S.ghost_pose, 8, 4, false); add(S.ghost_col, 8, 3, false);
+  add(S.rng_s_hi, 8, 1, false); add(S.rng_s_lo, 8, 1, false); add(S.rng_inc_hi, 8, 1, false); add(S.rng_inc_lo, 8, 1, false);
+  if (S.next_seed) add(S.episode_seed, 8, 1, false);
+  if (S.poses) add(h->poses_h.episode, 8, 3, true);
+  add(S.ent_proto, 4, E, false);
+  add(S.num_slots, 4, 1, false); add(S.agent_slot, 4, 1, false); add(S.carrying, 4, 1, false);
+  add(S.step_count, 4, 1, false); add(S.num_picked, 4, 1, false); add(S.ghost_slot, 4, 1, false);
+  add(S.ghost_proto, 4, 1, false); add(S.rng_has32, 4, 1, false); add(S.rng_cache, 4, 1, false);
+  add(S.env_level, 4, 1, false);
+  add(S.room_tex, 4, (size_t)S.R * 3, true);
+  if (S.layouts) add(h->layouts_h.episode, 1, (size_t)h->layouts_h.rows * h->layouts_h.cols, true);
+  auto align16 = [](size_t x) { return (int32_t)((x + 15) & ~(size_t)15); };
+  B.world_off = B.room_off = B.quad_off = B.seg_off = -1;
+  size_t end = off;
+  if (h->level_mazes || !h->cfg.shared_geometry) {
+    B.world_off = align16(off);
+    B.room_off = B.world_off + 16;
+    B.quad_off = align16(B.room_off + (size_t)S.R * sizeof(mwb_room));
+    B.seg_off = align16(B.quad_off + (size_t)S.Q * sizeof(mwb_quad));
+    end = B.seg_off + (size_t)S.S * sizeof(mwb_seg);
+  }
+  B.rec_bytes = align16(end);
+  B.num_cols = (int32_t)cols.size();
+  B.env_geom = S.env_geom;
+  B.R = S.R;
+  B.Q = S.Q;
+  B.S = S.S;
+  B.num_rooms = S.num_rooms;
+  B.num_quads = S.num_quads;
+  B.num_segs = S.num_segs;
+  B.rooms = S.rooms;
+  B.quads = S.quads;
+  B.segs = S.segs;
+}
+
+extern "C" int mwb_enable_state_bank(mwb_handle* h, int32_t slots) {
+  if (!h) return fail(MWB_EINVAL, "null handle");
+  if (h->S.bank) return fail(MWB_ESTATE, "the state bank is already on");
+  if (!h->have_params || !h->S.ops)
+    return fail(MWB_ESTATE, "the state bank needs device resets (params and a reset program: mwb_set_levels, or "
+                            "mwb_set_params and mwb_set_program); host-generated worlds are reset on the host");
+  if (slots < 1) return fail(MWB_EINVAL, "slots must be at least 1");
+  DevState& S = h->S;
+  std::vector<BankCol> cols;
+  StateBank& B = h->bank_h;
+  bank_layout(h, cols, B);
+  void *records, *level, *next, *episode, *pairs, *winner, *dcols;
+  int rc = alloc_control_arrays(h, "state bank", {{&records, (size_t)slots * B.rec_bytes, false},
+                                                  {&level, (size_t)slots * sizeof(int32_t), true},
+                                                  {&next, (size_t)S.N * sizeof(int32_t), true},
+                                                  {&episode, (size_t)S.N * sizeof(int32_t), true},
+                                                  {&pairs, 2 * (size_t)slots * sizeof(int32_t), false},
+                                                  {&winner, (size_t)slots * sizeof(int32_t), false},
+                                                  {&dcols, cols.size() * sizeof(BankCol), false}});
+  if (rc) return rc;
+  B.records = (uint8_t*)records;
+  B.bank_level = (int32_t*)level;
+  B.next_state = (int32_t*)next;
+  B.episode_state = (int32_t*)episode;
+  B.cols = (const BankCol*)dcols;
+  B.slots = slots;
+  h->d_bank_pairs = (int32_t*)pairs;
+  h->d_bank_winner = (int32_t*)winner;
+  StateBank* d = nullptr;
+  if (alloc_arr(h, &d, 1)) return fail(MWB_ECUDA, "state bank allocation failed");
+  if (h2d(dcols, cols.data(), cols.size() * sizeof(BankCol), h->stream) != 0 || h2d(d, &B, sizeof(B), h->stream) != 0 ||
+      sync_stream(h->stream) != 0)
+    return fail(MWB_ECUDA, "upload failed");
+  S.bank = d;
+  return MWB_OK;
+}
+
+extern "C" int mwb_save_states(mwb_handle* h, const int32_t* env_ids, const int32_t* slots, int n, void* stream) {
+  if (!h) return fail(MWB_EINVAL, "null handle");
+  if (!h->S.bank) return fail(MWB_ESTATE, "the state bank is off (mwb_enable_state_bank)");
+  if (n < 0 || (n > 0 && (!env_ids || !slots))) return fail(MWB_EINVAL, "bad arguments");
+  if (n == 0) return MWB_OK;
+  const StateBank& B = h->bank_h;
+  const bool dev_ids = is_device_ptr(env_ids), dev_slots = is_device_ptr(slots);
+  if (dev_ids != dev_slots) return fail(MWB_EINVAL, "env_ids and slots must both be device or both be host memory");
+  stream_t s = stream ? (stream_t)stream : h->stream;
+  const int32_t *e = env_ids, *k = slots;
+  if (!dev_ids) {
+    // checked here; a slot named twice keeps its last entry (so at most `slots` pairs go up)
+    std::vector<int32_t> seen(B.slots, 0), up;
+    for (int t = n - 1; t >= 0; --t) {
+      if (env_ids[t] < 0 || env_ids[t] >= h->S.N) return fail(MWB_EINVAL, "env id out of range");
+      if (slots[t] < 0 || slots[t] >= B.slots) return fail(MWB_EINVAL, "slot out of range");
+    }
+    for (int t = n - 1; t >= 0; --t)
+      if (!seen[slots[t]]) {
+        seen[slots[t]] = 1;
+        up.push_back(t);
+      }
+    n = (int)up.size();
+    std::vector<int32_t> pairs(2 * (size_t)n);
+    for (int t = 0; t < n; ++t) {
+      pairs[t] = env_ids[up[n - 1 - t]];
+      pairs[n + t] = slots[up[n - 1 - t]];
+    }
+    if (stream_enter(h, s)) return MWB_ECUDA;
+    if (h2d(h->d_bank_pairs, pairs.data(), pairs.size() * sizeof(int32_t), s) != 0) return fail(MWB_ECUDA, "upload failed");
+    e = h->d_bank_pairs;
+    k = h->d_bank_pairs + n;
+  } else if (stream_enter(h, s)) {
+    return MWB_ECUDA;
+  }
+#ifndef MWB_HOSTSIM
+  CK(cudaMemsetAsync(h->d_bank_winner, 0xFF, (size_t)B.slots * sizeof(int32_t), s));
+  bank_mark_kernel<<<(n + 127) / 128, 128, 0, s>>>(e, k, n, h->S.N, B.slots, h->d_bank_winner);
+  bank_save_kernel<<<(unsigned)(((size_t)n + 3) / 4), 128, 0, s>>>(h->S, e, k, n, h->d_bank_winner);
+  h->launches += 2;
+  CK(cudaGetLastError());
+  if (stream_leave(h, s)) return MWB_ECUDA;
+  if (!stream) CK(cudaStreamSynchronize(s));
+#else
+  int32_t* winner = h->d_bank_winner;
+  for (int q = 0; q < B.slots; ++q) winner[q] = -1;
+  for (int t = 0; t < n; ++t)
+    if (e[t] >= 0 && e[t] < h->S.N && k[t] >= 0 && k[t] < B.slots && t > winner[k[t]]) winner[k[t]] = t;
+  for (int t = 0; t < n; ++t)
+    if (e[t] >= 0 && e[t] < h->S.N && k[t] >= 0 && k[t] < B.slots && winner[k[t]] == t)
+      bank_save(h->S.bank, h->S.env_level, h->S.levels, e[t], k[t]);
+#endif
   return MWB_OK;
 }
 
@@ -2135,11 +2309,14 @@ static const uint32_t kSnapMagicSeeds = 0x20000000u;
 static const uint32_t kSnapMagicMazes = 0x00200000u;
 // one with start poses on writes the "W" in lower case ("MwBS", "MwbS", ...) and carries the four start pose arrays
 static const uint32_t kSnapMagicPoses = 0x00002000u;
-static const uint32_t kSnapMagicModes = kSnapMagicSeeds | kSnapMagicMazes | kSnapMagicPoses;
+// one with the state bank on writes the "M" in lower case ("mWBS", "mwbs", ...) and carries the records, bank_level,
+// next_state and episode_state
+static const uint32_t kSnapMagicBank = 0x00000020u;
+static const uint32_t kSnapMagicModes = kSnapMagicSeeds | kSnapMagicMazes | kSnapMagicPoses | kSnapMagicBank;
 
 static uint32_t snapshot_magic(const mwb_handle* h) {
   const uint32_t seeds = (h->S.next_seed ? kSnapMagicSeeds : 0u) | (h->S.layouts ? kSnapMagicMazes : 0u) |
-                         (h->S.poses ? kSnapMagicPoses : 0u);
+                         (h->S.poses ? kSnapMagicPoses : 0u) | (h->S.bank ? kSnapMagicBank : 0u);
   if (h->level_mazes) return (h->S.next_level ? kSnapMagicWorldsLevelChanges : kSnapMagicWorlds) | seeds;
   return (h->S.next_level ? kSnapMagicLevelChanges : kSnapMagic) | seeds;
 }
@@ -2151,7 +2328,8 @@ static std::string snapshot_mode(uint32_t magic) {
                                                 : "level changes on, per-env worlds") +
          (magic & kSnapMagicSeeds ? ", episode seeds on" : ", episode seeds off") +
          (magic & kSnapMagicMazes ? ", maze layouts on" : ", maze layouts off") +
-         (magic & kSnapMagicPoses ? ", start poses on" : ", start poses off");
+         (magic & kSnapMagicPoses ? ", start poses on" : ", start poses off") +
+         (magic & kSnapMagicBank ? ", state bank on" : ", state bank off");
 }
 
 struct SnapHeader {
@@ -2180,7 +2358,8 @@ struct SnapSection {
 
 // The sections of a blob after its header, in blob order: every array that changes while episodes run (entity lists,
 // counters, camera / lighting parameters, RNG streams, pending-reset flags), the geometry currently on the device and
-// the level ranges, then the episode-seed, maze-layout and start-pose arrays of handles with those modes on.  A handle with level
+// the level ranges, then the episode-seed, maze-layout and start-pose arrays and the state bank of handles with those
+// modes on.  A handle with level
 // changes on closes the blob with its level-change section: env_level, next_level, level_draws, level_weights and
 // `tail` (adopted on restore: the assignment is state).  A static table of several levels closes it with the host's
 // env_level (checked on restore, never overwritten).
@@ -2209,6 +2388,11 @@ static std::vector<SnapSection> snapshot_sections(mwb_handle* h, LevelChangeTail
     const StartPoses& P = h->poses_h;
     dev(P.next, N * E * 3 * sizeof(double)); dev(P.next_agent, N * 3 * sizeof(double)); dev(P.pending, N);
     dev(P.episode, N * 3 * sizeof(double));
+  }
+  if (S.bank) {
+    const StateBank& B = h->bank_h;
+    dev(B.records, (size_t)B.slots * B.rec_bytes); dev(B.bank_level, (size_t)B.slots * sizeof(int32_t));
+    dev(B.next_state, N * sizeof(int32_t)); dev(B.episode_state, N * sizeof(int32_t));
   }
   if (S.next_level) {
     SA(env_level, N); SA(next_level, N); SA(level_draws, N); SA(level_weights, S.num_levels);
@@ -2277,6 +2461,8 @@ extern "C" int mwb_restore(mwb_handle* h, const void* blob, size_t bytes) {
                                 snapshot_mode(want.magic) + ")");
   if (hd.N != want.N || hd.E != want.E || hd.R != want.R || hd.Q != want.Q || hd.S != want.S)
     return fail(MWB_EINVAL, "snapshot does not match this handle's configuration");
+  if (h->S.bank && hd.G == want.G && hd.bytes != want.bytes)
+    return fail(MWB_EINVAL, "snapshot of a state bank of another size");
   const bool shared = h->cfg.shared_geometry != 0;
   if (hd.G != want.G || hd.bytes != want.bytes)
     return fail(shared ? MWB_ESTATE : MWB_EINVAL, shared ? "snapshot of a handle with another number of levels"
@@ -2367,6 +2553,8 @@ extern "C" int mwb_state_array(mwb_handle* h, int which, void** dev_ptr, int64_t
   const char* seeds_off = S.next_seed ? nullptr : "episode seeds are off (mwb_enable_episode_seeds)";
   const char* mazes_off = S.layouts ? nullptr : "maze layouts are off (mwb_enable_maze_layouts)";
   const char* poses_off = S.poses ? nullptr : "start poses are off (mwb_enable_start_poses)";
+  const char* bank_off = S.bank ? nullptr : "the state bank is off (mwb_enable_state_bank)";
+  const StateBank& B = h->bank_h;
   const char* params_off = h->have_params && S.ops ? nullptr
                            : "the handle has no device resets (params and a reset program: mwb_set_levels, or "
                              "mwb_set_params and mwb_set_program); host-generated worlds carry their own draws";
@@ -2393,6 +2581,9 @@ extern "C" int mwb_state_array(mwb_handle* h, int which, void** dev_ptr, int64_t
     case MWB_ARRAY_NEXT_AGENT_POSE: p = P.next_agent; n = N * 3; off = poses_off; break;          // float64 [N][3]
     case MWB_ARRAY_POSE_PENDING: p = P.pending; off = poses_off; break;                           // uint8 [N]
     case MWB_ARRAY_EPISODE_START: p = P.episode; n = N * 3; off = poses_off; break;               // float64 [N][3]
+    case MWB_ARRAY_NEXT_STATE: p = B.next_state; off = bank_off; break;                           // int32 [N]
+    case MWB_ARRAY_EPISODE_STATE: p = B.episode_state; off = bank_off; break;                     // int32 [N]
+    case MWB_ARRAY_BANK_LEVEL: p = B.bank_level; n = B.slots; off = bank_off; break;              // int32 [slots]
     case MWB_ARRAY_LEVEL_PARAMS: p = (void*)S.level_params; n = (int64_t)h->levels.size(); off = params_off; break;  // mwb_params [L]
     default: return fail(MWB_EINVAL, "unknown array");
   }

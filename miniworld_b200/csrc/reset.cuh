@@ -13,7 +13,10 @@
 // on (mwb_enable_maze_layouts) a Maze reset can instead build a layout written into next_maze (take_maze, maze_design),
 // with the goal box and the agent in the layout's cells.  With start poses on (mwb_enable_start_poses) a reset can take
 // designed poses for the agent and the placed entities (take_poses, designed_pose), as place_entity(pos=..., dir=...).
+// With the state bank on (mwb_enable_state_bank) a reset with a pending slot can instead load a saved env state
+// (bank_load in bank.cuh) and return before the program runs.
 #pragma once
+#include "bank.cuh"
 #include "maze.cuh"
 #include "physics.cuh"
 
@@ -159,6 +162,8 @@ MWB_DEV_NOINLINE const double* designed_pose(const StartPoses* P, int i, int e, 
 
 MWB_DEV void device_reset(const DevState& S, int i) {
   const size_t N = S.N;
+  // a pending saved state wins over everything else and consumes only next_state (bank.cuh)
+  if (S.bank && bank_load(S.bank, i, S.env_level[i], S.next_level != nullptr)) return;
   if (S.next_seed) take_seed(S, i);
   NpRng rng = load_rng(S, i);
   const int lvl = S.next_level ? resolve_level(S, i) : S.env_level[i];

@@ -41,6 +41,36 @@ struct StartPoses {
   double* episode;              // [N][3] the agent's pose at the start of the env's running episode
 };
 
+// One scalar of an env's state in a state-bank record: env i's copy lives at base + i * env_stride (a per-env row of
+// the structure of arrays, or an element of an [N][k] array), the record's at byte rec_off; bytes is 1, 4 or 8.
+struct BankCol {
+  uint8_t* base;
+  int32_t env_stride;
+  int32_t rec_off;
+  int32_t bytes;
+  int32_t pad_;
+};
+
+// The state bank (mwb_enable_state_bank).  A record is rec_bytes bytes, 16-byte aligned: the BankCol scalars in record
+// order, then, on handles with per-env worlds, the world section at world_off: int32 {rooms, quads, segments in use,
+// 1 = the record holds a world}, then room, quad and segment arrays of the handle's capacities at room_off / quad_off /
+// seg_off.  The geometry addresses are the handle's, which no call can replace once the bank is on.
+struct StateBank {
+  uint8_t* records;             // [slots][rec_bytes]
+  int32_t* bank_level;          // [slots] level of the state a slot holds, -1 = empty
+  int32_t* next_state;          // [N] slot the env's next reset loads, -1 = none
+  int32_t* episode_state;       // [N] slot the running episode was loaded from, -1 = the level's program ran
+  const BankCol* cols;          // [num_cols] in record order
+  int32_t num_cols, slots;
+  int64_t rec_bytes;
+  int32_t world_off, room_off, quad_off, seg_off;   // world_off -1: the handle has no per-env worlds
+  int32_t env_geom, R, Q, S;
+  int32_t *num_rooms, *num_quads, *num_segs;
+  mwb_room* rooms;
+  mwb_quad* quads;
+  mwb_seg* segs;
+};
+
 struct TriRec;
 struct MeshSegInfo;
 struct MazeDev;
@@ -152,6 +182,8 @@ struct DevState {
   const struct MazeLayouts* layouts;
   // start poses (mwb_enable_start_poses); null on a handle without them, one pointer for the same reason
   const struct StartPoses* poses;
+  // state bank (mwb_enable_state_bank); null on a handle without it, one pointer for the same reason
+  const struct StateBank* bank;
   int32_t autoreset;
   // StochasticActionWrapper on the device (reference wrappers.py:49-71): per step one uniform() draw from
   // the env's own stream; below act_prob the chosen action stands, else act_random (< 0: integers(0, 6))

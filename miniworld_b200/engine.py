@@ -135,7 +135,8 @@ EXPORTS = (
     "mwb_snapshot_size", "mwb_snapshot", "mwb_restore", "mwb_set_obs_format",
     "mwb_flag_write", "mwb_flag_wait_geq", "mwb_flag_mode", "mwb_state_array", "mwb_debug_camera", "mwb_set_obs_peer",
     "mwb_set_levels", "mwb_enable_level_changes", "mwb_state_in_host_memory", "mwb_set_level_maze",
-    "mwb_enable_episode_seeds", "mwb_enable_maze_layouts", "mwb_enable_start_poses",
+    "mwb_enable_episode_seeds", "mwb_enable_maze_layouts", "mwb_enable_start_poses", "mwb_enable_state_bank",
+    "mwb_save_states",
 )
 OBS_FORMATS = {"hwc": 0, "cwh": 1, "grey": 2}
 
@@ -177,6 +178,8 @@ def load_library():
     lib.mwb_enable_episode_seeds.argtypes = [vp]
     lib.mwb_enable_maze_layouts.argtypes = [vp]
     lib.mwb_enable_start_poses.argtypes = [vp]
+    lib.mwb_enable_state_bank.argtypes = [vp, C.c_int32]
+    lib.mwb_save_states.argtypes = [vp, vp, vp, C.c_int, vp]
     lib.mwb_state_in_host_memory.argtypes = []
     lib.mwb_seed.argtypes = [vp, vp, C.c_int, vp]
     lib.mwb_reset.argtypes = [vp, vp, C.c_int, vp]
@@ -496,6 +499,19 @@ class Engine:
         (mwb_enable_start_poses); needs device resets."""
         self._check(self.lib.mwb_enable_start_poses(self.h))
 
+    def enable_state_bank(self, slots):
+        """`slots` state records; resets with "next_state" set load a filled one, and every reset records the loaded
+        slot in "episode_state" from now on (mwb_enable_state_bank); needs device resets, after every other mode."""
+        self._check(self.lib.mwb_enable_state_bank(self.h, int(slots)))
+
+    def save_states(self, env_ids, slots, stream=None):
+        """Env env_ids[t] into slot slots[t] (mwb_save_states): int32 numpy arrays (checked) or int32 CUDA tensors
+        (enqueued on `stream`, out-of-range entries skipped on the device)."""
+        if isinstance(env_ids, np.ndarray):
+            env_ids, slots = np.ascontiguousarray(env_ids, np.int32), np.ascontiguousarray(slots, np.int32)
+        self._check(self.lib.mwb_save_states(self.h, _dev_or_host_ptr(env_ids), _dev_or_host_ptr(slots), len(env_ids),
+                                             stream))
+
     # ---- reset
     def seed(self, env_ids, states):
         ids = np.ascontiguousarray(env_ids, np.int32)
@@ -571,7 +587,8 @@ class Engine:
         """uint32[N] (numpy or CUDA tensor): bit e = entity slot e passes the reference's occlusion query."""
         self._check(self.lib.mwb_visible_ents(self.h, _dev_or_host_ptr(mask), stream))
 
-    # name -> (mwb_state_array id, element type, shape): "env" = [N], "ents" = [max_ents, N], "level" = [n_levels],
+    # name -> (mwb_state_array id, element type, shape): "env" = [N], "ents" = [max_ents, N], "level" = [count]
+    # ([n_levels], or [slots] for bank_level),
     # "params" = [n_levels, PARAMS_DOUBLES] (mwb_params records as float64 words), "env_rows" = [N, count / N],
     # "env_slots" = [N, max_ents, 3]
     ARRAYS = {"counter": (0, "<i4", "env"), "step_count": (1, "<i4", "env"), "ent_x": (2, "<f8", "ents"),
@@ -581,7 +598,8 @@ class Engine:
               "next_maze": (18, "|u1", "env_rows"), "next_maze_cells": (19, "<i4", "env_rows"),
               "maze_pending": (20, "|u1", "env"), "episode_maze": (21, "|u1", "env_rows"),
               "next_pose": (22, "<f8", "env_slots"), "next_agent_pose": (23, "<f8", "env_rows"),
-              "pose_pending": (24, "|u1", "env"), "episode_start": (25, "<f8", "env_rows")}
+              "pose_pending": (24, "|u1", "env"), "episode_start": (25, "<f8", "env_rows"),
+              "next_state": (26, "<i4", "env"), "episode_state": (27, "<i4", "env"), "bank_level": (28, "<i4", "level")}
 
     def state_array(self, name, shape=None):
         """Zero-copy view of a state array (mwb_state_array) as an object with __cuda_array_interface__:
@@ -591,7 +609,8 @@ class Engine:
         "next_seed" / "episode_seed" int64 [N]; with maze layouts on, "next_maze" / "episode_maze" uint8
         [N, rows * cols], "next_maze_cells" int32 [N, 2] and "maze_pending" uint8 [N]; with start poses on,
         "next_pose" float64 [N, max_ents, 3], "next_agent_pose" / "episode_start" float64 [N, 3] and "pose_pending"
-        uint8 [N].  `shape` gives the view
+        uint8 [N]; with the state bank on, "next_state" / "episode_state" int32 [N] and "bank_level" int32 [slots].
+        `shape` gives the view
         another shape of the same size (the maze layouts as [N, rows, cols]).  On the host build of the kernels the
         arrays live in host memory, and the view is a numpy array over the same memory instead."""
         which, typestr, axis = self.ARRAYS[name]
