@@ -202,7 +202,8 @@ typedef struct mwb_op {
                              /* PUT: proto, append-only flag                                                    */
   int32_t ireg_a, stride_a;  /* PLACE: proto = a + ireg[ireg_a]*stride_a + ireg[ireg_b]*stride_b */
   int32_t ireg_b, stride_b;  /*        (ireg_* = -1: unused)                                     */
-  int32_t room;              /* PLACE: fixed room index or -1 (sample by area)                   */
+  int32_t room;              /* PLACE: fixed room index or -1 (sample by area).  CHOICE / UNIFORM: the draw's    */
+                             /* index d, 0, 1, ... in program order (mwb_enable_reset_draws)                    */
   int32_t dir_freg;          /* PLACE: freg holding dir, or -1 (draw uniform(-pi, pi))           */
   int32_t is_agent;          /* PLACE: this is place_agent()                                     */
   double f[4];               /* UNIFORM: lo, hi.  PLACE: min_x, max_x, min_z, max_z (NaN = room) */
@@ -453,6 +454,31 @@ int mwb_enable_maze_layouts(mwb_handle* h);
  * compared. */
 int mwb_enable_start_poses(mwb_handle* h);
 
+/* Reset draws (environment design over what an episode contains: object kinds and colours, box sizes, goal sides,
+ * headings).  Valid on a handle with device resets (params and a reset program), before the state bank: MWB_ESTATE
+ * when the handle resets on the host, has the mode on already or has the bank on.  A level's reset draws are the CHOICE
+ * and UNIFORM ops of its program; op.room of each must hold its index d = 0, 1, ... in program order (MWB_EINVAL
+ * otherwise), and D is the largest draw count over the handle's levels at the call (MWB_EINVAL when it is 0).  Three
+ * arrays, read and written in place through mwb_state_array, stream-ordered, without a sync:
+ *   next_draws float64 [N][D]      designed outcome of draw d at the env's next reset (all NaN at the call);
+ *   draws_pending uint8 [N]        nonzero: the rows wait for the env's next reset (all 0 at the call);
+ *   episode_draws float64 [N][D]   outcome of each draw of the env's running episode (all NaN at the call).
+ * At every reset of env i (mwb_reset, and the next-step auto-reset inside mwb_step) that runs a program, at any level,
+ * draws_pending[i] = 0 when it was set, and the rows stay as written.  With it set, each draw d of the level the reset
+ * resolves to (after the level, seed and bank rules) is made from the env's stream as usual, and its result is then
+ * replaced by next_draws[i][d] when that value lies in the draw's support: for a choice over n an integer in [0, n),
+ * for a uniform over [lo, hi] a finite value with lo <= v <= hi.  Otherwise (NaN included) the drawn value stays.  So
+ * the stream advances as without a design, a seed plus a design reproduces an episode, and a design only selects an
+ * outcome the level can produce itself.  Rows beyond the level's draw count are ignored.  Every such reset writes the
+ * outcome of each draw, designed or drawn, into episode_draws[i][d] (choices as exact integers) and NaN beyond the
+ * level's count; after a terminating step it still names the episode that ended.  A designed start pose
+ * (mwb_enable_start_poses) still wins for the position and dir of its placement.  A state-bank load consumes only
+ * next_state: pending draws wait for the next reset that runs a program, and episode_draws is part of the record.
+ * Handles that never call this behave exactly as before it existed, and the addition changes no struct, so
+ * MWB_ABI_VERSION stays as it is.  Snapshots of a handle with the mode on carry the three arrays and are marked as such
+ * in the header; restoring across the mode fails with MWB_ESTATE before anything else is compared. */
+int mwb_enable_reset_draws(mwb_handle* h);
+
 /* State bank (Go-Explore, backplay and demonstration-start curricula, branching rollouts): save env states into device
  * records and start an env's next episode from one.  Valid on a handle with device resets, after the level table, any
  * Maze levels and the other modes are set up: MWB_ESTATE when the handle resets on the host or has the bank on already,
@@ -466,9 +492,9 @@ int mwb_enable_start_poses(mwb_handle* h);
  * A record is everything a running episode is: the entity list (proto, pose, colour, size), num_slots, agent_slot,
  * carrying, step_count, the counter (CollectHealth's health), the camera, sky and light parameters, max_forward_step,
  * the ghost entity, the RNG stream, the env's room texture variants, env_level, the episode_seed / episode_maze /
- * episode_start records of the modes that are on and, when the saved env's level has per-env worlds, its world block
+ * episode_start / episode_draws records of the modes that are on and, when the saved env's level has per-env worlds, its world block
  * (the rooms, quads and segments in use).  Not in a record: needs_reset, the pending inputs (next_level, level_draws,
- * next_seed, the pending layout, cells and poses), next_state, episode_state, episodes_done, the level table and its
+ * next_seed, the pending layout, cells, poses and draws), next_state, episode_state, episodes_done, the level table and its
  * params.
  * At every reset of env i (mwb_reset, and the next-step auto-reset inside mwb_step) with next_state[i] = s >= 0, before
  * anything else, next_state[i] = -1; then, when slot s exists and is filled and its level is the env's level or level
@@ -659,6 +685,10 @@ int mwb_debug_camera(mwb_handle* h, float* out /* host [num_envs][16] */);
 #define MWB_ARRAY_NEXT_STATE 26       /* int32 [num_envs]  slot the env's next reset loads, -1 = none                  */
 #define MWB_ARRAY_EPISODE_STATE 27    /* int32 [num_envs]  slot the running episode was loaded from, -1 = none         */
 #define MWB_ARRAY_BANK_LEVEL 28       /* int32 [slots]  level of the state each slot holds, -1 = empty                 */
+/* with reset draws on (mwb_enable_reset_draws; MWB_ESTATE otherwise); count = elements, D per env: */
+#define MWB_ARRAY_NEXT_DRAWS 29       /* float64 [num_envs][D]  designed outcome of each reset draw, next reset        */
+#define MWB_ARRAY_DRAWS_PENDING 30    /* uint8 [num_envs]  nonzero = the designed draws wait for the next reset        */
+#define MWB_ARRAY_EPISODE_DRAWS 31    /* float64 [num_envs][D]  outcome of each reset draw of the running episode      */
 int mwb_state_array(mwb_handle* h, int which, void** dev_ptr, int64_t* count);
 /* 1 when this library keeps the handle's state arrays (mwb_state_array) in host memory -- the CPU build of the kernels
  * used by the test suite -- and 0 for libmwb.so, whose arrays are device memory. */

@@ -21,6 +21,9 @@ Per-environment semantics are exactly those of the reference's `MiniWorldEnv.res
     (`next_maze`, `set_env_maze`), and `info["maze"]` holds the layout of each running episode;
   * with `start_poses=True`, an env's next reset can place the agent and the entities at poses written into device
     tensors (`next_pose`, `set_env_pose`), and `info["start"]` holds where each running episode's agent started;
+  * with `reset_draws=True`, an env's next reset can take designed outcomes of its level's reset draws (object kinds and
+    colours, box sizes, goal sides, headings) written into a device tensor (`next_draws`, `set_env_draws`), and
+    `info["draws"]` holds the outcome of every draw of each running episode;
   * with `state_bank=K`, envs can be saved into K device-side records (`save_states`) and an env's next reset can load
     one (`next_state`, `set_env_state`), and `info["state"]` names the record each running episode was loaded from.
 
@@ -172,6 +175,8 @@ _NEEDS = {**dict.fromkeys(("env_level", "next_level", "level_weights"), (
               "maze_layouts", RuntimeError, "this batch has no maze layouts: construct it with maze_layouts=True")),
           **dict.fromkeys(("next_pose", "next_agent_pose", "pose_pending", "episode_start"), (
               "start_poses", RuntimeError, "this batch has no start poses: construct it with start_poses=True")),
+          **dict.fromkeys(("next_draws", "draws_pending", "episode_draws"), (
+              "reset_draws", RuntimeError, "this batch has no reset draws: construct it with reset_draws=True")),
           **dict.fromkeys(("next_state", "episode_state", "bank_level"), (
               "state_bank", RuntimeError, "this batch has no state bank: construct it with state_bank=K")),
           "level_params": ("device_reset", TypeError, "level params change at device resets; host-reset levels draw "
@@ -256,6 +261,22 @@ class BatchedMiniWorld:
     agent's (x, z, dir) at the start of every running episode, designed or drawn; after a terminating step they still
     name the episode that just ended.
 
+    `reset_draws=True` (one level or a table; levels that reset on the device, one of them with a draw) decides what
+    episodes contain, for environment design over object composition, goal-side balancing and size curricula.  A level's
+    reset draws are the choices and uniforms its `_gen_world()` makes itself (not those inside place_entity), numbered
+    0, 1, ... in call order; `draw_specs[level]` lists them (index, kind "choice" with n or "uniform" with lo and hi,
+    label): Hallway's heading; TMaze's and YMaze's goal side and heading; PickupObjects' kind (0 Ball, 1 Box, 2 Key) and
+    colour (index into COLOR_NAMES) per object; RoomObjects' Box, Ball and Key colours; PutNext's box size per colour.
+    With `draws_pending[i]` set, env i's next reset at any level, the auto-reset inside `step` included, makes each draw d
+    as usual and then replaces its result with `next_draws[i, d]` when that lies in the draw's support (a choice over n:
+    an integer in [0, n); a uniform over [lo, hi]: finite, lo <= v <= hi), as `reset(options={"draws": {d: v}})` does on
+    the host.  Otherwise (NaN, the rows' initial value, included) the drawn value stays, so the stream position never
+    changes and a seed plus a design reproduces an episode.  The reset clears `draws_pending` and leaves the rows as
+    written; rows beyond the level's draw count are ignored.  `episode_draws` / `info["draws"]` (float64 [N, D], D the
+    largest draw count of the batch's levels) hold every draw's outcome of each running episode, NaN beyond its level's
+    count; after a terminating step they still name the episode that just ended.  A designed start pose still wins for
+    position and dir; a state-bank load leaves pending draws for the next reset that runs a program.
+
     `state_bank=K` (one level or a table; levels that reset on the device) keeps K records of env states on the device,
     for Go-Explore, backplay and branching rollouts: `save_states(env_ids, slots)` copies env env_ids[t] into slot
     slots[t] (entity list, counters, health, camera, lighting, colours, textures, the RNG stream, the level, the mode
@@ -272,7 +293,7 @@ class BatchedMiniWorld:
     def __init__(self, level, num_envs, obs_width=80, obs_height=60, domain_rand=False, autoreset=True,
                  msaa_samples=8, device=0, want_depth=False, level_kwargs=None, obs_format="hwc", env_level=None,
                  dynamic_levels=False, level_seed=0, env_offset=0, per_env_worlds=False, episode_seeds=False,
-                 maze_layouts=False, start_poses=False, state_bank=None):
+                 maze_layouts=False, start_poses=False, state_bank=None, reset_draws=False):
         self.num_envs = int(num_envs)
         self.obs_width, self.obs_height = int(obs_width), int(obs_height)
         self.domain_rand = bool(domain_rand)
@@ -283,6 +304,7 @@ class BatchedMiniWorld:
         self.episode_seeds = bool(episode_seeds)
         self.maze_layouts = bool(maze_layouts)
         self.start_poses = bool(start_poses)
+        self.reset_draws = bool(reset_draws)
         if state_bank is not None and (isinstance(state_bank, bool) or not isinstance(state_bank, (int, np.integer))
                                        or state_bank < 1):
             raise ValueError("state_bank is a number of slots >= 1, got %r" % (state_bank,))
@@ -305,7 +327,8 @@ class BatchedMiniWorld:
         self._init_engine(defs, table, msaa_samples, autoreset)
         self._view_map = _Views(self.engine, self.device, dict(
             dynamic_levels=self.dynamic_levels, episode_seeds=self.episode_seeds, maze_layouts=self.maze_layouts,
-            start_poses=self.start_poses, state_bank=self.state_bank, device_reset=self.device_reset),
+            start_poses=self.start_poses, state_bank=self.state_bank, reset_draws=self.reset_draws,
+            device_reset=self.device_reset),
             getattr(self, "maze_shape", None))
         if self.dynamic_levels:
             self.level_seed, self.env_offset = int(level_seed), int(env_offset)
@@ -323,6 +346,15 @@ class BatchedMiniWorld:
                 raise TypeError("start poses are taken by device resets; host-reset levels place entities in Python "
                                 "(reset(options={\"poses\": ...}) of the level itself)")
             self.engine.enable_start_poses()
+        if self.reset_draws:
+            if not self.device_reset:
+                self.engine.close()
+                raise TypeError("reset draws are taken by device resets; host-reset levels draw in Python "
+                                "(reset(options={\"draws\": ...}) of the level itself)")
+            if not any(self.draw_specs):
+                self.engine.close()
+                raise ValueError("reset_draws needs a level with a reset draw; %s make none" % ", ".join(self.level_ids))
+            self.engine.enable_reset_draws()
         if self.state_bank:
             if not self.device_reset:
                 self.engine.close()
@@ -433,6 +465,8 @@ class BatchedMiniWorld:
         # the entity-list slots each level's reset fills: kind, whether it is the agent, whether it takes a design
         self.level_slots = [[dict(slot=e, kind=k, agent=a, designable=ds) for e, (k, a, ds) in enumerate(d.program.slots)]
                             if d.program is not None else None for d in defs]
+        # the reset draws of each level's program (reset_draws=True): index, kind, n or lo / hi, label
+        self.draw_specs = [[dict(spec) for spec in d.program.draws] if d.program is not None else None for d in defs]
         self.program, self.maze_template = (None, None) if table else (d0.program, d0.maze)
         self.autoreset = bool(autoreset)
         if self.device_reset:
@@ -516,6 +550,10 @@ class BatchedMiniWorld:
                 # the agent's (x, z, dir) at the start of each env's current episode (after a terminating step still
                 # the ended one's)
                 self._info["start"] = self.episode_start
+            if self.reset_draws:
+                # the outcome of every reset draw of each env's current episode (after a terminating step still the
+                # ended one's)
+                self._info["draws"] = self.episode_draws
             if self.state_bank:
                 # the slot each env's current episode was loaded from, -1 for none (after a terminating step still the
                 # ended one's)
@@ -528,7 +566,7 @@ class BatchedMiniWorld:
         return self._view_map
 
     def _write_pending(self, what, ids, arrays):
-        """The part set_env_level / set_env_seed / set_env_maze / set_env_pose / set_env_state share: check the env ids `ids` (1-D
+        """The part set_env_level / set_env_seed / set_env_maze / set_env_pose / set_env_draws / set_env_state share: check the env ids `ids` (1-D
         integers in [0, N)), then write each (array name or view, values) of `arrays` at those envs -- values one per id
         (a numpy array, or a CUDA tensor) or one for all -- an env listed more than once taking its last entry.  On the host build the write is
         numpy's; on the device it is torch ops on the current stream, without a sync."""
@@ -755,6 +793,49 @@ class BatchedMiniWorld:
         else:
             rows = np.stack([np.broadcast_to(c, ids.shape) for c in comps], axis=1)
         self._write_pending("set_env_pose", ids, [(target, rows), ("pose_pending", 1)])
+
+    # ------------------------------------------------------------------ reset draws (reset_draws=True)
+    @property
+    def next_draws(self):
+        """float64 [N, D] view of the designed outcome of each reset draw at each env's next reset with `draws_pending`
+        set; write it in place (stream-ordered, no sync).  A value applies when it lies in the draw's support."""
+        return self._views()["next_draws"]
+
+    @property
+    def draws_pending(self):
+        """uint8 [N] view: nonzero when the designed draws wait for env i's next reset, which clears it."""
+        return self._views()["draws_pending"]
+
+    @property
+    def episode_draws(self):
+        """float64 [N, D] view of the outcome of each reset draw of each env's running episode, NaN beyond its level's
+        draw count."""
+        return self._views()["episode_draws"]
+
+    def set_env_draws(self, env_ids, index, values):
+        """Design draw `index` (an int in [0, D); `draw_specs` numbers each level's draws) of the listed envs' next
+        episodes: `values` is one value for all or one per env (NaN: draw as usual); envs in mid-episode finish it
+        first.  An env listed more than once takes its last entry.  Sets `draws_pending`; rows written earlier stay.
+        Host values are checked to be real numbers; CUDA tensors are written as they are.  The write is numpy's on the
+        host build, torch ops on the current stream without a sync on the device."""
+        view = self._views()["next_draws"]           # a batch without the mode raises before any input check
+        D = view.shape[1]
+        if isinstance(index, bool) or not isinstance(index, (int, np.integer)) or not 0 <= index < D:
+            raise ValueError("index must be an int in [0, %d), got %r" % (D, index))
+        ids = np.atleast_1d(_host(env_ids))
+        if hasattr(values, "is_cuda") and values.is_cuda:
+            torch = self._ensure_torch()
+            vals = values.to(torch.float64)
+            got = tuple(vals.shape)
+        else:
+            vals = np.asarray(_host(values))
+            if not (np.issubdtype(vals.dtype, np.floating) or np.issubdtype(vals.dtype, np.integer)):
+                raise ValueError("set_env_draws: values are real numbers, got %s" % vals.dtype)
+            vals = vals.astype(np.float64)
+            got = vals.shape
+        if got not in ((), ids.shape):
+            raise ValueError("set_env_draws: values are one value or one per env id (%d), got shape %s" % (ids.size, got))
+        self._write_pending("set_env_draws", ids, [(view[:, int(index)], vals), ("draws_pending", 1)])
 
     # ------------------------------------------------------------------ state bank (state_bank=K)
     @property
@@ -1064,9 +1145,10 @@ class BatchedMiniWorld:
     def _torch_writes(self):
         """True when torch work may write arrays the kernels read: next_level / level_weights (level changes on),
         next_seed (episode seeds on), the pending maze layouts (maze layouts on), the designed start poses (start poses
-        on), the pending slots (state bank on) or the params table (once set_level_param has written it)."""
+        on), the designed draws (reset draws on), the pending slots (state bank on) or the params table (once
+        set_level_param has written it)."""
         return ((self.dynamic_levels or self.episode_seeds or self.maze_layouts or self.start_poses
-                 or self.state_bank or self._params_written)
+                 or self.reset_draws or self.state_bank or self._params_written)
                 and not self.engine.host_memory)
 
     def _level_stream(self):

@@ -123,6 +123,7 @@ struct mwb_handle {
   std::vector<MazeDev> mazes_h;       // host copies of S.maze / S.maze_cdf, one entry per level
   MazeLayouts layouts_h;              // host copy of *S.layouts (mwb_enable_maze_layouts)
   StartPoses poses_h;                 // host copy of *S.poses (mwb_enable_start_poses)
+  ResetDraws draws_h;                 // host copy of *S.draws (mwb_enable_reset_draws)
   StateBank bank_h;                   // host copy of *S.bank (mwb_enable_state_bank)
   int32_t* d_bank_pairs;              // [2][slots] staging of a host mwb_save_states call (env ids, then slots)
   int32_t* d_bank_winner;             // [slots] per-call scratch: the last entry of each slot
@@ -1576,6 +1577,46 @@ extern "C" int mwb_enable_start_poses(mwb_handle* h) {
   return MWB_OK;
 }
 
+extern "C" int mwb_enable_reset_draws(mwb_handle* h) {
+  if (!h) return fail(MWB_EINVAL, "null handle");
+  if (h->S.draws) return fail(MWB_ESTATE, "reset draws are already on");
+  if (h->S.bank) return fail(MWB_ESTATE, "reset draws cannot be turned on once the state bank is on (its record layout depends on it)");
+  if (!h->have_params || !h->S.ops)
+    return fail(MWB_ESTATE, "reset draws need device resets (params and a reset program: mwb_set_levels, or "
+                            "mwb_set_params and mwb_set_program); host-generated worlds draw on the host");
+  // D: the largest draw count over the levels, whose draws must be numbered 0, 1, ... in program order
+  int D = 0;
+  for (size_t l = 0; l < h->levels.size(); ++l) {
+    int count = 0;
+    for (int k = 0; k < h->levels[l].num_ops; ++k) {
+      const mwb_op& op = h->ops_h[(size_t)h->levels[l].op_first + k];
+      if (op.op != MWB_OP_CHOICE && op.op != MWB_OP_UNIFORM) continue;
+      if (op.room != count++)
+        return fail(MWB_EINVAL, "the CHOICE / UNIFORM ops of level " + std::to_string(l) +
+                                    " must hold their draw index 0, 1, ... in program order in `room`");
+    }
+    D = std::max(D, count);
+  }
+  if (D == 0) return fail(MWB_EINVAL, "no level of this handle makes a reset draw (CHOICE / UNIFORM op)");
+  const size_t N = h->S.N;
+  void *next, *pending, *episode;
+  // NaN rows (0xFF bytes): no design until one is written, and no outcome before the first reset
+  int rc = alloc_control_arrays(h, "reset draw", {{&next, N * D * sizeof(double), true}, {&pending, N, false},
+                                                  {&episode, N * D * sizeof(double), true}});
+  if (rc) return rc;
+  ResetDraws& R = h->draws_h;
+  R.next = (double*)next;
+  R.pending = (uint8_t*)pending;
+  R.episode = (double*)episode;
+  R.D = D;
+  R.pad_ = 0;
+  ResetDraws* d = nullptr;
+  if (alloc_arr(h, &d, 1)) return fail(MWB_ECUDA, "reset draw state allocation failed");
+  if (h2d(d, &R, sizeof(R), h->stream) != 0 || sync_stream(h->stream) != 0) return fail(MWB_ECUDA, "upload failed");
+  h->S.draws = d;
+  return MWB_OK;
+}
+
 // The record layout of the handle as it stands (StateBank in state.h): the scalars of one env, widest first so that
 // each lands aligned, then the world section on handles with per-env worlds.
 static void bank_layout(const mwb_handle* h, std::vector<BankCol>& cols, StateBank& B) {
@@ -1602,6 +1643,7 @@ static void bank_layout(const mwb_handle* h, std::vector<BankCol>& cols, StateBa
   add(S.rng_s_hi, 8, 1, false); add(S.rng_s_lo, 8, 1, false); add(S.rng_inc_hi, 8, 1, false); add(S.rng_inc_lo, 8, 1, false);
   if (S.next_seed) add(S.episode_seed, 8, 1, false);
   if (S.poses) add(h->poses_h.episode, 8, 3, true);
+  if (S.draws) add(h->draws_h.episode, 8, h->draws_h.D, true);
   add(S.ent_proto, 4, E, false);
   add(S.num_slots, 4, 1, false); add(S.agent_slot, 4, 1, false); add(S.carrying, 4, 1, false);
   add(S.step_count, 4, 1, false); add(S.num_picked, 4, 1, false); add(S.ghost_slot, 4, 1, false);
@@ -2312,11 +2354,15 @@ static const uint32_t kSnapMagicPoses = 0x00002000u;
 // one with the state bank on writes the "M" in lower case ("mWBS", "mwbs", ...) and carries the records, bank_level,
 // next_state and episode_state
 static const uint32_t kSnapMagicBank = 0x00000020u;
-static const uint32_t kSnapMagicModes = kSnapMagicSeeds | kSnapMagicMazes | kSnapMagicPoses | kSnapMagicBank;
+// one with reset draws on sets the high bit of the mode letter (every letter's case bit already names a mode) and
+// carries next_draws, draws_pending and episode_draws
+static const uint32_t kSnapMagicDraws = 0x80000000u;
+static const uint32_t kSnapMagicModes = kSnapMagicSeeds | kSnapMagicMazes | kSnapMagicPoses | kSnapMagicBank | kSnapMagicDraws;
 
 static uint32_t snapshot_magic(const mwb_handle* h) {
   const uint32_t seeds = (h->S.next_seed ? kSnapMagicSeeds : 0u) | (h->S.layouts ? kSnapMagicMazes : 0u) |
-                         (h->S.poses ? kSnapMagicPoses : 0u) | (h->S.bank ? kSnapMagicBank : 0u);
+                         (h->S.poses ? kSnapMagicPoses : 0u) | (h->S.bank ? kSnapMagicBank : 0u) |
+                         (h->S.draws ? kSnapMagicDraws : 0u);
   if (h->level_mazes) return (h->S.next_level ? kSnapMagicWorldsLevelChanges : kSnapMagicWorlds) | seeds;
   return (h->S.next_level ? kSnapMagicLevelChanges : kSnapMagic) | seeds;
 }
@@ -2329,7 +2375,8 @@ static std::string snapshot_mode(uint32_t magic) {
          (magic & kSnapMagicSeeds ? ", episode seeds on" : ", episode seeds off") +
          (magic & kSnapMagicMazes ? ", maze layouts on" : ", maze layouts off") +
          (magic & kSnapMagicPoses ? ", start poses on" : ", start poses off") +
-         (magic & kSnapMagicBank ? ", state bank on" : ", state bank off");
+         (magic & kSnapMagicBank ? ", state bank on" : ", state bank off") +
+         (magic & kSnapMagicDraws ? ", reset draws on" : ", reset draws off");
 }
 
 struct SnapHeader {
@@ -2358,7 +2405,7 @@ struct SnapSection {
 
 // The sections of a blob after its header, in blob order: every array that changes while episodes run (entity lists,
 // counters, camera / lighting parameters, RNG streams, pending-reset flags), the geometry currently on the device and
-// the level ranges, then the episode-seed, maze-layout and start-pose arrays and the state bank of handles with those
+// the level ranges, then the episode-seed, maze-layout, start-pose and reset-draw arrays and the state bank of handles with those
 // modes on.  A handle with level
 // changes on closes the blob with its level-change section: env_level, next_level, level_draws, level_weights and
 // `tail` (adopted on restore: the assignment is state).  A static table of several levels closes it with the host's
@@ -2388,6 +2435,10 @@ static std::vector<SnapSection> snapshot_sections(mwb_handle* h, LevelChangeTail
     const StartPoses& P = h->poses_h;
     dev(P.next, N * E * 3 * sizeof(double)); dev(P.next_agent, N * 3 * sizeof(double)); dev(P.pending, N);
     dev(P.episode, N * 3 * sizeof(double));
+  }
+  if (S.draws) {
+    const ResetDraws& R = h->draws_h;
+    dev(R.next, N * R.D * sizeof(double)); dev(R.pending, N); dev(R.episode, N * R.D * sizeof(double));
   }
   if (S.bank) {
     const StateBank& B = h->bank_h;
@@ -2554,6 +2605,8 @@ extern "C" int mwb_state_array(mwb_handle* h, int which, void** dev_ptr, int64_t
   const char* mazes_off = S.layouts ? nullptr : "maze layouts are off (mwb_enable_maze_layouts)";
   const char* poses_off = S.poses ? nullptr : "start poses are off (mwb_enable_start_poses)";
   const char* bank_off = S.bank ? nullptr : "the state bank is off (mwb_enable_state_bank)";
+  const char* draws_off = S.draws ? nullptr : "reset draws are off (mwb_enable_reset_draws)";
+  const ResetDraws& Dr = h->draws_h;
   const StateBank& B = h->bank_h;
   const char* params_off = h->have_params && S.ops ? nullptr
                            : "the handle has no device resets (params and a reset program: mwb_set_levels, or "
@@ -2584,6 +2637,9 @@ extern "C" int mwb_state_array(mwb_handle* h, int which, void** dev_ptr, int64_t
     case MWB_ARRAY_NEXT_STATE: p = B.next_state; off = bank_off; break;                           // int32 [N]
     case MWB_ARRAY_EPISODE_STATE: p = B.episode_state; off = bank_off; break;                     // int32 [N]
     case MWB_ARRAY_BANK_LEVEL: p = B.bank_level; n = B.slots; off = bank_off; break;              // int32 [slots]
+    case MWB_ARRAY_NEXT_DRAWS: p = Dr.next; n = N * Dr.D; off = draws_off; break;                 // float64 [N][D]
+    case MWB_ARRAY_DRAWS_PENDING: p = Dr.pending; off = draws_off; break;                         // uint8 [N]
+    case MWB_ARRAY_EPISODE_DRAWS: p = Dr.episode; n = N * Dr.D; off = draws_off; break;           // float64 [N][D]
     case MWB_ARRAY_LEVEL_PARAMS: p = (void*)S.level_params; n = (int64_t)h->levels.size(); off = params_off; break;  // mwb_params [L]
     default: return fail(MWB_EINVAL, "unknown array");
   }

@@ -13,7 +13,8 @@
 // on (mwb_enable_maze_layouts) a Maze reset can instead build a layout written into next_maze (take_maze, maze_design),
 // with the goal box and the agent in the layout's cells.  With start poses on (mwb_enable_start_poses) a reset can take
 // designed poses for the agent and the placed entities (take_poses, designed_pose), as place_entity(pos=..., dir=...).
-// With the state bank on (mwb_enable_state_bank) a reset with a pending slot can instead load a saved env state
+// With reset draws on (mwb_enable_reset_draws) a reset can replace the outcomes of its CHOICE / UNIFORM ops with
+// designed ones inside their support, and records every outcome (take_draws, designed_draw).  With the state bank on (mwb_enable_state_bank) a reset with a pending slot can instead load a saved env state
 // (bank_load in bank.cuh) and return before the program runs.
 #pragma once
 #include "bank.cuh"
@@ -160,11 +161,45 @@ MWB_DEV_NOINLINE const double* designed_pose(const StartPoses* P, int i, int e, 
   return isfinite(r[0]) && isfinite(r[1]) ? r : nullptr;
 }
 
+// Whether env i's reset takes the designed draws (mwb_enable_reset_draws; include/mwb.h states the rule): as take_poses,
+// and the env's episode_draws row is refilled with NaN, which the level's draws then overwrite.  Out of line, like
+// designed_draw, and given the record's address rather than its fields, so that handles without the mode keep their
+// registers.
+MWB_DEV_NOINLINE bool take_draws(const ResetDraws* R, int i) {
+  MWB_WARP_SYNC();
+  const bool take = R->pending[i] != 0;
+  MWB_WARP_SYNC();
+  if (take) R->pending[i] = 0;
+  for (int d = 0; d < R->D; ++d) R->episode[(size_t)i * R->D + d] = MWB_NAN;
+  MWB_WARP_SYNC();
+  return take;
+}
+
+// The outcome of reset draw `op` (a CHOICE or UNIFORM, op->room = its index d) of env i, which the stream drew as v:
+// with take set, next[i][d] when it lies in the draw's support (a choice over n: an integer in [0, n); a uniform over
+// [lo, hi]: finite and lo <= x <= hi), else v.  The outcome is recorded in episode[i][d].  Out of line, like
+// designed_pose, so that handles without the mode keep their registers.
+MWB_DEV_NOINLINE double designed_draw(const ResetDraws* R, int i, const mwb_op* op, double v, int take) {
+  const int d = op->room;
+  if (d < 0 || d >= R->D) return v;
+  if (take) {
+    const double x = R->next[(size_t)i * R->D + d];
+    if (op->op == MWB_OP_CHOICE ? x >= 0.0 && x < (double)op->b && x == floor(x)
+                                : isfinite(x) && x >= op->f[0] && x <= op->f[1])
+      v = op->op == MWB_OP_CHOICE ? (double)(int)x : x;
+  }
+  R->episode[(size_t)i * R->D + d] = v;
+  return v;
+}
+
 MWB_DEV void device_reset(const DevState& S, int i) {
   const size_t N = S.N;
   // a pending saved state wins over everything else and consumes only next_state (bank.cuh)
   if (S.bank && bank_load(S.bank, i, S.env_level[i], S.next_level != nullptr)) return;
   if (S.next_seed) take_seed(S, i);
+  // bit 4 of flags below: this reset takes designed draws (taken before anything below is loaded: a call while those
+  // values are live costs reset_kernel registers)
+  const int draw_flag = S.draws && take_draws(S.draws, i) ? 16 : 0;
   NpRng rng = load_rng(S, i);
   const int lvl = S.next_level ? resolve_level(S, i) : S.env_level[i];
   // the resolved level decides everything below, its domain_rand included: a reset that switches levels draws by the
@@ -179,10 +214,10 @@ MWB_DEV void device_reset(const DevState& S, int i) {
   const mwb_room* rooms = S.rooms + (size_t)g * S.R;
   int n_rooms = S.num_rooms[g];
   // bit 0: the rooms' textures are drawn (_gen_static_data ran); bits 1 / 2: a designed maze's goal / agent cell is
-  // still to be placed; bit 3: this reset takes designed start poses (one variable, so that the designed paths add no
-  // register to the loop below)
-  int flags = 0;
-  if (S.poses && take_poses(S.poses->pending + i)) flags = 8;
+  // still to be placed; bit 3: this reset takes designed start poses; bit 4: it takes designed draws (one variable, so
+  // that the designed paths add no register to the loop below)
+  int flags = draw_flag;
+  if (S.poses && take_poses(S.poses->pending + i)) flags |= 8;
   if (S.layouts) {
     const MazeLayouts& Y = *S.layouts;
     const size_t cells = (size_t)Y.rows * Y.cols;
@@ -269,9 +304,14 @@ MWB_DEV void device_reset(const DevState& S, int i) {
       continue;
     }
     if (op.op == MWB_OP_CHOICE) {
-      ireg[op.a & 7] = (int)rng_integers(rng, (uint32_t)op.b);
+      // a designed draw is drawn first, so that the stream advances as it would without the design
+      int v = (int)rng_integers(rng, (uint32_t)op.b);
+      if (S.draws) v = (int)designed_draw(S.draws, i, &op, (double)v, flags & 16);
+      ireg[op.a & 7] = v;
     } else if (op.op == MWB_OP_UNIFORM) {
-      freg[op.a & 7] = rng_uniform(rng, op.f[0], d_sub(op.f[1], op.f[0]));
+      double v = rng_uniform(rng, op.f[0], d_sub(op.f[1], op.f[0]));
+      if (S.draws) v = designed_draw(S.draws, i, &op, v, flags & 16);
+      freg[op.a & 7] = v;
     } else if (op.op == MWB_OP_PLACE) {
       if (!(flags & 1)) {
         draw_room_textures(S, i, rooms, n_rooms, L.domain_rand != 0, rng);

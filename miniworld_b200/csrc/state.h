@@ -41,6 +41,15 @@ struct StartPoses {
   double* episode;              // [N][3] the agent's pose at the start of the env's running episode
 };
 
+// The reset draw arrays (mwb_enable_reset_draws).  A level's reset draws are the CHOICE and UNIFORM ops of its program,
+// op.room holding draw d's index; D is the largest draw count over the handle's levels.
+struct ResetDraws {
+  double* next;                 // [N][D] designed outcome of draw d at the env's next reset (NaN: draw as usual)
+  uint8_t* pending;             // [N] 1 = the rows wait for the env's next reset
+  double* episode;              // [N][D] outcome of each draw of the env's running episode, NaN beyond the level's count
+  int32_t D, pad_;
+};
+
 // One scalar of an env's state in a state-bank record: env i's copy lives at base + i * env_stride (a per-env row of
 // the structure of arrays, or an element of an [N][k] array), the record's at byte rec_off; bytes is 1, 4 or 8.
 struct BankCol {
@@ -182,6 +191,8 @@ struct DevState {
   const struct MazeLayouts* layouts;
   // start poses (mwb_enable_start_poses); null on a handle without them, one pointer for the same reason
   const struct StartPoses* poses;
+  // reset draws (mwb_enable_reset_draws); null on a handle without them, one pointer for the same reason
+  const struct ResetDraws* draws;
   // state bank (mwb_enable_state_bank); null on a handle without it, one pointer for the same reason
   const struct StateBank* bank;
   int32_t autoreset;

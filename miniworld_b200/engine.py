@@ -136,7 +136,7 @@ EXPORTS = (
     "mwb_flag_write", "mwb_flag_wait_geq", "mwb_flag_mode", "mwb_state_array", "mwb_debug_camera", "mwb_set_obs_peer",
     "mwb_set_levels", "mwb_enable_level_changes", "mwb_state_in_host_memory", "mwb_set_level_maze",
     "mwb_enable_episode_seeds", "mwb_enable_maze_layouts", "mwb_enable_start_poses", "mwb_enable_state_bank",
-    "mwb_save_states",
+    "mwb_save_states", "mwb_enable_reset_draws",
 )
 OBS_FORMATS = {"hwc": 0, "cwh": 1, "grey": 2}
 
@@ -179,6 +179,7 @@ def load_library():
     lib.mwb_enable_maze_layouts.argtypes = [vp]
     lib.mwb_enable_start_poses.argtypes = [vp]
     lib.mwb_enable_state_bank.argtypes = [vp, C.c_int32]
+    lib.mwb_enable_reset_draws.argtypes = [vp]
     lib.mwb_save_states.argtypes = [vp, vp, vp, C.c_int, vp]
     lib.mwb_state_in_host_memory.argtypes = []
     lib.mwb_seed.argtypes = [vp, vp, C.c_int, vp]
@@ -499,6 +500,12 @@ class Engine:
         (mwb_enable_start_poses); needs device resets."""
         self._check(self.lib.mwb_enable_start_poses(self.h))
 
+    def enable_reset_draws(self):
+        """Resets with "draws_pending" set replace the outcomes of their level's reset draws with the in-support values
+        of "next_draws", and every reset records its outcomes in "episode_draws" from now on (mwb_enable_reset_draws);
+        needs device resets and a level with a draw, before the state bank."""
+        self._check(self.lib.mwb_enable_reset_draws(self.h))
+
     def enable_state_bank(self, slots):
         """`slots` state records; resets with "next_state" set load a filled one, and every reset records the loaded
         slot in "episode_state" from now on (mwb_enable_state_bank); needs device resets, after every other mode."""
@@ -599,7 +606,9 @@ class Engine:
               "maze_pending": (20, "|u1", "env"), "episode_maze": (21, "|u1", "env_rows"),
               "next_pose": (22, "<f8", "env_slots"), "next_agent_pose": (23, "<f8", "env_rows"),
               "pose_pending": (24, "|u1", "env"), "episode_start": (25, "<f8", "env_rows"),
-              "next_state": (26, "<i4", "env"), "episode_state": (27, "<i4", "env"), "bank_level": (28, "<i4", "level")}
+              "next_state": (26, "<i4", "env"), "episode_state": (27, "<i4", "env"), "bank_level": (28, "<i4", "level"),
+              "next_draws": (29, "<f8", "env_rows"), "draws_pending": (30, "|u1", "env"),
+              "episode_draws": (31, "<f8", "env_rows")}
 
     def state_array(self, name, shape=None):
         """Zero-copy view of a state array (mwb_state_array) as an object with __cuda_array_interface__:
@@ -609,7 +618,8 @@ class Engine:
         "next_seed" / "episode_seed" int64 [N]; with maze layouts on, "next_maze" / "episode_maze" uint8
         [N, rows * cols], "next_maze_cells" int32 [N, 2] and "maze_pending" uint8 [N]; with start poses on,
         "next_pose" float64 [N, max_ents, 3], "next_agent_pose" / "episode_start" float64 [N, 3] and "pose_pending"
-        uint8 [N]; with the state bank on, "next_state" / "episode_state" int32 [N] and "bank_level" int32 [slots].
+        uint8 [N]; with the state bank on, "next_state" / "episode_state" int32 [N] and "bank_level" int32 [slots];
+        with reset draws on, "next_draws" / "episode_draws" float64 [N, D] and "draws_pending" uint8 [N].
         `shape` gives the view
         another shape of the same size (the maze layouts as [N, rows, cols]).  On the host build of the kernels the
         arrays live in host memory, and the view is a numpy array over the same memory instead."""

@@ -27,5 +27,5 @@ class Hallway(GoalBoxRule, MiniWorldEnv, utils.EzPickle):
     def device_program(self, prog):
         room = self.rooms[0]
         prog.place(prog.proto(Box(color="red")), min_x=room.max_x - 2)
-        heading = prog.uniform(-math.pi / 4, math.pi / 4)
+        heading = prog.uniform(-math.pi / 4, math.pi / 4, label="agent heading")
         prog.place_agent(dir=heading, max_x=room.max_x - 2)

@@ -42,7 +42,7 @@ class Maze(GoalBoxRule, MiniWorldEnv, utils.EzPickle):
             remaining = [(0, 1), (0, -1), (-1, 0), (1, 0)]
             order = []
             while len(order) < 4:                      # shuffle by repeated choice (4 draws)
-                pick = remaining[self.np_random.choice(len(remaining))]
+                pick = remaining[self._stream().choice(len(remaining))]   # a carve draw, not a reset draw
                 remaining.remove(pick)
                 order.append(pick)
             for dj, di in order:

@@ -37,9 +37,9 @@ class PickupObjects(MiniWorldEnv, utils.EzPickle):
     def device_program(self, prog):
         ncol = len(COLOR_NAMES)
         table = prog.proto_table([[self._make(k, c) for c in COLOR_NAMES] for k in range(3)])
-        for _ in range(self.num_objs):
-            kind = prog.choice(3)
-            color = prog.choice(ncol)
+        for k in range(self.num_objs):
+            kind = prog.choice(3, label="kind of object %d (0 Ball, 1 Box, 2 Key)" % k)
+            color = prog.choice(ncol, label="colour of object %d (index into COLOR_NAMES)" % k)
             prog.place(table, index=(kind, color))
         prog.place_agent()
 

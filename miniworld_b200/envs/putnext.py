@@ -27,7 +27,7 @@ class PutNext(MiniWorldEnv, utils.EzPickle):
 
     def device_program(self, prog):
         for color in COLOR_NAMES:
-            size = prog.uniform(0.6, 0.85)                    # drawn while the Box is constructed
+            size = prog.uniform(0.6, 0.85, label="size of the %s box" % color)   # drawn while the Box is constructed
             prog.place(prog.proto(Box(color=color, size=0.8)), size=size)
         prog.place_agent()
 

@@ -28,8 +28,10 @@ class RoomObjects(MiniWorldEnv, utils.EzPickle):
 
     def device_program(self, prog):
         prog.set_agent(self.agent)                           # radius 1.5
-        for make in (lambda c: Box(color=c, size=0.9), lambda c: Ball(color=c, size=0.9), lambda c: Key(color=c)):
-            colour = prog.choice(len(COLOR_NAMES))           # drawn while the entity is constructed, before place_entity
+        for name, make in (("Box", lambda c: Box(color=c, size=0.9)), ("Ball", lambda c: Ball(color=c, size=0.9)),
+                           ("Key", lambda c: Key(color=c))):
+            # drawn while the entity is constructed, before place_entity
+            colour = prog.choice(len(COLOR_NAMES), label="colour of the %s (index into COLOR_NAMES)" % name)
             prog.place(prog.proto_row([make(c) for c in COLOR_NAMES]), index=colour)
         prog.place_agent()
 

@@ -39,10 +39,10 @@ class TMaze(MiniWorldEnv, utils.EzPickle):
             gx, _, gz = self.goal_pos
             prog.place(box, min_x=gx, max_x=gx, min_z=gz, max_z=gz)
         else:
-            side = prog.choice(2)
+            side = prog.choice(2, label="goal side (0: -z arm, 1: +z arm)")
             prog.place(box, room=1, max_z=bar.min_z + 2, when=(side, 0))
             prog.place(box, room=1, min_z=bar.max_z - 2, when=(side, 1), same_slot=True)
-        heading = prog.uniform(-math.pi / 4, math.pi / 4)
+        heading = prog.uniform(-math.pi / 4, math.pi / 4, label="agent heading")
         prog.place_agent(dir=heading, room=0)
 
     def step(self, action):

@@ -31,6 +31,7 @@ class ResetProgram:
         self.protos = []
         self.proto_kinds = []          # class name of each prototype's entity
         self.slots = []                # (kind, is_agent, takes a designed pose) of each entity-list slot the reset fills
+        self.draws = []                # spec of each reset draw (CHOICE / UNIFORM op), in program order
         self._ireg = 0
         self._freg = 0
         self.agent_proto = self.proto(Agent())
@@ -83,19 +84,25 @@ class ResetProgram:
         self.uses_maze = True
 
     # ---- random draws
-    def choice(self, n):
+    def _draw(self, op, spec, label):
+        """Number reset draw `op` (its index in `room`, mwb_enable_reset_draws) and keep its spec."""
+        op["room"] = len(self.draws)
+        self.draws.append(dict(index=len(self.draws), **spec, label=label))
+        self.ops.append(op)
+
+    def choice(self, n, label=None):
         op = np.zeros((), OP_DTYPE)
         op["op"], op["a"], op["b"] = OP_CHOICE, self._ireg, int(n)
-        self.ops.append(op)
+        self._draw(op, dict(kind="choice", n=int(n)), label)
         self._ireg += 1
         assert self._ireg <= 8
         return _Reg(self._ireg - 1)
 
-    def uniform(self, lo, hi):
+    def uniform(self, lo, hi, label=None):
         op = np.zeros((), OP_DTYPE)
         op["op"], op["a"] = OP_UNIFORM, self._freg
         op["f"][:2] = (float(lo), float(hi))
-        self.ops.append(op)
+        self._draw(op, dict(kind="uniform", lo=float(lo), hi=float(hi)), label)
         self._freg += 1
         assert self._freg <= 8
         return _Reg(self._freg - 1)

@@ -164,6 +164,46 @@ class Room:
         self.wall_uvm = np.concatenate(uvm) if uvm else np.zeros((0, 2))
 
 
+class _DesignedDraws:
+    """`np_random` while `_gen_world()` runs with designed reset draws (reset(options={"draws": {d: v}})): the draws the
+    level makes itself -- choice(n), integers(low, high) and uniform(lo, hi) of one value, numbered 0, 1, ... in call
+    order -- are made from the stream as usual, then draw d's result is replaced by design[d] when that lies in the
+    draw's support (an integer in [low, high); a finite value in [lo, hi]).  `drawn` records every outcome.  Placement,
+    texture and carve draws go to the stream itself (MiniWorldEnv._stream)."""
+
+    def __init__(self, stream, design):
+        self.stream, self.design, self.drawn = stream, design, []
+
+    def __getattr__(self, name):
+        return getattr(self.stream, name)
+
+    def _take(self, v, ok):
+        x = self.design.get(len(self.drawn))
+        x = float(x) if x is not None else math.nan
+        if ok(x):
+            v = type(v)(x)
+        self.drawn.append(float(v))
+        return v
+
+    def _integer(self, v, low, high):
+        return self._take(v, lambda x: low <= x < high and x == math.floor(x))
+
+    def choice(self, a, *args, **kw):
+        v = self.stream.choice(a, *args, **kw)
+        return self._integer(v, 0, int(a)) if isinstance(a, (int, np.integer)) and not args and not kw else v
+
+    def integers(self, low, high=None, *args, **kw):
+        v = self.stream.integers(low, high, *args, **kw)
+        lo, hi = (0, low) if high is None else (low, high)
+        return self._integer(v, lo, hi) if np.ndim(v) == 0 else v
+
+    def uniform(self, low=0.0, high=1.0, *args, **kw):
+        v = self.stream.uniform(low, high, *args, **kw)
+        if np.ndim(v) or np.ndim(low) or np.ndim(high):
+            return v
+        return self._take(v, lambda x: math.isfinite(x) and low <= x <= high)
+
+
 class MiniWorldEnv(gym.Env):
     """Single-environment MiniWorld with the reference's Gymnasium API, executed on the GPU."""
 
@@ -206,7 +246,10 @@ class MiniWorldEnv(gym.Env):
     def reset(self, *, seed=None, options=None):
         """New episode: regenerate the world (host), push it to the engine, render.  `options` may hold designed start
         poses: "poses" {slot: (x, z, dir)} for the place_entity calls that fill those entity-list slots and
-        "agent_pose" (x, z, dir) for place_agent (see place_entity); Maze levels also read a designed layout."""
+        "agent_pose" (x, z, dir) for place_agent (see place_entity); Maze levels also read a designed layout.  "draws"
+        {d: v} designs the level's reset draws, the choice / integers / uniform calls _gen_world() makes itself, numbered
+        0, 1, ... in call order: each is made as usual, then replaced by v when v lies in its support (_DesignedDraws);
+        `episode_draws` then lists every outcome.  Placement and texture draws are not reset draws."""
         super().reset(seed=seed)
         self.step_count = 0
         self.agent = Agent()
@@ -215,7 +258,15 @@ class MiniWorldEnv(gym.Env):
         self.wall_segs = []
         self.reset_options = options        # what the level's _gen_world may read (Maze: a designed layout)
         self._start_design = options if options and ("poses" in options or "agent_pose" in options) else None
-        self._gen_world()
+        if options and "draws" in options:
+            self._np_random = _DesignedDraws(self.np_random, dict(options["draws"]))
+            try:
+                self._gen_world()
+            finally:
+                self.episode_draws = self._np_random.drawn
+                self._np_random = self._np_random.stream
+        else:
+            self._gen_world()
         self._start_design = None           # placements after the reset (CollectHealth's respawns) run as written
 
         rand = self.np_random if self.domain_rand else None
@@ -312,28 +363,34 @@ class MiniWorldEnv(gym.Env):
             x, z, d = design
             pos = np.array([x, 0.0 if pos is None else float(pos[1]), z])
             dir = d if math.isfinite(d) else dir
+        rng = self._stream()
         if pos is not None:
-            ent.dir = dir if dir is not None else self.np_random.uniform(-math.pi, math.pi)
+            ent.dir = dir if dir is not None else rng.uniform(-math.pi, math.pi)
             ent.pos = pos
             self.entities.append(ent)
             return ent
         while True:
-            r = room if room else list(self.rooms)[self.np_random.choice(len(list(self.rooms)), p=self.room_probs)]
+            r = room if room else list(self.rooms)[rng.choice(len(list(self.rooms)), p=self.room_probs)]
             lx = r.min_x if min_x is None else min_x
             hx = r.max_x if max_x is None else max_x
             lz = r.min_z if min_z is None else min_z
             hz = r.max_z if max_z is None else max_z
-            pos = self.np_random.uniform(low=[lx - ent.radius, 0, lz - ent.radius],
-                                         high=[hx + ent.radius, 0, hz + ent.radius])
+            pos = rng.uniform(low=[lx - ent.radius, 0, lz - ent.radius], high=[hx + ent.radius, 0, hz + ent.radius])
             if not r.point_inside(pos):
                 continue
             if self.intersect(ent, pos, ent.radius):
                 continue
             ent.pos = pos
-            ent.dir = dir if dir is not None else self.np_random.uniform(-math.pi, math.pi)
+            ent.dir = dir if dir is not None else rng.uniform(-math.pi, math.pi)
             break
         self.entities.append(ent)
         return ent
+
+    def _stream(self):
+        """The env's numpy stream itself, for draws that are not reset draws (placement, textures, maze carving), also
+        while a reset with designed draws runs."""
+        rng = self.np_random
+        return rng.stream if isinstance(rng, _DesignedDraws) else rng
 
     def _designed_pose(self, ent):
         """(x, z, dir) of the designed start pose that applies to placing `ent` now, or None."""
@@ -381,7 +438,7 @@ class MiniWorldEnv(gym.Env):
 
     def _gen_static_data(self):
         for room in self.rooms:
-            room._gen_static_data(self.params, self.np_random if self.domain_rand else None)
+            room._gen_static_data(self.params, self._stream() if self.domain_rand else None)
         self.wall_segs = np.concatenate([r.wall_segs for r in self.rooms])
         self.room_probs = np.array([r.area for r in self.rooms], dtype=float)
         self.room_probs /= np.sum(self.room_probs)
