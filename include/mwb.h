@@ -514,6 +514,48 @@ int mwb_enable_state_bank(mwb_handle* h, int32_t slots);
  * device.  MWB_ESTATE without the bank. */
 int mwb_save_states(mwb_handle* h, const int32_t* env_ids, const int32_t* slots, int n, void* stream);
 
+/* Goal distance (SPL, shortest-path filters of environment design, distance-shaped rewards, imitation): the geodesic
+ * distance from every env's agent to its goal, the running episode's shortest path and an expert action, on the
+ * device.  One grid per level, grids[l] for level l: node (k, l') of nx x nz sits at (min_x + (k + 0.5) h,
+ * min_z + (l' + 0.5) h), h = MWB_GOAL_GRID_STEP, flat index l' * nx + k; goal_slot is the entity-list slot of the
+ * goal of a level whose rule is near(goal) (MWB_RULE_GOAL), -1 for a level without one. */
+#define MWB_GOAL_GRID_STEP 0.25
+#define MWB_GOAL_GRID_CAP 65536        /* nodes of one grid */
+typedef struct mwb_goal_grid {
+  double min_x, min_z;
+  int32_t nx, nz;
+  int32_t goal_slot;         /* -1 = no goal rule: the level's envs report NaN / -1                */
+  int32_t reserved;          /* 0                                                                  */
+} mwb_goal_grid;
+/* Valid on a handle with device resets and a level table or Maze level set up (MWB_ESTATE when it resets on the host
+ * or has the mode on already; mwb_set_levels, mwb_set_maze and mwb_set_level_maze fail with MWB_ESTATE afterwards,
+ * since the grids cover the levels' rooms).  MWB_EINVAL for a null array, a nonzero reserved field, no level with a
+ * goal slot, a goal slot outside [0, max_ents) or a grid with nx or nz < 1; MWB_ECAPACITY for a grid of more than
+ * MWB_GOAL_GRID_CAP nodes.  G is the largest grid (nx * nz) over the levels with a goal.  Arrays, read in place through
+ * mwb_state_array, stream-ordered, all read-only:
+ *   goal_dist float64 [N]        metres from the agent's pose after the last mwb_step / mwb_reset (NaN before the
+ *                                first, and at levels without a goal);
+ *   expert_action int32 [N]      0 turn_left, 1 turn_right, 2 move_forward, -1 = none;
+ *   episode_shortest float64 [N] goal_dist right after the reset that started the running episode (a program reset
+ *                                or a state-bank load); after a terminating step it still names the episode that ended;
+ *   goal_field uint16 [N][G]     the env's distance field, in units of h / 5, 0xFFFF = unreachable or blocked.
+ * A reset of env i (program or bank load) builds env i's field from its world as the reset left it, in a kernel that
+ * follows the reset in mwb_reset and K1 in mwb_step; that kernel then writes goal_dist and expert_action of every env,
+ * and episode_shortest of the envs it reset.  With r the agent prototype's radius, a node inside some room is a source
+ * when an agent standing there is near(goal) (the rule's own threshold, walls ignored), and free when no wall lies
+ * within r + h/2 and no entity other than the agent and the goal within r + h/2 + its radius.  Edges join free-or-source
+ * 8-neighbours; orthogonal ones cost 5, diagonal ones 7 and need both orthogonal neighbours they pass free-or-source;
+ * the field is the shortest-path distance from the nearest source, capped at 0xFFFE.  goal_dist is 0 when the agent is
+ * near(goal), else the minimum over the free nodes with a finite field of the 4 x 4 block k0 - 1 .. k0 + 2 (k0 =
+ * floor((x - min_x) / h - 0.5), same for z) of field * 0.05 + the straight distance, +inf when there is none.  The
+ * expert heads for the goal when that node's field is 0 or the agent is near, else for the node's neighbour with the
+ * least field + edge cost (ties: lowest flat index), moving forward when within half the level's default turn_step of
+ * the heading to it and turning towards it otherwise.  mwb_restore rebuilds every field and keeps episode_shortest
+ * from the blob.  Handles that never call this behave exactly as before it existed, and the addition changes no
+ * existing struct, so MWB_ABI_VERSION stays as it is.  Snapshots of a handle with the mode on carry episode_shortest
+ * and are marked as such in the header; restoring across the mode fails with MWB_ESTATE. */
+int mwb_enable_goal_distance(mwb_handle* h, const mwb_goal_grid* grids /* [n_levels] */);
+
 /* Maze levels in a level table (curricula over maze sizes: MazeS2 -> MazeS3 -> Maze, next to fixed-layout levels).
  * Valid on a shared_geometry = 1 handle after mwb_set_levels (MWB_ESTATE otherwise).  Level `level` (MWB_EINVAL
  * outside [0, L)) becomes a per-env-world level: every reset of an env at that level carves a fresh maze from these
@@ -689,6 +731,11 @@ int mwb_debug_camera(mwb_handle* h, float* out /* host [num_envs][16] */);
 #define MWB_ARRAY_NEXT_DRAWS 29       /* float64 [num_envs][D]  designed outcome of each reset draw, next reset        */
 #define MWB_ARRAY_DRAWS_PENDING 30    /* uint8 [num_envs]  nonzero = the designed draws wait for the next reset        */
 #define MWB_ARRAY_EPISODE_DRAWS 31    /* float64 [num_envs][D]  outcome of each reset draw of the running episode      */
+/* with goal distance on (mwb_enable_goal_distance; MWB_ESTATE otherwise), read-only; count = elements: */
+#define MWB_ARRAY_GOAL_DIST 32        /* float64 [num_envs]  geodesic metres from the agent to the goal                 */
+#define MWB_ARRAY_EXPERT_ACTION 33    /* int32 [num_envs]  action along the shortest path, -1 = none                   */
+#define MWB_ARRAY_EPISODE_SHORTEST 34 /* float64 [num_envs]  goal_dist right after the running episode's reset          */
+#define MWB_ARRAY_GOAL_FIELD 35       /* uint16 [num_envs][G]  distance field in units of h / 5, 0xFFFF = none          */
 int mwb_state_array(mwb_handle* h, int which, void** dev_ptr, int64_t* count);
 /* 1 when this library keeps the handle's state arrays (mwb_state_array) in host memory -- the CPU build of the kernels
  * used by the test suite -- and 0 for libmwb.so, whose arrays are device memory. */
@@ -706,7 +753,7 @@ int mwb_flag_wait_geq(void* cuda_stream, const uint32_t* dev_ptr, uint32_t value
 int mwb_flag_mode(void);
 
 /* sizeof() of every ABI struct, in declaration order (config, params, tex_desc, mesh_desc,
- * room, quad, seg, proto, entity, op, geometry, world, rng_state, state_view, maze_desc, level): lets a
+ * room, quad, seg, proto, entity, op, geometry, world, rng_state, state_view, maze_desc, level, goal_grid): lets a
  * binding verify its mirror of this header.  Returns the number of entries written. */
 int mwb_abi_sizes(int32_t* out, int cap);
 

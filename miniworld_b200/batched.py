@@ -25,7 +25,9 @@ Per-environment semantics are exactly those of the reference's `MiniWorldEnv.res
     colours, box sizes, goal sides, headings) written into a device tensor (`next_draws`, `set_env_draws`), and
     `info["draws"]` holds the outcome of every draw of each running episode;
   * with `state_bank=K`, envs can be saved into K device-side records (`save_states`) and an env's next reset can load
-    one (`next_state`, `set_env_state`), and `info["state"]` names the record each running episode was loaded from.
+    one (`next_state`, `set_env_state`), and `info["state"]` names the record each running episode was loaded from;
+  * with `goal_distance=True`, every step and reset leaves each env's geodesic distance to its goal (`goal_dist`), an
+    expert action (`expert_action`) and its episode's shortest path (`episode_shortest`) on the device.
 
 Outputs are torch CUDA tensors by default (zero-copy from the kernels); `step_host`
 performs the same step with pinned host buffers for callers that want numpy.
@@ -33,7 +35,7 @@ performs the same step with pinned host buffers for callers that want numpy.
 import numpy as np
 
 from . import pack
-from .engine import (Engine, LEVEL_CAP, LOWERED_PARAMS, OP_PLACE, OP_PUT, PARAMS_COLUMN, PROTO_DTYPE, RULE_GOAL,
+from .engine import (Engine, GOAL_GRID_DTYPE, LEVEL_CAP, LOWERED_PARAMS, OP_PLACE, OP_PUT, PARAMS_COLUMN, PROTO_DTYPE, RULE_GOAL,
                      RULE_NONE, RULE_HEALTH, RULE_PICKUP, RULE_PUTNEXT, RULE_SIDEWALK, RULE_SIGN, generator_from_state,
                      rng_state_of, RNG_DTYPE)
 from .envs import LEVELS
@@ -179,6 +181,8 @@ _NEEDS = {**dict.fromkeys(("env_level", "next_level", "level_weights"), (
               "reset_draws", RuntimeError, "this batch has no reset draws: construct it with reset_draws=True")),
           **dict.fromkeys(("next_state", "episode_state", "bank_level"), (
               "state_bank", RuntimeError, "this batch has no state bank: construct it with state_bank=K")),
+          **dict.fromkeys(("goal_dist", "expert_action", "episode_shortest", "goal_field"), (
+              "goal_distance", RuntimeError, "this batch has no goal distance: construct it with goal_distance=True")),
           "level_params": ("device_reset", TypeError, "level params change at device resets; host-reset levels draw "
                            "theirs in Python (set them on the level's own DomainParams)")}
 
@@ -288,12 +292,25 @@ class BatchedMiniWorld:
     `step_count` included.  `episode_state` / `info["state"]` name the slot each running episode was loaded from, or -1;
     after a terminating step they still name the episode that just ended.  `bank_level` holds each slot's level (-1 =
     empty).  A record takes about 264 B + 68 B per entity slot + 12 B per room; at levels with per-env worlds it has
-    room for one world block as well (about 123 KB for an 8 x 8 Maze), so 4096 slots of such a batch take over 0.5 GB."""
+    room for one world block as well (about 123 KB for an 8 x 8 Maze), so 4096 slots of such a batch take over 0.5 GB.
+
+    `goal_distance=True` (one level or a table; levels that reset on the device, one of them with a goal rule: Hallway,
+    OneRoom, FourRooms, TMaze, YMaze, WallGap and the Maze family) gives the shortest path to the goal on the device, for
+    SPL, shortest-path filters of environment design, distance-shaped rewards and imitation learning.  Each goal level
+    gets a grid of 0.25 m over its rooms' bounding box (`goal_grids`, `grid_shape`); every reset, a state-bank load
+    included, builds the env's distance field over it from the world it left (`goal_field`, uint16 [N, G] in units of
+    0.05 m, node (k, l) at index l * nx + k, 0xFFFF unreachable), and after every step and reset `goal_dist` /
+    `info["goal_dist"]` (float64 [N], metres) hold the agent's geodesic distance to the goal: 0 when it is near the goal,
+    +inf when no free node near it reaches the goal, NaN at levels without a goal rule.  `expert_action` (int32 [N]) is
+    the action along a shortest path (turn left, turn right or move forward; -1 where goal_dist is not finite), and
+    `episode_shortest` / `info["shortest"]` the goal_dist right after the reset that started the running episode; after
+    a terminating step it still names the episode that just ended.  navigation.py restates the definitions in numpy.
+    Memory is 3 G + 21 bytes per env (G: the largest grid, 10 609 nodes for an 8 x 8 Maze)."""
 
     def __init__(self, level, num_envs, obs_width=80, obs_height=60, domain_rand=False, autoreset=True,
                  msaa_samples=8, device=0, want_depth=False, level_kwargs=None, obs_format="hwc", env_level=None,
                  dynamic_levels=False, level_seed=0, env_offset=0, per_env_worlds=False, episode_seeds=False,
-                 maze_layouts=False, start_poses=False, state_bank=None, reset_draws=False):
+                 maze_layouts=False, start_poses=False, state_bank=None, reset_draws=False, goal_distance=False):
         self.num_envs = int(num_envs)
         self.obs_width, self.obs_height = int(obs_width), int(obs_height)
         self.domain_rand = bool(domain_rand)
@@ -305,6 +322,7 @@ class BatchedMiniWorld:
         self.maze_layouts = bool(maze_layouts)
         self.start_poses = bool(start_poses)
         self.reset_draws = bool(reset_draws)
+        self.goal_distance = bool(goal_distance)
         if state_bank is not None and (isinstance(state_bank, bool) or not isinstance(state_bank, (int, np.integer))
                                        or state_bank < 1):
             raise ValueError("state_bank is a number of slots >= 1, got %r" % (state_bank,))
@@ -328,7 +346,7 @@ class BatchedMiniWorld:
         self._view_map = _Views(self.engine, self.device, dict(
             dynamic_levels=self.dynamic_levels, episode_seeds=self.episode_seeds, maze_layouts=self.maze_layouts,
             start_poses=self.start_poses, state_bank=self.state_bank, reset_draws=self.reset_draws,
-            device_reset=self.device_reset),
+            goal_distance=self.goal_distance, device_reset=self.device_reset),
             getattr(self, "maze_shape", None))
         if self.dynamic_levels:
             self.level_seed, self.env_offset = int(level_seed), int(env_offset)
@@ -355,6 +373,8 @@ class BatchedMiniWorld:
                 self.engine.close()
                 raise ValueError("reset_draws needs a level with a reset draw; %s make none" % ", ".join(self.level_ids))
             self.engine.enable_reset_draws()
+        if self.goal_distance:
+            self._enable_goal_distance(defs)
         if self.state_bank:
             if not self.device_reset:
                 self.engine.close()
@@ -373,6 +393,37 @@ class BatchedMiniWorld:
         self._torch = None
         self._bufs = None
         self._params_written = False
+
+    def _enable_goal_distance(self, defs):
+        """goal_distance=True: one grid per level from its definition instance (navigation.level_grid), goal slot -1 at
+        levels without a goal rule."""
+        from .navigation import level_grid
+        if not self.device_reset:
+            self.engine.close()
+            raise TypeError("goal distance is built by device resets; host-reset levels build their worlds in Python "
+                            "(MiniWorldEnv.goal_distance() of the level itself)")
+        grids = np.zeros(len(defs), GOAL_GRID_DTYPE)
+        grids["goal_slot"] = -1
+        for l, d in enumerate(defs):
+            if d.rule[0] != RULE_GOAL:
+                continue
+            try:
+                grids[l]["min_x"], grids[l]["min_z"], grids[l]["nx"], grids[l]["nz"] = level_grid(d.pe)
+            except ValueError:
+                self.engine.close()
+                raise
+            grids[l]["goal_slot"] = d.rule[1]
+        if not (grids["goal_slot"] >= 0).any():
+            self.engine.close()
+            raise ValueError("goal_distance needs a level with a goal rule; %s have none" % ", ".join(map(str, self.level_ids)))
+        self.goal_grids = grids
+        self.engine.enable_goal_distance(grids)
+
+    @property
+    def grid_shape(self):
+        """(nz, nx) of each level's goal grid, None at levels without a goal rule (goal_distance=True)."""
+        self._views()["goal_dist"]                   # a batch without the mode raises
+        return [(int(g["nz"]), int(g["nx"])) if g["goal_slot"] >= 0 else None for g in self.goal_grids]
 
     def _init_level(self, level, level_kwargs):
         d = _define_level(level, level_kwargs, self.domain_rand, self.obs_width, self.obs_height)
@@ -489,7 +540,8 @@ class BatchedMiniWorld:
             self._host_done = np.zeros(self.num_envs, bool)
         elif self.maze_template is not None:
             eng.set_params(d0.pe.params)
-            eng.set_protos(self.program.proto_array())
+            self.proto_table = self.program.proto_array()
+            eng.set_protos(self.proto_table)
             eng.set_maze(self.maze_template, d0.maze_cdf)
             eng.set_program(self.program.op_array())
         else:
@@ -501,7 +553,8 @@ class BatchedMiniWorld:
                 protos.extend(d.program.protos)
                 rows.append(dict(rule=d.rule, max_episode_steps=d.max_episode_steps, params=d.pe.params,
                                  geometry=d.geometry, ops=ops, domain_rand=int(d.domain_rand)))
-            eng.set_protos(np.array(protos, PROTO_DTYPE))
+            self.proto_table = np.array(protos, PROTO_DTYPE)
+            eng.set_protos(self.proto_table)
             eng.set_levels(rows, self._env_level)
             for lvl, d in enumerate(defs):
                 if d.maze is not None:
@@ -554,6 +607,11 @@ class BatchedMiniWorld:
                 # the outcome of every reset draw of each env's current episode (after a terminating step still the
                 # ended one's)
                 self._info["draws"] = self.episode_draws
+            if self.goal_distance:
+                # the agent's geodesic distance to the goal now, and the shortest path of each env's current episode
+                # (after a terminating step still the ended one's)
+                self._info["goal_dist"] = self.goal_dist
+                self._info["shortest"] = self.episode_shortest
             if self.state_bank:
                 # the slot each env's current episode was loaded from, -1 for none (after a terminating step still the
                 # ended one's)
@@ -853,6 +911,30 @@ class BatchedMiniWorld:
     def bank_level(self):
         """int32 [K] view of the level of the state each slot holds, -1 for an empty slot (read-only)."""
         return self._views()["bank_level"]
+
+    # ------------------------------------------------------------------ goal distance (goal_distance=True)
+    @property
+    def goal_dist(self):
+        """float64 [N] view of each agent's geodesic distance to its goal in metres after the last step or reset
+        (read-only): 0 near the goal, +inf when unreachable, NaN at levels without a goal rule."""
+        return self._views()["goal_dist"]
+
+    @property
+    def expert_action(self):
+        """int32 [N] view of the action along a shortest path to the goal (0 turn left, 1 turn right, 2 move forward),
+        -1 where goal_dist is not finite (read-only)."""
+        return self._views()["expert_action"]
+
+    @property
+    def episode_shortest(self):
+        """float64 [N] view of goal_dist right after the reset that started each env's running episode (read-only)."""
+        return self._views()["episode_shortest"]
+
+    @property
+    def goal_field(self):
+        """uint16 [N, G] view of each env's distance field in units of 0.05 m, 0xFFFF for unreachable and blocked
+        nodes; env i's grid is goal_field[i, :nz * nx].reshape(nz, nx) with grid_shape[level] (read-only)."""
+        return self._views()["goal_field"]
 
     def entity_xz(self, slot):
         """float64 [N, 2]: the (x, z) floor position of entity-list slot `slot` of every env, read from the device

@@ -1,6 +1,7 @@
 // mwb.cu -- libmwb.so: the C ABI of include/mwb.h on top of the CUDA kernels.
 //
 //   step_kernel   (K1)  physics.cuh + reset.cuh   one warp per env
+//   nav_kernel          navigation.cuh            one block per env, after K1 and reset_kernel (goal distance on)
 //   render_kernel (K2)  raster.cuh                one block per env, one warp per 8x4 half-tile
 //   scatter / gather    host <-> SoA state exchange for host-generated worlds
 //
@@ -22,6 +23,7 @@
 #include "raster.cuh"
 #include "visibility.cuh"
 #include "reset.cuh"
+#include "navigation.cuh"
 
 #ifndef MWB_HOSTSIM
 #include <cuda_runtime.h>
@@ -124,6 +126,7 @@ struct mwb_handle {
   MazeLayouts layouts_h;              // host copy of *S.layouts (mwb_enable_maze_layouts)
   StartPoses poses_h;                 // host copy of *S.poses (mwb_enable_start_poses)
   ResetDraws draws_h;                 // host copy of *S.draws (mwb_enable_reset_draws)
+  GoalNav nav_h;                      // host copy of *S.nav (mwb_enable_goal_distance)
   StateBank bank_h;                   // host copy of *S.bank (mwb_enable_state_bank)
   int32_t* d_bank_pairs;              // [2][slots] staging of a host mwb_save_states call (env ids, then slots)
   int32_t* d_bank_winner;             // [slots] per-call scratch: the last entry of each slot
@@ -377,6 +380,12 @@ __global__ void bank_save_kernel(DevState S, const int32_t* envs, const int32_t*
   const int e = envs[t], s = slots[t];
   if (e < 0 || e >= S.N || s < 0 || s >= S.bank->slots || winner[s] != t) return;
   bank_save(S.bank, S.env_level, S.levels, e, s);
+}
+// goal distance: one block per env, shared memory uint16 field [G] then uint8 classes [G] (navigation.cuh)
+__global__ void __launch_bounds__(MWB_NAV_THREADS) nav_kernel(DevState S) {
+  extern __shared__ __align__(16) uint8_t nav_smem[];
+  const int G = S.nav->G;
+  goal_nav(S, blockIdx.x, (uint16_t*)nav_smem, nav_smem + 2 * (size_t)G);
 }
 __global__ void scatter_kernel(DevState S, const WorldUpload* u, int n) {
   int t = blockIdx.x * blockDim.x + threadIdx.x;
@@ -905,7 +914,7 @@ extern "C" int mwb_abi_sizes(int32_t* out, int cap) {
                         (int32_t)sizeof(mwb_seg), (int32_t)sizeof(mwb_proto), (int32_t)sizeof(mwb_entity),
                         (int32_t)sizeof(mwb_op), (int32_t)sizeof(mwb_geometry), (int32_t)sizeof(mwb_world),
                         (int32_t)sizeof(mwb_rng_state), (int32_t)sizeof(mwb_state_view), (int32_t)sizeof(mwb_maze_desc),
-                        (int32_t)sizeof(mwb_level)};
+                        (int32_t)sizeof(mwb_level), (int32_t)sizeof(mwb_goal_grid)};
   const int n = (int)(sizeof(sz) / sizeof(sz[0]));
   for (int k = 0; k < n && k < cap; ++k) out[k] = sz[k];
   return n;
@@ -1284,6 +1293,7 @@ extern "C" int mwb_set_levels(mwb_handle* h, int n_levels, const mwb_level* leve
   if (h->S.next_level) return fail(MWB_ESTATE, "the level table is fixed once level changes are on");
   if (h->S.bank) return fail(MWB_ESTATE, "the level table is fixed once the state bank is on (its record layout depends on it)");
   if (h->level_mazes) return fail(MWB_ESTATE, "the level table is fixed once it has Maze levels (mwb_set_level_maze)");
+  if (h->S.nav) return fail(MWB_ESTATE, "the level table is fixed once goal distance is on (its grids are per level)");
   if (n_levels <= 0) return fail(MWB_EINVAL, "n_levels must be positive");
   if (n_levels > MWB_LEVEL_CAP) return fail(MWB_ECAPACITY, "more than MWB_LEVEL_CAP levels");
   if (n_ops <= 0) return fail(MWB_EINVAL, "empty op array");
@@ -1441,6 +1451,7 @@ extern "C" int mwb_set_maze(mwb_handle* h, const mwb_maze_desc* mz) {
   if (!h || !mz || !mz->cdf) return fail(MWB_EINVAL, "null argument");
   if (h->cfg.shared_geometry) return fail(MWB_ESTATE, "Maze needs per-env geometry (shared_geometry = 0)");
   if (h->S.bank) return fail(MWB_ESTATE, "the Maze templates are fixed once the state bank is on (its record layout depends on it)");
+  if (h->S.nav) return fail(MWB_ESTATE, "the Maze templates are fixed once goal distance is on (its grids cover them)");
   const int cells = mz->rows * mz->cols;
   if (cells <= 0 || cells > MWB_MAZE_MAX_CELLS) return fail(MWB_ECAPACITY, "maze too large");
   if (2 * cells - 1 > h->S.R) return fail(MWB_ECAPACITY, "max_rooms too small for this maze");
@@ -1486,6 +1497,7 @@ extern "C" int mwb_set_level_maze(mwb_handle* h, int level, const mwb_maze_desc*
     return fail(MWB_ESTATE, "Maze levels in a table need a shared_geometry = 1 handle and mwb_set_levels first");
   if (level < 0 || level >= (int)h->levels.size()) return fail(MWB_EINVAL, "level out of range");
   if (h->S.bank) return fail(MWB_ESTATE, "Maze levels cannot be added once the state bank is on (its record layout depends on it)");
+  if (h->S.nav) return fail(MWB_ESTATE, "Maze levels cannot be added once goal distance is on (its grids are per level)");
   const int cells = mz->rows * mz->cols;
   if (cells <= 0 || cells > MWB_MAZE_MAX_CELLS) return fail(MWB_ECAPACITY, "maze too large");
   // a maze of c cells is a spanning tree: 2c - 1 rooms, 8c - 2 quads and 4c segments, whatever the episode draws
@@ -1614,6 +1626,86 @@ extern "C" int mwb_enable_reset_draws(mwb_handle* h) {
   if (alloc_arr(h, &d, 1)) return fail(MWB_ECUDA, "reset draw state allocation failed");
   if (h2d(d, &R, sizeof(R), h->stream) != 0 || sync_stream(h->stream) != 0) return fail(MWB_ECUDA, "upload failed");
   h->S.draws = d;
+  return MWB_OK;
+}
+
+#ifndef MWB_HOSTSIM
+// nav_kernel's shared memory opt-in, per device: like K2's (ensure_k2_smem) an attribute of the kernel function that
+// handles with different grids share, so it is only ever raised
+static int g_nav_smem[16] = {};
+static int ensure_nav_smem(mwb_handle* h, int smem) {
+  int& granted = g_nav_smem[h->cfg.device & 15];
+  if (smem <= granted) return 0;
+  if (cudaFuncSetAttribute(nav_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) return -1;
+  granted = smem;
+  return 0;
+}
+#endif
+
+// Goal distance after a launch that reset or restored envs: every env's block (navigation.cuh), on stream s.
+static int launch_nav(mwb_handle* h, stream_t s) {
+#ifndef MWB_HOSTSIM
+  const int smem = 3 * h->nav_h.G;
+  if (ensure_nav_smem(h, smem)) return fail(MWB_ECUDA, "cudaFuncSetAttribute(nav_kernel, MaxDynamicSharedMemorySize) failed");
+  nav_kernel<<<h->S.N, MWB_NAV_THREADS, (size_t)smem, s>>>(h->S);
+  h->launches++;
+  CK(cudaGetLastError());
+#else
+  (void)s;
+  std::vector<uint16_t> f((size_t)h->nav_h.G);
+  std::vector<uint8_t> c((size_t)h->nav_h.G);
+  for (int i = 0; i < h->S.N; ++i) goal_nav(h->S, i, f.data(), c.data());
+#endif
+  return MWB_OK;
+}
+
+extern "C" int mwb_enable_goal_distance(mwb_handle* h, const mwb_goal_grid* grids) {
+  if (!h) return fail(MWB_EINVAL, "null handle");
+  if (h->S.nav) return fail(MWB_ESTATE, "goal distance is already on");
+  if (!h->have_params || !h->S.ops)
+    return fail(MWB_ESTATE, "goal distance needs device resets (params and a reset program: mwb_set_levels, or "
+                            "mwb_set_params and mwb_set_program); host-generated worlds arrive without a reset kernel");
+  if (!grids) return fail(MWB_EINVAL, "null grids");
+  int64_t G = 0;
+  for (size_t l = 0; l < h->levels.size(); ++l) {
+    const mwb_goal_grid& g = grids[l];
+    if (g.reserved != 0) return fail(MWB_EINVAL, "level " + std::to_string(l) + ": mwb_goal_grid.reserved must be 0");
+    if (g.goal_slot < 0) continue;
+    const std::string lv = "level " + std::to_string(l);
+    if (g.goal_slot >= h->S.E) return fail(MWB_EINVAL, lv + ": goal slot outside the entity list");
+    if (g.nx < 1 || g.nz < 1) return fail(MWB_EINVAL, lv + ": a goal grid needs nx, nz >= 1");
+    if ((int64_t)g.nx * g.nz > MWB_GOAL_GRID_CAP)
+      return fail(MWB_ECAPACITY, lv + ": goal grid of " + std::to_string((int64_t)g.nx * g.nz) +
+                                     " nodes, more than MWB_GOAL_GRID_CAP");
+    G = std::max(G, (int64_t)g.nx * g.nz);
+  }
+  if (G == 0) return fail(MWB_EINVAL, "no level of this handle has a goal slot");
+  const size_t N = h->S.N;
+  void *field, *cls, *dirty, *dist, *expert, *shortest;
+  // field 0xFFFF, distances NaN and actions -1 (0xFF bytes) until the first launch; every env builds its field then
+  int rc = alloc_control_arrays(h, "goal distance", {{&field, N * G * sizeof(uint16_t), true}, {&cls, N * G, false},
+                                                     {&dirty, N, true}, {&dist, N * sizeof(double), true},
+                                                     {&expert, N * sizeof(int32_t), true},
+                                                     {&shortest, N * sizeof(double), true}});
+  if (rc) return rc;
+  mwb_goal_grid* d_grids = nullptr;
+  if (alloc_arr(h, &d_grids, h->levels.size())) return fail(MWB_ECUDA, "goal distance state allocation failed");
+  GoalNav& V = h->nav_h;
+  V.grids = d_grids;
+  V.field = (uint16_t*)field;
+  V.node_class = (uint8_t*)cls;
+  V.dirty = (uint8_t*)dirty;
+  V.goal_dist = (double*)dist;
+  V.expert = (int32_t*)expert;
+  V.shortest = (double*)shortest;
+  V.G = (int32_t)G;
+  V.pad_ = 0;
+  GoalNav* d = nullptr;
+  if (alloc_arr(h, &d, 1)) return fail(MWB_ECUDA, "goal distance state allocation failed");
+  if (h2d(d_grids, grids, h->levels.size() * sizeof(mwb_goal_grid), h->stream) != 0 || h2d(d, &V, sizeof(V), h->stream) != 0 ||
+      sync_stream(h->stream) != 0)
+    return fail(MWB_ECUDA, "upload failed");
+  h->S.nav = d;
   return MWB_OK;
 }
 
@@ -1856,6 +1948,7 @@ extern "C" int mwb_reset(mwb_handle* h, const int32_t* env_ids, int n, void* str
   reset_kernel<<<(n + 3) / 4, 128, 0, s>>>(h->S, ids, n);
   h->launches++;
   CK(cudaGetLastError());
+  if (h->S.nav && launch_nav(h, s)) return MWB_ECUDA;
   if (stream_leave(h, s)) return MWB_ECUDA;
   if (!stream) CK(cudaStreamSynchronize(s));
 #else
@@ -1864,6 +1957,7 @@ extern "C" int mwb_reset(mwb_handle* h, const int32_t* env_ids, int n, void* str
     device_reset(h->S, i);
     h->S.needs_reset[i] = 0;
   }
+  if (h->S.nav) launch_nav(h, s);
 #endif
   return MWB_OK;
 }
@@ -2204,6 +2298,7 @@ extern "C" int mwb_step(mwb_handle* h, const int32_t* actions, const double* ste
 #else
   for (size_t i = 0; i < N; ++i) step_one(h->S, (int)i, d_act, d_sp, d_rew, d_te, d_tr);
 #endif
+  if (h->S.nav && launch_nav(h, s)) return MWB_ECUDA;
   const bool obs_host = obs && !is_device_ptr(obs), depth_host = depth && !is_device_ptr(depth);
   if (obs || depth) {
     int rc = launch_render(h, obs ? (obs_host ? h->d_obs : obs) : nullptr, depth ? (depth_host ? h->d_depth : depth) : nullptr, s,
@@ -2357,12 +2452,15 @@ static const uint32_t kSnapMagicBank = 0x00000020u;
 // one with reset draws on sets the high bit of the mode letter (every letter's case bit already names a mode) and
 // carries next_draws, draws_pending and episode_draws
 static const uint32_t kSnapMagicDraws = 0x80000000u;
-static const uint32_t kSnapMagicModes = kSnapMagicSeeds | kSnapMagicMazes | kSnapMagicPoses | kSnapMagicBank | kSnapMagicDraws;
+// one with goal distance on sets the high bit of the "M" and carries episode_shortest (the fields are rebuilt)
+static const uint32_t kSnapMagicNav = 0x00000080u;
+static const uint32_t kSnapMagicModes =
+    kSnapMagicSeeds | kSnapMagicMazes | kSnapMagicPoses | kSnapMagicBank | kSnapMagicDraws | kSnapMagicNav;
 
 static uint32_t snapshot_magic(const mwb_handle* h) {
   const uint32_t seeds = (h->S.next_seed ? kSnapMagicSeeds : 0u) | (h->S.layouts ? kSnapMagicMazes : 0u) |
                          (h->S.poses ? kSnapMagicPoses : 0u) | (h->S.bank ? kSnapMagicBank : 0u) |
-                         (h->S.draws ? kSnapMagicDraws : 0u);
+                         (h->S.draws ? kSnapMagicDraws : 0u) | (h->S.nav ? kSnapMagicNav : 0u);
   if (h->level_mazes) return (h->S.next_level ? kSnapMagicWorldsLevelChanges : kSnapMagicWorlds) | seeds;
   return (h->S.next_level ? kSnapMagicLevelChanges : kSnapMagic) | seeds;
 }
@@ -2376,7 +2474,8 @@ static std::string snapshot_mode(uint32_t magic) {
          (magic & kSnapMagicMazes ? ", maze layouts on" : ", maze layouts off") +
          (magic & kSnapMagicPoses ? ", start poses on" : ", start poses off") +
          (magic & kSnapMagicBank ? ", state bank on" : ", state bank off") +
-         (magic & kSnapMagicDraws ? ", reset draws on" : ", reset draws off");
+         (magic & kSnapMagicDraws ? ", reset draws on" : ", reset draws off") +
+         (magic & kSnapMagicNav ? ", goal distance on" : ", goal distance off");
 }
 
 struct SnapHeader {
@@ -2405,8 +2504,8 @@ struct SnapSection {
 
 // The sections of a blob after its header, in blob order: every array that changes while episodes run (entity lists,
 // counters, camera / lighting parameters, RNG streams, pending-reset flags), the geometry currently on the device and
-// the level ranges, then the episode-seed, maze-layout, start-pose and reset-draw arrays and the state bank of handles with those
-// modes on.  A handle with level
+// the level ranges, then the episode-seed, maze-layout, start-pose and reset-draw arrays, the state bank and
+// episode_shortest of handles with those modes on.  A handle with level
 // changes on closes the blob with its level-change section: env_level, next_level, level_draws, level_weights and
 // `tail` (adopted on restore: the assignment is state).  A static table of several levels closes it with the host's
 // env_level (checked on restore, never overwritten).
@@ -2445,6 +2544,7 @@ static std::vector<SnapSection> snapshot_sections(mwb_handle* h, LevelChangeTail
     dev(B.records, (size_t)B.slots * B.rec_bytes); dev(B.bank_level, (size_t)B.slots * sizeof(int32_t));
     dev(B.next_state, N * sizeof(int32_t)); dev(B.episode_state, N * sizeof(int32_t));
   }
+  if (S.nav) dev(h->nav_h.shortest, N * sizeof(double));
   if (S.next_level) {
     SA(env_level, N); SA(next_level, N); SA(level_draws, N); SA(level_weights, S.num_levels);
     v.push_back(SnapSection{nullptr, tail, sizeof(*tail)});
@@ -2550,6 +2650,11 @@ extern "C" int mwb_restore(mwb_handle* h, const void* blob, size_t bytes) {
     h->S.level_env_offset = tail.env_offset;
   }
   if (sync_stream(h->stream) != 0) return fail(MWB_ECUDA, "sync failed");
+  if (S.nav) {   // the fields are a function of the restored worlds: rebuild them all, keeping episode_shortest
+    if (dev_memset(h->nav_h.dirty, 2, (size_t)S.N) != 0) return fail(MWB_ECUDA, "memset failed");
+    if (launch_nav(h, h->stream)) return MWB_ECUDA;
+    if (sync_stream(h->stream) != 0) return fail(MWB_ECUDA, "sync failed");
+  }
   return MWB_OK;
 }
 
@@ -2607,6 +2712,8 @@ extern "C" int mwb_state_array(mwb_handle* h, int which, void** dev_ptr, int64_t
   const char* bank_off = S.bank ? nullptr : "the state bank is off (mwb_enable_state_bank)";
   const char* draws_off = S.draws ? nullptr : "reset draws are off (mwb_enable_reset_draws)";
   const ResetDraws& Dr = h->draws_h;
+  const char* nav_off = S.nav ? nullptr : "goal distance is off (mwb_enable_goal_distance)";
+  const GoalNav& V = h->nav_h;
   const StateBank& B = h->bank_h;
   const char* params_off = h->have_params && S.ops ? nullptr
                            : "the handle has no device resets (params and a reset program: mwb_set_levels, or "
@@ -2640,6 +2747,10 @@ extern "C" int mwb_state_array(mwb_handle* h, int which, void** dev_ptr, int64_t
     case MWB_ARRAY_NEXT_DRAWS: p = Dr.next; n = N * Dr.D; off = draws_off; break;                 // float64 [N][D]
     case MWB_ARRAY_DRAWS_PENDING: p = Dr.pending; off = draws_off; break;                         // uint8 [N]
     case MWB_ARRAY_EPISODE_DRAWS: p = Dr.episode; n = N * Dr.D; off = draws_off; break;           // float64 [N][D]
+    case MWB_ARRAY_GOAL_DIST: p = V.goal_dist; off = nav_off; break;                              // float64 [N]
+    case MWB_ARRAY_EXPERT_ACTION: p = V.expert; off = nav_off; break;                             // int32 [N]
+    case MWB_ARRAY_EPISODE_SHORTEST: p = V.shortest; off = nav_off; break;                        // float64 [N]
+    case MWB_ARRAY_GOAL_FIELD: p = V.field; n = N * V.G; off = nav_off; break;                    // uint16 [N][G]
     case MWB_ARRAY_LEVEL_PARAMS: p = (void*)S.level_params; n = (int64_t)h->levels.size(); off = params_off; break;  // mwb_params [L]
     default: return fail(MWB_EINVAL, "unknown array");
   }

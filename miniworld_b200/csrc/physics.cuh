@@ -170,18 +170,24 @@ MWB_DEV double near_threshold(double r0, bool r0_f32, double r1, bool r1_f32, do
   return d_add(d_add(r0, r1), extra);
 }
 
-// MiniWorldEnv.near(ent): np.linalg.norm(ent.pos - agent.pos) < ent.radius + agent.radius + 1.1 * max_forward_step
-// (3-D distance through BLAS ddot, i.e. an FMA chain)
-MWB_DEV bool near_agent(const DevState& S, int i, int b, int as, double ar) {
+// MiniWorldEnv.near(ent) for an agent of radius ar standing at (px, py, pz): np.linalg.norm(ent.pos - agent.pos) <
+// ent.radius + agent.radius + 1.1 * max_forward_step (3-D distance through BLAS ddot, i.e. an FMA chain)
+MWB_DEV bool near_point(const DevState& S, int i, int b, double px, double py, double pz, double ar) {
   const size_t N = S.N;
   const int bp = S.ent_proto[b * N + i];
   if (bp < 0) return false;
-  const double dx = d_sub(S.ent_px[b * N + i], S.ent_px[as * N + i]);
-  const double dy = d_sub(S.ent_py[b * N + i], S.ent_py[as * N + i]);
-  const double dz = d_sub(S.ent_pz[b * N + i], S.ent_pz[as * N + i]);
+  const double dx = d_sub(S.ent_px[b * N + i], px);
+  const double dy = d_sub(S.ent_py[b * N + i], py);
+  const double dz = d_sub(S.ent_pz[b * N + i], pz);
   const double d = d_sqrt(d_fma(dz, dz, d_fma(dy, dy, d_mul(dx, dx))));
   const EntDims pr = ent_dims(S, i, b, S.protos[bp]);
   return d < near_threshold(pr.radius, pr.f32, ar, false, d_mul(1.1, S.env_mfs[i]));
+}
+
+// MiniWorldEnv.near(ent) of the agent in slot `as`
+MWB_DEV bool near_agent(const DevState& S, int i, int b, int as, double ar) {
+  const size_t N = S.N;
+  return near_point(S, i, b, S.ent_px[as * N + i], S.ent_py[as * N + i], S.ent_pz[as * N + i], ar);
 }
 
 // MiniWorldEnv.near(ent0, ent1) between two entities of the list

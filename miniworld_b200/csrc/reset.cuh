@@ -194,6 +194,8 @@ MWB_DEV_NOINLINE double designed_draw(const ResetDraws* R, int i, const mwb_op* 
 
 MWB_DEV void device_reset(const DevState& S, int i) {
   const size_t N = S.N;
+  // the world changes: the goal distance kernel that follows rebuilds the env's field (navigation.cuh)
+  if (S.nav) S.nav->dirty[i] = 1;
   // a pending saved state wins over everything else and consumes only next_state (bank.cuh)
   if (S.bank && bank_load(S.bank, i, S.env_level[i], S.next_level != nullptr)) return;
   if (S.next_seed) take_seed(S, i);

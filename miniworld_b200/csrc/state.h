@@ -50,6 +50,18 @@ struct ResetDraws {
   int32_t D, pad_;
 };
 
+// The goal distance arrays (mwb_enable_goal_distance); navigation.cuh builds and reads them.
+struct GoalNav {
+  const mwb_goal_grid* grids;   // [levels]
+  uint16_t* field;              // [N][G] distance field of the env's running episode, units of h / 5
+  uint8_t* node_class;          // [N][G] MWB_NAV_* bits of each node (the field alone does not tell a source that is not free)
+  uint8_t* dirty;               // [N] 1 = reset since the last build (episode_shortest follows), other nonzero = rebuild only
+  double* goal_dist;            // [N]
+  int32_t* expert;              // [N]
+  double* shortest;             // [N]
+  int32_t G, pad_;
+};
+
 // One scalar of an env's state in a state-bank record: env i's copy lives at base + i * env_stride (a per-env row of
 // the structure of arrays, or an element of an [N][k] array), the record's at byte rec_off; bytes is 1, 4 or 8.
 struct BankCol {
@@ -195,6 +207,8 @@ struct DevState {
   const struct ResetDraws* draws;
   // state bank (mwb_enable_state_bank); null on a handle without it, one pointer for the same reason
   const struct StateBank* bank;
+  // goal distance (mwb_enable_goal_distance); null on a handle without it, one pointer for the same reason
+  const struct GoalNav* nav;
   int32_t autoreset;
   // StochasticActionWrapper on the device (reference wrappers.py:49-71): per step one uniform() draw from
   // the env's own stream; below act_prob the chosen action stands, else act_random (< 0: integers(0, 6))

@@ -29,7 +29,9 @@ class ShardedMiniWorld:
         `local.episode_seed` are its slice of the single-process arrays, and so are the maze layout arrays of `maze_layouts=True`
         the start pose arrays of `start_poses=True` and the draw arrays of `reset_draws=True` (`local.set_env_draws`
         takes local env ids).  `state_bank=K` gives every rank a bank of K slots of its own:
-        `local.save_states` / `local.set_env_state` take this rank's local env ids, and records stay on their rank."""
+        `local.save_states` / `local.set_env_state` take this rank's local env ids, and records stay on their rank.
+        `goal_distance=True` is passed on as it is: `local.goal_dist`, `local.expert_action` and
+        `local.episode_shortest` are this rank's slice of the single-process arrays."""
         from .batched import BatchedMiniWorld, default_env_level
         self.dist = dist
         self.rank = dist.get_rank() if dist is not None else 0

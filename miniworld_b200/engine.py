@@ -80,6 +80,11 @@ ENTITY_DTYPE = np.dtype([
 OP_DTYPE = np.dtype([
     ("op", "i4"), ("a", "i4"), ("b", "i4"), ("ireg_a", "i4"), ("stride_a", "i4"), ("ireg_b", "i4"),
     ("stride_b", "i4"), ("room", "i4"), ("dir_freg", "i4"), ("is_agent", "i4"), ("f", "f8", 4)], align=True)
+# mwb_goal_grid (mwb_enable_goal_distance): one level's grid and goal slot (-1 = no goal rule)
+GOAL_GRID_DTYPE = np.dtype([("min_x", "<f8"), ("min_z", "<f8"), ("nx", "<i4"), ("nz", "<i4"), ("goal_slot", "<i4"),
+                            ("reserved", "<i4")])
+GOAL_GRID_STEP = 0.25
+GOAL_GRID_CAP = 65536
 RNG_DTYPE = np.dtype([
     ("state_hi", "u8"), ("state_lo", "u8"), ("inc_hi", "u8"), ("inc_lo", "u8"),
     ("has_uint32", "i4"), ("uinteger", "u4")], align=True)
@@ -122,7 +127,7 @@ def _expected_sizes():
     return [C.sizeof(Config), C.sizeof(Params), C.sizeof(TexDesc), C.sizeof(MeshDesc),
             ROOM_DTYPE.itemsize, QUAD_DTYPE.itemsize, SEG_DTYPE.itemsize, PROTO_DTYPE.itemsize,
             ENTITY_DTYPE.itemsize, OP_DTYPE.itemsize, C.sizeof(Geometry), C.sizeof(World),
-            RNG_DTYPE.itemsize, C.sizeof(StateView), C.sizeof(MazeDesc), C.sizeof(Level)]
+            RNG_DTYPE.itemsize, C.sizeof(StateView), C.sizeof(MazeDesc), C.sizeof(Level), GOAL_GRID_DTYPE.itemsize]
 
 
 EXPORTS = (
@@ -136,7 +141,7 @@ EXPORTS = (
     "mwb_flag_write", "mwb_flag_wait_geq", "mwb_flag_mode", "mwb_state_array", "mwb_debug_camera", "mwb_set_obs_peer",
     "mwb_set_levels", "mwb_enable_level_changes", "mwb_state_in_host_memory", "mwb_set_level_maze",
     "mwb_enable_episode_seeds", "mwb_enable_maze_layouts", "mwb_enable_start_poses", "mwb_enable_state_bank",
-    "mwb_save_states", "mwb_enable_reset_draws",
+    "mwb_save_states", "mwb_enable_reset_draws", "mwb_enable_goal_distance",
 )
 OBS_FORMATS = {"hwc": 0, "cwh": 1, "grey": 2}
 
@@ -180,6 +185,7 @@ def load_library():
     lib.mwb_enable_start_poses.argtypes = [vp]
     lib.mwb_enable_state_bank.argtypes = [vp, C.c_int32]
     lib.mwb_enable_reset_draws.argtypes = [vp]
+    lib.mwb_enable_goal_distance.argtypes = [vp, vp]
     lib.mwb_save_states.argtypes = [vp, vp, vp, C.c_int, vp]
     lib.mwb_state_in_host_memory.argtypes = []
     lib.mwb_seed.argtypes = [vp, vp, C.c_int, vp]
@@ -506,6 +512,13 @@ class Engine:
         needs device resets and a level with a draw, before the state bank."""
         self._check(self.lib.mwb_enable_reset_draws(self.h))
 
+    def enable_goal_distance(self, grids):
+        """`grids` (GOAL_GRID_DTYPE [n_levels]): the goal distance kernel follows every step and reset from now on and
+        fills "goal_dist", "expert_action", "episode_shortest" and "goal_field" (mwb_enable_goal_distance); needs
+        device resets, a level with a goal slot and grids of at most GOAL_GRID_CAP nodes."""
+        grids = np.ascontiguousarray(grids, GOAL_GRID_DTYPE)
+        self._check(self.lib.mwb_enable_goal_distance(self.h, _ptr(grids)))
+
     def enable_state_bank(self, slots):
         """`slots` state records; resets with "next_state" set load a filled one, and every reset records the loaded
         slot in "episode_state" from now on (mwb_enable_state_bank); needs device resets, after every other mode."""
@@ -608,7 +621,9 @@ class Engine:
               "pose_pending": (24, "|u1", "env"), "episode_start": (25, "<f8", "env_rows"),
               "next_state": (26, "<i4", "env"), "episode_state": (27, "<i4", "env"), "bank_level": (28, "<i4", "level"),
               "next_draws": (29, "<f8", "env_rows"), "draws_pending": (30, "|u1", "env"),
-              "episode_draws": (31, "<f8", "env_rows")}
+              "episode_draws": (31, "<f8", "env_rows"), "goal_dist": (32, "<f8", "env"),
+              "expert_action": (33, "<i4", "env"), "episode_shortest": (34, "<f8", "env"),
+              "goal_field": (35, "<u2", "env_rows")}
 
     def state_array(self, name, shape=None):
         """Zero-copy view of a state array (mwb_state_array) as an object with __cuda_array_interface__:
@@ -619,7 +634,9 @@ class Engine:
         [N, rows * cols], "next_maze_cells" int32 [N, 2] and "maze_pending" uint8 [N]; with start poses on,
         "next_pose" float64 [N, max_ents, 3], "next_agent_pose" / "episode_start" float64 [N, 3] and "pose_pending"
         uint8 [N]; with the state bank on, "next_state" / "episode_state" int32 [N] and "bank_level" int32 [slots];
-        with reset draws on, "next_draws" / "episode_draws" float64 [N, D] and "draws_pending" uint8 [N].
+        with reset draws on, "next_draws" / "episode_draws" float64 [N, D] and "draws_pending" uint8 [N]; with goal
+        distance on, "goal_dist" / "episode_shortest" float64 [N], "expert_action" int32 [N] and "goal_field" uint16
+        [N, G].
         `shape` gives the view
         another shape of the same size (the maze layouts as [N, rows, cols]).  On the host build of the kernels the
         arrays live in host memory, and the view is a numpy array over the same memory instead."""

@@ -257,6 +257,7 @@ class MiniWorldEnv(gym.Env):
         self.rooms = []
         self.wall_segs = []
         self.reset_options = options        # what the level's _gen_world may read (Maze: a designed layout)
+        self._goal_nav = None               # goal_distance()'s field of this episode, built on first use
         self._start_design = options if options and ("poses" in options or "agent_pose" in options) else None
         if options and "draws" in options:
             self._np_random = _DesignedDraws(self.np_random, dict(options["draws"]))
@@ -431,6 +432,30 @@ class MiniWorldEnv(gym.Env):
             ent1 = self.agent
         dist = np.linalg.norm(ent0.pos - ent1.pos)
         return dist < ent0.radius + ent1.radius + 1.1 * self.max_forward_step
+
+    def goal_distance(self):
+        """The agent's geodesic distance to the goal in metres, as BatchedMiniWorld(goal_distance=True) computes it
+        (navigation.py): 0 when near the goal, +inf when unreachable, NaN for a level without a goal rule."""
+        return self._goal_query()[0]
+
+    def expert_action(self):
+        """The action along a shortest path to the goal (0 turn left, 1 turn right, 2 move forward), -1 where
+        goal_distance() is not finite."""
+        return self._goal_query()[1]
+
+    def _goal_query(self):
+        from . import navigation as nav
+        rule = getattr(self, "device_rule", None)
+        if rule is None or rule[0] != "goal":
+            return math.nan, -1
+        rooms, segs, ents, agent = nav.world_of(self)
+        if self._goal_nav is None:     # the goal and the walls stay put during an episode of a goal level
+            grid = nav.level_grid(self)
+            cls = nav.node_classes(grid, rooms, segs, ents, agent, rule[1], self.max_forward_step)
+            self._goal_nav = grid, cls, nav.distance_field(cls, grid[2], grid[3])
+        grid, cls, field = self._goal_nav
+        return nav.query(grid, field, cls, ents, agent, rule[1], self.max_forward_step, float(self.agent.dir),
+                         float(self.params.params["turn_step"].default))
 
     def _load_tex(self, tex_name):
         rand = self.np_random if self.params.sample(self.np_random, "tex_rand") else None
