@@ -623,6 +623,30 @@ int mwb_render_top_view(mwb_handle* h, const double extents[4], int render_agent
  *   mask         uint32[N] (host or device): bit e = entity-list slot e passed its query          */
 int mwb_visible_ents(mwb_handle* h, uint32_t* mask, void* stream);
 
+/* ---- designed cameras: views of every env from poses the caller writes ------------------------------
+ * A pose row is (x, z, dir), float64, with the level's heading convention dir_vec = (cos dir, 0, -sin dir).
+ * The view of env i from row (x, z, dir) is exactly what the reference's render_obs() / render_depth() return
+ * after agent.pos = (x, agent.pos[1], z) and agent.dir = dir with nothing else changed: the same entity list (a
+ * carried object at its own pose), textures, sky, light and the running episode's cam_height, cam_fwd_disp,
+ * cam_pitch and cam_fov_y.  The agent's body is not drawn (render_obs's render_agent=False); render_agent != 0
+ * additionally draws Agent.render()'s marker triangle (entity.py:518-539) at the agent's REAL pose in the state,
+ * as the top view does: a third-person view.  Frame size, MSAA and observation format are the handle's own.
+ * A row with any non-finite entry, or with |dir| >= 105414350 (the range in which the glibc-exact sin / cos are
+ * validated; reduce headings modulo 2 pi first), is skipped: that env's frame and depth in that view are left
+ * untouched and no camera is computed for it.
+ * Neither call changes any env state.
+ *   poses        float64[views][N][3] (host or device)
+ *   obs          frames [views][N] in the observation format (host or device), or NULL for depth only
+ *   depth        float32[views][N][H][W] (host or device) or NULL
+ * Host destinations go through the handle's staging one view at a time; device ones are written in place on
+ * `stream` without a host sync. */
+int mwb_render_views(mwb_handle* h, const double* poses, int views, int render_agent, uint8_t* obs, float* depth,
+                     void* stream);
+
+/* get_visible_ents (as mwb_visible_ents) with the agent moved to env i's row of poses float64[N][3] (host or
+ * device) as mwb_render_views defines it; a skipped row leaves mask[i] as it is. */
+int mwb_visible_ents_from(mwb_handle* h, const double* poses, uint32_t* mask, void* stream);
+
 /* ---- state exchange (env.agent.pos, env.entities[i].pos ... views; checkpointing) ------ */
 int mwb_get_state(mwb_handle* h, const mwb_state_view* out);
 

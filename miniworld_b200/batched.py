@@ -1271,14 +1271,85 @@ class BatchedMiniWorld:
         self.engine.render_top_view(ext, out, render_agent)
         return out
 
-    def visible_ents(self, out=None):
+    def visible_ents(self, out=None, poses=None):
         """uint32 [N]: bit e set iff entity-list slot e of that env passes the reference's occlusion query
-        (get_visible_ents, miniworld.py:1238-1333)."""
+        (get_visible_ents, miniworld.py:1238-1333).  With `poses` (float64 [N, 3] rows (x, z, dir), a CUDA tensor or
+        numpy array) the query runs from each env's designed camera as `render_views` defines it; a row that
+        `render_views` skips leaves that env's entry of `out` as it is."""
+        if poses is not None:
+            poses = self._view_rows("visible_ents", poses, single=True)
         if out is None:
-            torch = self._ensure_torch()
-            out = torch.zeros(self.num_envs, dtype=torch.int32, device=torch.device("cuda", self.device))
-        self.engine.visible_ents(out)
+            if self.engine.host_memory:
+                out = np.zeros(self.num_envs, np.uint32)
+            else:
+                torch = self._ensure_torch()
+                out = torch.zeros(self.num_envs, dtype=torch.int32, device=torch.device("cuda", self.device))
+        stream = None if (self.engine.host_memory or poses is None) else _torch_stream(self._ensure_torch(), self.device)
+        self.engine.visible_ents(out, stream=stream, poses=poses)
         return out
+
+    def _view_rows(self, what, poses, single=False):
+        """Checked pose rows: a contiguous float64 CUDA tensor or numpy array [V, N, 3] (or [N, 3])."""
+        if hasattr(poses, "is_cuda"):
+            if poses.dtype != self._ensure_torch().float64:
+                raise ValueError("%s: poses must be float64, not %s" % (what, poses.dtype))
+            if not poses.is_cuda and not self.engine.host_memory:
+                poses = poses.numpy()
+            elif not poses.is_contiguous():
+                poses = poses.contiguous()
+        else:
+            if np.asarray(poses).dtype != np.float64:
+                raise ValueError("%s: poses must be float64, not %s" % (what, np.asarray(poses).dtype))
+            poses = np.ascontiguousarray(poses)
+        shape = tuple(poses.shape)
+        ok = shape == (self.num_envs, 3) if single else (len(shape) in (2, 3) and shape[-2:] == (self.num_envs, 3))
+        if not ok or (len(shape) == 3 and shape[0] <= 0):
+            raise ValueError("%s: poses must have shape %s, not %s" % (
+                what, "[N, 3]" if single else "[V, N, 3] or [N, 3] with N = %d" % self.num_envs, shape))
+        return poses
+
+    def render_views(self, poses, render_agent=False, out=None, depth=None):
+        """Render every env from designed cameras (mwb_render_views).  `poses`: float64 [V, N, 3] or [N, 3] rows
+        (x, z, dir), a CUDA tensor or numpy array; the view of env i from (x, z, dir) is what the reference's
+        render_obs() / render_depth() return after agent.pos = (x, agent.pos[1], z), agent.dir = dir, nothing else
+        changed (same entities, textures, light and the episode's camera parameters).  `render_agent=True` also draws
+        the agent's marker triangle at its real pose: a third-person view.  A row with a non-finite entry, or with
+        |dir| >= 105414350 (beyond the range the glibc-exact sin / cos are validated for), is skipped: its frame (and
+        depth) in that view is left as it is in `out` / `depth`.  No env state changes.
+        Returns frames [V, N, *frame] (or [N, *frame]) in the batch's observation layout -- `out` filled in place or a
+        fresh zero tensor -- and, when `depth` is True or an array / tensor float32 [V, N, H, W, 1] (or [N, H, W, 1])
+        to fill, (frames, depth).  With CUDA tensors throughout the call runs on torch's current stream without a
+        host sync."""
+        poses = self._view_rows("render_views", poses)
+        one = poses.ndim == 2 if isinstance(poses, np.ndarray) else poses.dim() == 2
+        V = 1 if one else int(poses.shape[0])
+        lead = () if one else (V,)
+        H, W = self.obs_height, self.obs_width
+        host = self.engine.host_memory
+        if out is None or depth is True:
+            torch = None if host else self._ensure_torch()
+            dev = None if host else torch.device("cuda", self.device)
+            zeros = (lambda shape, dt: np.zeros(shape, dt)) if host else \
+                (lambda shape, dt: torch.zeros(shape, dtype={np.uint8: torch.uint8, np.float64: torch.float64,
+                                                             np.float32: torch.float32}[dt], device=dev))
+            if out is None:
+                out = zeros(lead + self.obs_shape, self.obs_dtype)
+            if depth is True:
+                depth = zeros(lead + (self.num_envs, H, W, 1), np.float32)
+        for name, arr, shape, dt in (("out", out, lead + self.obs_shape, np.dtype(self.obs_dtype)),
+                                     ("depth", depth, lead + (self.num_envs, H, W, 1), np.dtype(np.float32))):
+            if arr is None or arr is False:
+                continue
+            adt = arr.dtype if isinstance(arr, np.ndarray) else np.dtype(str(arr.dtype).replace("torch.", ""))
+            contig = arr.flags["C_CONTIGUOUS"] if isinstance(arr, np.ndarray) else arr.is_contiguous()
+            if tuple(arr.shape) != shape or adt != dt or not contig:
+                raise ValueError("render_views: %s must be a contiguous %s array of shape %s, not %s %s" % (
+                    name, dt.name, shape, adt.name, tuple(arr.shape)))
+        if depth is False:
+            depth = None
+        stream = None if host else _torch_stream(self._ensure_torch(), self.device)
+        self.engine.render_views(poses, V, obs=out, depth=depth, render_agent=render_agent, stream=stream)
+        return out if depth is None else (out, depth)
 
     # ------------------------------------------------------------------ state views
     def get_state(self, **kw):

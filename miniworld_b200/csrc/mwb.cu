@@ -147,6 +147,7 @@ struct mwb_handle {
   bool obs_is_peer;               // this launch's observation buffer lives on another GPU (K2 stages whole frames)
   int k2_static_smem;             // static shared memory of the K2 instantiation in use (cudaFuncGetAttributes)
   TriRec* vis_tris;              // scratch of mwb_visible_ents, allocated on first use
+  double* d_view_rows;           // [N][3] staging of host rows for mwb_render_views / mwb_visible_ents_from, on first use
   ViewSpec view;                 // what the next render launch draws (agent camera unless mwb_render_top_view)
   int k2_parts;                   // blocks per env frame (1 at 80x60, 4 at 160x120)
 #ifndef MWB_HOSTSIM
@@ -417,8 +418,10 @@ template <int MSAA>
 static void hostsim_render_t(const DevState& S, const RenderAssets& A, const ViewSpec& view, uint8_t* obs, float* depth) {
   const int W = S.obs_w, H = S.obs_h;
   for (int i = 0; i < S.N; ++i) {
-    Camera cam = view.mode == 1 ? make_top_camera(S, i, view) : make_camera(S, i);
-    FrameMap fm = build_frame_map(S, i, view.mode == 1 && view.render_agent != 0);
+    if (view.mode == 2 && view_row_skipped(view.rows + (size_t)i * 3)) continue;   // like K2: the frame is left as it is
+    Camera cam = view.mode == 1 ? make_top_camera(S, i, view)
+               : view.mode == 2 ? make_row_camera(S, i, view.rows + (size_t)i * 3) : make_camera(S, i);
+    FrameMap fm = build_frame_map(S, i, view.mode != 0 && view.render_agent != 0);
     std::vector<TriRec> tris;
     TriRec rec;
     int seg;
@@ -538,7 +541,7 @@ static void hostsim_render(const DevState& S, const RenderAssets& A, const ViewS
   if (obs_out && fmt != MWB_OBS_HWC_U8) {
     const int W = S.obs_w, H = S.obs_h;
     for (int i = 0; i < S.N; ++i)
-      for (int y = 0; y < H; ++y)
+      for (int y = 0; y < H && !(view.mode == 2 && view_row_skipped(view.rows + (size_t)i * 3)); ++y)
         for (int x = 0; x < W; ++x) {
           const uint8_t* c = obs + (((size_t)i * H + y) * W + x) * 3;
           if (fmt == MWB_OBS_CWH_U8) {
@@ -577,22 +580,27 @@ static int k2_frame_stage_bytes(const mwb_handle* h) {
 }
 static int k2_smem_bytes(const mwb_handle* h) { return k2_list_bytes(h) + k2_frame_stage_bytes(h); }
 
-// K2's instantiations, one per block shape x MSAA count; they share one signature.  Block shape on H100 (DESIGN.md
+// K2's instantiations, one per block shape x MSAA count x camera kind (the agent's / the top view's, or designed
+// cameras: mwb_render_views); they share one signature.  Block shape on H100 (DESIGN.md
 // §3): 256 threads x 3 blocks / SM when one block renders a whole frame (K2 0.90 vs 1.04 ms for 4096 FourRooms envs
 // at 80x60), 320 x 3 when frames are split over several blocks (1.56 vs 1.64 ms for 512 PickupObjects envs at 160x120).
-typedef decltype(&render_kernel<1, 256, 3>) K2Kernel;
-static const K2Kernel k2_kernels[8] = {
-    render_kernel<1, 256, 3>, render_kernel<4, 256, 3>, render_kernel<8, 256, 3>, render_kernel<16, 256, 3>,
-    render_kernel<1, 320, 3>, render_kernel<4, 320, 3>, render_kernel<8, 320, 3>, render_kernel<16, 320, 3>};
+typedef decltype(&render_kernel<1, 256, 3, false>) K2Kernel;
+static const K2Kernel k2_kernels[16] = {
+    render_kernel<1, 256, 3, false>, render_kernel<4, 256, 3, false>, render_kernel<8, 256, 3, false>,
+    render_kernel<16, 256, 3, false>, render_kernel<1, 320, 3, false>, render_kernel<4, 320, 3, false>,
+    render_kernel<8, 320, 3, false>, render_kernel<16, 320, 3, false>,
+    render_kernel<1, 256, 3, true>, render_kernel<4, 256, 3, true>, render_kernel<8, 256, 3, true>,
+    render_kernel<16, 256, 3, true>, render_kernel<1, 320, 3, true>, render_kernel<4, 320, 3, true>,
+    render_kernel<8, 320, 3, true>, render_kernel<16, 320, 3, true>};
 static int k2_threads(const mwb_handle* h) { return h->k2_parts == 1 ? 256 : 320; }
 static int k2_index(const mwb_handle* h) {
   const int m = h->S.msaa;
-  return (h->k2_parts == 1 ? 0 : 4) + (m == 1 ? 0 : m == 4 ? 1 : m == 8 ? 2 : 3);
+  return (h->view.mode == 2 ? 8 : 0) + (h->k2_parts == 1 ? 0 : 4) + (m == 1 ? 0 : m == 4 ? 1 : m == 8 ? 2 : 3);
 }
 
 // The opt-in for large dynamic shared memory is an attribute of the kernel FUNCTION (per device), not of a
 // handle: several handles with different triangle capacities share it, so it is only ever raised.
-static int g_k2_smem[16][8] = {};
+static int g_k2_smem[16][16] = {};
 static int ensure_k2_smem(mwb_handle* h, int smem) {
   int& granted = g_k2_smem[h->cfg.device & 15][k2_index(h)];
   if (smem <= granted) return 0;
@@ -721,6 +729,7 @@ extern "C" int mwb_create(const mwb_config* cfg, mwb_handle** out) {
   h->mesh_bin_idx_buf = h->mesh_bin_off_buf = nullptr;
   memset(&h->view, 0, sizeof(ViewSpec));
   h->vis_tris = nullptr;
+  h->d_view_rows = nullptr;
   h->obs_format = MWB_OBS_HWC_U8;
   h->obs_px_bytes = 3;
   h->obs_peer_hint = -1;
@@ -2205,12 +2214,14 @@ static int launch_render(mwb_handle* h, uint8_t* obs, float* depth, stream_t s, 
 #ifndef MWB_HOSTSIM
   {
     const long long threads = (long long)h->S.N * (6 + 2 * h->S.E);
-    frame_trig_kernel<<<(unsigned)((threads + 127) / 128), 128, 0, s>>>(h->S);
+    if (h->view.mode == 2) frame_trig_kernel<true><<<(unsigned)((threads + 127) / 128), 128, 0, s>>>(h->S, h->view);
+    else frame_trig_kernel<false><<<(unsigned)((threads + 127) / 128), 128, 0, s>>>(h->S, h->view);
     h->launches++;
     CK(cudaGetLastError());
   }
   if (h->S.mesh_cap > 0) {
-    mesh_setup_kernel<<<dim3(h->S.N, h->S.E), 256, 0, s>>>(h->S, h->A, h->view);
+    if (h->view.mode == 2) mesh_setup_kernel<true><<<dim3(h->S.N, h->S.E), 256, 0, s>>>(h->S, h->A, h->view);
+    else mesh_setup_kernel<false><<<dim3(h->S.N, h->S.E), 256, 0, s>>>(h->S, h->A, h->view);
     h->launches++;
     CK(cudaGetLastError());
   }
@@ -2370,7 +2381,55 @@ extern "C" int mwb_render_top_view(mwb_handle* h, const double extents[4], int r
   return finish_outputs(h, obs, obs_host, nullptr, false, nullptr, nullptr, nullptr, s, stream != nullptr);
 }
 
-extern "C" int mwb_visible_ents(mwb_handle* h, uint32_t* mask, void* stream) {
+// Device rows of a designed view: `poses` itself, or its [N][3] block uploaded to the handle's staging (host rows).
+static const double* device_rows(mwb_handle* h, const double* poses, stream_t s) {
+  if (is_device_ptr(poses)) return poses;
+  if (!h->d_view_rows && alloc_arr(h, &h->d_view_rows, (size_t)h->S.N * 3)) return nullptr;
+  if (h2d(h->d_view_rows, poses, (size_t)h->S.N * 3 * sizeof(double), s) != 0) return nullptr;
+  return h->d_view_rows;
+}
+
+extern "C" int mwb_render_views(mwb_handle* h, const double* poses, int views, int render_agent, uint8_t* obs, float* depth,
+                                void* stream) {
+  if (!h || !poses || (!obs && !depth)) return fail(MWB_EINVAL, "null argument");
+  if (views <= 0) return fail(MWB_EINVAL, "views must be positive");
+  stream_t s = stream ? (stream_t)stream : h->stream;
+  if (stream_enter(h, s)) return MWB_ECUDA;
+  const size_t N = h->S.N, px = (size_t)h->S.obs_w * h->S.obs_h;
+  const size_t frame_bytes = N * px * h->obs_px_bytes, depth_bytes = N * px * sizeof(float);
+  const bool obs_host = obs && !is_device_ptr(obs), depth_host = depth && !is_device_ptr(depth);
+  int rc = MWB_OK;
+  for (int v = 0; v < views && rc == MWB_OK; ++v) {
+    uint8_t* obs_v = obs ? obs + (size_t)v * frame_bytes : nullptr;
+    float* depth_v = depth ? depth + (size_t)v * N * px : nullptr;
+    const double* rows = device_rows(h, poses + (size_t)v * N * 3, s);
+    if (!rows) { rc = fail(MWB_ECUDA, "row upload failed"); break; }
+    // host destinations: the staging starts as the caller's frames, so that skipped rows come back unchanged
+    if ((obs_host && h2d(h->d_obs, obs_v, frame_bytes, s) != 0) || (depth_host && h2d(h->d_depth, depth_v, depth_bytes, s) != 0)) {
+      rc = fail(MWB_ECUDA, "staging upload failed");
+      break;
+    }
+    h->view.mode = 2;
+    h->view.render_agent = render_agent != 0;
+    h->view.rows = rows;
+    rc = launch_render(h, obs ? (obs_host ? h->d_obs : obs_v) : nullptr, depth ? (depth_host ? h->d_depth : depth_v) : nullptr, s,
+                       obs_host ? obs_v : nullptr, depth_host ? depth_v : nullptr);
+    memset(&h->view, 0, sizeof(ViewSpec));
+    if (rc == MWB_OK && !h->frames_copied) {
+      if ((obs_host && d2h(obs_v, h->d_obs, frame_bytes, s) != 0) || (depth_host && d2h(depth_v, h->d_depth, depth_bytes, s) != 0))
+        rc = fail(MWB_ECUDA, "readback failed");
+    }
+    h->frames_copied = false;
+  }
+  if (rc) return rc;
+  if (stream_leave(h, s)) return MWB_ECUDA;
+  if (obs_host || depth_host || !stream)
+    if (sync_stream(s) != 0) return fail(MWB_ECUDA, "stream sync failed");
+  return MWB_OK;
+}
+
+// get_visible_ents from the agent's camera (rows null) or from designed cameras ([N][3] rows, device or host)
+static int visible_ents_impl(mwb_handle* h, const double* poses, uint32_t* mask, void* stream) {
   if (!h || !mask) return fail(MWB_EINVAL, "null argument");
   if (!h->have_protos) return fail(MWB_ESTATE, "protos not set");
   stream_t s = stream ? (stream_t)stream : h->stream;
@@ -2379,20 +2438,28 @@ extern "C" int mwb_visible_ents(mwb_handle* h, uint32_t* mask, void* stream) {
   if (!h->vis_tris && alloc_arr(h, &h->vis_tris, (size_t)N * cap)) return fail(MWB_ECUDA, "scratch allocation failed");
   const bool host = !is_device_ptr(mask);
   uint32_t* d_mask = host ? reinterpret_cast<uint32_t*>(h->d_ids) : mask;   // d_ids: N x int32 staging, free between calls
+  const double* rows = nullptr;
+  if (poses) {
+    rows = device_rows(h, poses, s);
+    if (!rows) return fail(MWB_ECUDA, "row upload failed");
+    // skipped rows leave their entries: the staging starts as the caller's mask
+    if (host && h2d(d_mask, mask, (size_t)N * sizeof(uint32_t), s) != 0) return fail(MWB_ECUDA, "staging upload failed");
+  }
 #ifndef MWB_HOSTSIM
   switch (h->S.msaa) {
-    case 1: visible_ents_kernel<1><<<N, 256, 0, s>>>(h->S, h->A, h->vis_tris, cap, box0, d_mask); break;
-    case 4: visible_ents_kernel<4><<<N, 256, 0, s>>>(h->S, h->A, h->vis_tris, cap, box0, d_mask); break;
-    case 16: visible_ents_kernel<16><<<N, 256, 0, s>>>(h->S, h->A, h->vis_tris, cap, box0, d_mask); break;
-    default: visible_ents_kernel<8><<<N, 256, 0, s>>>(h->S, h->A, h->vis_tris, cap, box0, d_mask); break;
+    case 1: visible_ents_kernel<1><<<N, 256, 0, s>>>(h->S, h->A, h->vis_tris, cap, box0, d_mask, rows); break;
+    case 4: visible_ents_kernel<4><<<N, 256, 0, s>>>(h->S, h->A, h->vis_tris, cap, box0, d_mask, rows); break;
+    case 16: visible_ents_kernel<16><<<N, 256, 0, s>>>(h->S, h->A, h->vis_tris, cap, box0, d_mask, rows); break;
+    default: visible_ents_kernel<8><<<N, 256, 0, s>>>(h->S, h->A, h->vis_tris, cap, box0, d_mask, rows); break;
   }
   h->launches++;
   CK(cudaGetLastError());
 #else
   const int W = h->S.obs_w, H = h->S.obs_h, M = h->S.msaa;
   for (int i = 0; i < N; ++i) {
+    if (rows && view_row_skipped(rows + (size_t)i * 3)) continue;
     TriRec* tris = h->vis_tris + (size_t)i * cap;
-    const Camera cam = make_camera(h->S, i);
+    const Camera cam = rows ? make_row_camera(h->S, i, rows + (size_t)i * 3) : make_camera(h->S, i);
     int ent_slot[32];
     const int n_query = queried_entities(h->S, i, ent_slot);
     int n_room = 0;
@@ -2429,6 +2496,13 @@ extern "C" int mwb_visible_ents(mwb_handle* h, uint32_t* mask, void* stream) {
     if (sync_stream(s) != 0) return fail(MWB_ECUDA, "stream sync failed");
   }
   return MWB_OK;
+}
+
+extern "C" int mwb_visible_ents(mwb_handle* h, uint32_t* mask, void* stream) { return visible_ents_impl(h, nullptr, mask, stream); }
+
+extern "C" int mwb_visible_ents_from(mwb_handle* h, const double* poses, uint32_t* mask, void* stream) {
+  if (!poses) return fail(MWB_EINVAL, "null argument");
+  return visible_ents_impl(h, poses, mask, stream);
 }
 
 // ------------------------------------------------------------------ ABI: snapshot / restore

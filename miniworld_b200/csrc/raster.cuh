@@ -103,7 +103,10 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 
 // ---- per-frame trigonometry: thread (env i, k): k < 6 the camera's cos / sin, else entity slot (k - 6) / 2 -----------
-__global__ void frame_trig_kernel(DevState S) {
+// (VIEWS: the launch draws designed cameras, view.mode 2, and the heading comes from env i's row.  The designed-camera
+// path is a separate instantiation of this kernel, the mesh pre-pass and K2, so the agent-camera code is unchanged.)
+template <bool VIEWS>
+__global__ void frame_trig_kernel(DevState S, ViewSpec view) {
   const int per = 6 + 2 * S.E;
   const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (g >= (long long)S.N * per) return;
@@ -112,6 +115,10 @@ __global__ void frame_trig_kernel(DevState S) {
   if (k < 6) {
     double ang[3];
     camera_angles(S, i, ang);
+    if (VIEWS) {
+      if (view_row_skipped(view.rows + (size_t)i * 3)) return;      // no camera for a skipped row
+      ang[0] = view.rows[(size_t)i * 3 + 2];
+    }
     S.cam_trig[(size_t)k * N + i] = (k & 1) ? mwb_libm::sin_glibc(ang[k >> 1]) : mwb_libm::cos_glibc(ang[k >> 1]);
     return;
   }
@@ -125,6 +132,7 @@ __global__ void frame_trig_kernel(DevState S) {
 }
 
 // ---- mesh pre-pass: block (env i, entity slot e) sets up that entity's triangles ----------
+template <bool VIEWS>
 __global__ void __launch_bounds__(256) mesh_setup_kernel(DevState S, RenderAssets A, ViewSpec view) {
   const int i = blockIdx.x, e = blockIdx.y;
   const size_t N = S.N;
@@ -133,6 +141,7 @@ __global__ void __launch_bounds__(256) mesh_setup_kernel(DevState S, RenderAsset
   __shared__ int box[4];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   MeshSegInfo* info = S.mesh_seg + (size_t)i * S.E + e;
+  if (VIEWS && view_row_skipped(view.rows + (size_t)i * 3)) return;   // K2 skips this env's frame too
   const int p = e == S.ghost_slot[i] ? S.ghost_proto[i] : (e < S.num_slots[i] ? S.ent_proto[e * N + i] : -1);
   if (p < 0 || S.protos[p].kind != MWB_KIND_MESH) {
     if (tid == 0) info->count = 0;
@@ -144,7 +153,7 @@ __global__ void __launch_bounds__(256) mesh_setup_kernel(DevState S, RenderAsset
     } else {
       double trig[6];
       for (int k = 0; k < 6; ++k) trig[k] = S.cam_trig[(size_t)k * N + i];
-      cam = make_camera(S, i, trig);
+      cam = VIEWS ? make_view_camera(S, i, view, trig) : make_camera(S, i, trig);
     }
     box[0] = box[1] = 0x7fffffff;
     box[2] = box[3] = -1;
@@ -285,7 +294,7 @@ __global__ void depth_lut_kernel(float* __restrict__ lut) {
 // ---- K2 --------------------------------------------------------------------------------
 // THREADS x MINB: block size and resident blocks per SM the kernel is compiled for.  Warps claim half-tiles from a
 // shared counter instead of striding, which evens out the per-warp work.
-template <int MSAA, int THREADS, int MINB>
+template <int MSAA, int THREADS, int MINB, bool VIEWS>
 __global__ void __launch_bounds__(THREADS, MINB)
 render_kernel(DevState S, RenderAssets A, ViewSpec view, int fmt, uint8_t* __restrict__ obs, float* __restrict__ depth, int env0,
               int parts, int tri_cap, int stage_bytes, int frame_stage_bytes, K2Layout lay, int* __restrict__ overflow) {
@@ -294,6 +303,8 @@ render_kernel(DevState S, RenderAssets A, ViewSpec view, int fmt, uint8_t* __res
   // large frames are cut into `parts` blocks per env (each redoes the cheap geometry phase and
   // rasterises its share of the half-tiles), which evens out the load when few envs are resident
   const int i = env0 + (int)blockIdx.x / parts, part = (int)blockIdx.x % parts;
+  // a skipped row of a designed view: the whole block leaves before any barrier (the condition is the block's env's)
+  if (VIEWS && view_row_skipped(view.rows + (size_t)i * 3)) return;
   // set-up triangles of rooms + boxes: shared memory, or this env's HBM block for big levels (per level: the
   // env's own capacity bounds its list; tri_cap, the largest level's, is the stride of the HBM blocks)
   const LevelDev& lv = env_level_of(S, i);
@@ -348,10 +359,10 @@ render_kernel(DevState S, RenderAssets A, ViewSpec view, int fmt, uint8_t* __res
       double tr[6];
 #pragma unroll
       for (int k = 0; k < 6; ++k) tr[k] = S.cam_trig[(size_t)k * S.N + i];
-      cam = make_camera(S, i, tr);
+      cam = VIEWS ? make_view_camera(S, i, view, tr) : make_camera(S, i, tr);
     }
   } else if (tid == 32) {
-    fmap = build_frame_map(S, i, view.mode == 1 && view.render_agent != 0);   // meanwhile another warp lays out the draw list
+    fmap = build_frame_map(S, i, (VIEWS || view.mode == 1) && view.render_agent != 0);   // meanwhile another warp lays out the draw list
   } else if (tid >= 64 && tid < 64 + 2 * MWB_MAX_DRAWN) {
     // ... and the (cos, sin) of every entity slot's model rotation, for the twelve triangle tasks of each Box
     const int e = (tid - 64) >> 1;

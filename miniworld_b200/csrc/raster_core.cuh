@@ -107,14 +107,29 @@ struct Camera {
   float osx, otx, osy, oty;      // x_clip = osx x + otx, y_clip = osy (-z) + oty, z_clip = -0.01 y, w = 1
 };
 
-// Which view a render launch draws: the agent's camera (render_obs, miniworld.py:1177-1221) or the
+// Which view a render launch draws: the agent's camera (render_obs, miniworld.py:1177-1221), the
 // orthographic map of render_top_view (miniworld.py:1088-1175): glOrtho(l, r, b, t, -100, 100) under
-// the model-view that maps world (x, y, z) to eye (x, -z, y), plus the agent's marker triangle.
+// the model-view that maps world (x, y, z) to eye (x, -z, y), plus the agent's marker triangle, or a
+// designed camera (mwb_render_views): render_obs with the agent moved to env i's row (x, z, dir) of `rows`.
 struct ViewSpec {
-  int mode;                      // 0 = agent camera, 1 = top view
-  int render_agent;              // top view: draw Agent.render()'s triangle (entity.py:518-539)
-  double l, r, b, t;             // glOrtho extents (top view)
+  int mode;                      // 0 = agent camera, 1 = top view, 2 = designed camera
+  int render_agent;              // top view / designed camera: draw Agent.render()'s triangle (entity.py:518-539)
+  union {
+    struct { double l, r, b, t; };   // glOrtho extents (top view)
+    const double* rows;              // designed camera: [N][3] rows (x, z, dir) of the current view
+  };
 };
+
+// Largest |heading| a designed camera takes: the range the glibc-exact sin / cos are validated for
+// (libm_sincos.cuh); beyond it their table index is meaningless.
+#define MWB_VIEW_MAX_DIR 105414350.0
+
+// designed camera: a row with a non-finite entry or |dir| >= MWB_VIEW_MAX_DIR is skipped (its frame is left as it
+// is; no trig is evaluated for it).  x * 0 + z * 0 is +-0 when both are finite and NaN otherwise, so |dir| plus it is
+// |dir| exactly or NaN, and one comparison (false for NaN) covers the row: K2's default path keeps its spill count.
+MWB_DEV bool view_row_skipped(const double* row) {
+  return !(fabs(row[2]) + (row[0] * 0.0 + row[1] * 0.0) < MWB_VIEW_MAX_DIR);
+}
 
 // The three camera angles of env i (heading, pitch, half the vertical field of view), float64.
 MWB_DEV void camera_angles(const DevState& S, int i, double ang[3]) {
@@ -148,10 +163,9 @@ MWB_DEV void camera_common(const DevState& S, int i, Camera& c) {
 // sin / cos so that the oracle, fed the same (pos, dir, cam_*) doubles on the host, derives the
 // identical float32 basis.  (The six evaluations are independent: the kernel spreads them over
 // six threads.)
-MWB_DEV Camera make_camera(const DevState& S, int i, const double trig[6]) {
+// The agent at (px, py, pz); every camera parameter is env i's.
+MWB_DEV Camera make_camera_at(const DevState& S, int i, double px, double py, double pz, const double trig[6]) {
   const size_t N = S.N;
-  const int as = S.agent_slot[i];
-  double px = S.ent_px[as * N + i], py = S.ent_py[as * N + i], pz = S.ent_pz[as * N + i];
   double h = S.cam[0 * N + i], fd = S.cam[1 * N + i];
   const double ct = trig[0], st = trig[1], cp = trig[2], sp = trig[3];
   Camera c;
@@ -178,6 +192,29 @@ MWB_DEV Camera make_camera(const DevState& S, int i, const double trig[6]) {
   return c;
 }
 
+MWB_DEV Camera make_camera(const DevState& S, int i, const double trig[6]) {
+  const size_t N = S.N;
+  const int as = S.agent_slot[i];
+  const double px = S.ent_px[as * N + i], py = S.ent_py[as * N + i], pz = S.ent_pz[as * N + i];
+  return make_camera_at(S, i, px, py, pz, trig);
+}
+
+// The perspective camera of a render launch (view.mode 0 or 2) from the trig frame_trig_kernel evaluated: the
+// agent's eye, or the eye at env i's row
+MWB_DEV Camera make_view_camera(const DevState& S, int i, const ViewSpec& view, const double trig[6]) {
+  const size_t N = S.N;
+  const int as = S.agent_slot[i];
+  double px, pz;
+  if (view.mode == 2) {
+    px = view.rows[(size_t)i * 3];
+    pz = view.rows[(size_t)i * 3 + 1];
+  } else {
+    px = S.ent_px[as * N + i];
+    pz = S.ent_pz[as * N + i];
+  }
+  return make_camera_at(S, i, px, S.ent_py[as * N + i], pz, trig);
+}
+
 // render_top_view's camera: the projection matrix entries are formed in float64 and rounded once, as
 // glOrtho's GLdouble arguments end up in a float32 matrix.
 MWB_DEV Camera make_top_camera(const DevState& S, int i, const ViewSpec& v) {
@@ -202,6 +239,20 @@ MWB_DEV Camera make_camera(const DevState& S, int i) {
     trig[2 * k + 1] = mwb_libm::sin_glibc(ang[k]);
   }
   return make_camera(S, i, trig);
+}
+
+// The designed camera of env i, `row` = (x, z, dir): the agent's camera after agent.pos = (x, agent.pos[1], z),
+// agent.dir = dir -- the same float64 steps, so a row equal to the agent's pose gives the identical basis.
+MWB_DEV Camera make_row_camera(const DevState& S, int i, const double* row) {
+  double ang[3], trig[6];
+  camera_angles(S, i, ang);
+  ang[0] = row[2];
+  for (int k = 0; k < 3; ++k) {
+    trig[2 * k] = mwb_libm::cos_glibc(ang[k]);
+    trig[2 * k + 1] = mwb_libm::sin_glibc(ang[k]);
+  }
+  const int as = S.agent_slot[i];
+  return make_camera_at(S, i, row[0], S.ent_py[as * (size_t)S.N + i], row[1], trig);
 }
 
 // vertex after the exact part of the pipeline: window-homogeneous position + z numerator

@@ -590,6 +590,16 @@ class MiniWorldEnv(gym.Env):
         self._push_world()
         return {e for e in eng.visible_ents() if any(e is x for x in self.entities)}
 
+    def render_view(self, x, z, dir, render_agent=False):
+        """(rgb uint8[H, W, 3], depth float32[H, W, 1]) from a designed camera: what render_obs() / render_depth()
+        return after agent.pos = (x, agent.pos[1], z), agent.dir = dir, without changing the agent.
+        `render_agent=True` also draws the agent's marker triangle at its real pose (a third-person view)."""
+        if not (math.isfinite(x) and math.isfinite(z) and abs(dir) < 105414350.0):
+            raise ValueError("render_view needs a finite x, z and |dir| < 105414350, got (%r, %r, %r)" % (x, z, dir))
+        eng = self._require_engine()
+        self._push_world()
+        return eng.render_view((float(x), float(z), float(dir)), render_agent)
+
     def _require_vis_engine(self):
         if self.device is None:
             raise RuntimeError("MiniWorldEnv was built with device=None (world generation only)")
