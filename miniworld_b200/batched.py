@@ -32,6 +32,8 @@ Per-environment semantics are exactly those of the reference's `MiniWorldEnv.res
 Outputs are torch CUDA tensors by default (zero-copy from the kernels); `step_host`
 performs the same step with pinned host buffers for callers that want numpy.
 """
+from collections import namedtuple
+
 import numpy as np
 
 from . import pack
@@ -168,23 +170,44 @@ def default_env_level(num_envs, n_levels):
     return np.repeat(np.arange(n_levels, dtype=np.int32), [base + (1 if k < extra else 0) for k in range(n_levels)])
 
 
+# The run-time modes, in the order the constructor turns them on (the state bank last: its record layout depends on the
+# other modes).  `flag`: the constructor argument and attribute (Engine.enable_<flag> turns the mode on, except
+# enable_level_changes); `arrays`: the state arrays it adds, whose accessors raise RuntimeError(`missing`) on a batch
+# without it; `host_reset`: the TypeError of a batch without device resets (None where an earlier check refuses
+# one: level changes need a sequence of levels, maze layouts device Maze templates); `info`: (key, array) pairs.
+_Mode = namedtuple("_Mode", "flag arrays missing host_reset info")
+_MODES = (
+    _Mode("dynamic_levels", ("env_level", "next_level", "level_weights"),
+          "levels are fixed in this batch: construct it with dynamic_levels=True", None, [("level", "env_level")]),
+    _Mode("episode_seeds", ("next_seed", "episode_seed"),
+          "this batch has no episode seeds: construct it with episode_seeds=True",
+          "episode seeds are taken by device resets; host-reset levels keep RNG streams in Python",
+          [("seed", "episode_seed")]),
+    _Mode("maze_layouts", ("next_maze", "next_maze_cells", "maze_pending", "episode_maze"),
+          "this batch has no maze layouts: construct it with maze_layouts=True", None, [("maze", "episode_maze")]),
+    _Mode("start_poses", ("next_pose", "next_agent_pose", "pose_pending", "episode_start"),
+          "this batch has no start poses: construct it with start_poses=True",
+          "start poses are taken by device resets; host-reset levels place entities in Python "
+          "(reset(options={\"poses\": ...}) of the level itself)", [("start", "episode_start")]),
+    _Mode("reset_draws", ("next_draws", "draws_pending", "episode_draws"),
+          "this batch has no reset draws: construct it with reset_draws=True",
+          "reset draws are taken by device resets; host-reset levels draw in Python "
+          "(reset(options={\"draws\": ...}) of the level itself)", [("draws", "episode_draws")]),
+    _Mode("goal_distance", ("goal_dist", "expert_action", "episode_shortest", "goal_field"),
+          "this batch has no goal distance: construct it with goal_distance=True",
+          "goal distance is built by device resets; host-reset levels build their worlds in Python "
+          "(MiniWorldEnv.goal_distance() of the level itself)",
+          [("goal_dist", "goal_dist"), ("shortest", "episode_shortest")]),
+    _Mode("state_bank", ("next_state", "episode_state", "bank_level"),
+          "this batch has no state bank: construct it with state_bank=K",
+          "the state bank loads states at device resets; host-reset levels keep their worlds and RNG streams in Python",
+          [("state", "episode_state")]),
+)
+
 # the flag a run-time array needs, and what its accessor raises on a batch built without it
-_NEEDS = {**dict.fromkeys(("env_level", "next_level", "level_weights"), (
-              "dynamic_levels", RuntimeError, "levels are fixed in this batch: construct it with dynamic_levels=True")),
-          **dict.fromkeys(("next_seed", "episode_seed"), (
-              "episode_seeds", RuntimeError, "this batch has no episode seeds: construct it with episode_seeds=True")),
-          **dict.fromkeys(("next_maze", "next_maze_cells", "maze_pending", "episode_maze"), (
-              "maze_layouts", RuntimeError, "this batch has no maze layouts: construct it with maze_layouts=True")),
-          **dict.fromkeys(("next_pose", "next_agent_pose", "pose_pending", "episode_start"), (
-              "start_poses", RuntimeError, "this batch has no start poses: construct it with start_poses=True")),
-          **dict.fromkeys(("next_draws", "draws_pending", "episode_draws"), (
-              "reset_draws", RuntimeError, "this batch has no reset draws: construct it with reset_draws=True")),
-          **dict.fromkeys(("next_state", "episode_state", "bank_level"), (
-              "state_bank", RuntimeError, "this batch has no state bank: construct it with state_bank=K")),
-          **dict.fromkeys(("goal_dist", "expert_action", "episode_shortest", "goal_field"), (
-              "goal_distance", RuntimeError, "this batch has no goal distance: construct it with goal_distance=True")),
-          "level_params": ("device_reset", TypeError, "level params change at device resets; host-reset levels draw "
-                           "theirs in Python (set them on the level's own DomainParams)")}
+_NEEDS = {name: (m.flag, RuntimeError, m.missing) for m in _MODES for name in m.arrays}
+_NEEDS["level_params"] = ("device_reset", TypeError, "level params change at device resets; host-reset levels draw "
+                          "theirs in Python (set them on the level's own DomainParams)")
 
 
 class _Views(dict):
@@ -311,23 +334,19 @@ class BatchedMiniWorld:
                  msaa_samples=8, device=0, want_depth=False, level_kwargs=None, obs_format="hwc", env_level=None,
                  dynamic_levels=False, level_seed=0, env_offset=0, per_env_worlds=False, episode_seeds=False,
                  maze_layouts=False, start_poses=False, state_bank=None, reset_draws=False, goal_distance=False):
+        given = locals()
         self.num_envs = int(num_envs)
         self.obs_width, self.obs_height = int(obs_width), int(obs_height)
         self.domain_rand = bool(domain_rand)
         self.want_depth = bool(want_depth)
         self.device = int(device)
-        self.dynamic_levels = bool(dynamic_levels)
         self.per_env_worlds = bool(per_env_worlds)
-        self.episode_seeds = bool(episode_seeds)
-        self.maze_layouts = bool(maze_layouts)
-        self.start_poses = bool(start_poses)
-        self.reset_draws = bool(reset_draws)
-        self.goal_distance = bool(goal_distance)
         if state_bank is not None and (isinstance(state_bank, bool) or not isinstance(state_bank, (int, np.integer))
                                        or state_bank < 1):
             raise ValueError("state_bank is a number of slots >= 1, got %r" % (state_bank,))
         self.bank_slots = int(state_bank or 0)
-        self.state_bank = self.bank_slots > 0
+        for m in _MODES:
+            setattr(self, m.flag, bool(given[m.flag]))
         table = isinstance(level, (list, tuple))
         if table:
             defs = self._init_levels(list(level), level_kwargs, env_level)
@@ -343,44 +362,28 @@ class BatchedMiniWorld:
         if self.maze_layouts:
             self._size_for_layouts(defs)
         self._init_engine(defs, table, msaa_samples, autoreset)
-        self._view_map = _Views(self.engine, self.device, dict(
-            dynamic_levels=self.dynamic_levels, episode_seeds=self.episode_seeds, maze_layouts=self.maze_layouts,
-            start_poses=self.start_poses, state_bank=self.state_bank, reset_draws=self.reset_draws,
-            goal_distance=self.goal_distance, device_reset=self.device_reset),
-            getattr(self, "maze_shape", None))
-        if self.dynamic_levels:
-            self.level_seed, self.env_offset = int(level_seed), int(env_offset)
-            self.engine.enable_level_changes(self.level_seed, self.env_offset)
-        if self.episode_seeds:
-            if not self.device_reset:
+        flags = {m.flag: getattr(self, m.flag) for m in _MODES}
+        self._view_map = _Views(self.engine, self.device, dict(flags, device_reset=self.device_reset),
+                                getattr(self, "maze_shape", None))
+        for m in _MODES:
+            if not flags[m.flag]:
+                continue
+            if m.host_reset is not None and not self.device_reset:
                 self.engine.close()
-                raise TypeError("episode seeds are taken by device resets; host-reset levels keep RNG streams in Python")
-            self.engine.enable_episode_seeds()
-        if self.maze_layouts:
-            self.engine.enable_maze_layouts()
-        if self.start_poses:
-            if not self.device_reset:
+                raise TypeError(m.host_reset)
+            if m.flag == "dynamic_levels":
+                self.level_seed, self.env_offset = int(level_seed), int(env_offset)
+                self.engine.enable_level_changes(self.level_seed, self.env_offset)
+            elif m.flag == "reset_draws" and not any(self.draw_specs):
                 self.engine.close()
-                raise TypeError("start poses are taken by device resets; host-reset levels place entities in Python "
-                                "(reset(options={\"poses\": ...}) of the level itself)")
-            self.engine.enable_start_poses()
-        if self.reset_draws:
-            if not self.device_reset:
-                self.engine.close()
-                raise TypeError("reset draws are taken by device resets; host-reset levels draw in Python "
-                                "(reset(options={\"draws\": ...}) of the level itself)")
-            if not any(self.draw_specs):
-                self.engine.close()
-                raise ValueError("reset_draws needs a level with a reset draw; %s make none" % ", ".join(self.level_ids))
-            self.engine.enable_reset_draws()
-        if self.goal_distance:
-            self._enable_goal_distance(defs)
-        if self.state_bank:
-            if not self.device_reset:
-                self.engine.close()
-                raise TypeError("the state bank loads states at device resets; host-reset levels keep their worlds and "
-                                "RNG streams in Python")
-            self.engine.enable_state_bank(self.bank_slots)     # last: the record layout depends on the other modes
+                raise ValueError("reset_draws needs a level with a reset draw; %s make none"
+                                 % ", ".join(self.level_ids))
+            elif m.flag == "goal_distance":
+                self._enable_goal_distance(defs)
+            elif m.flag == "state_bank":
+                self.engine.enable_state_bank(self.bank_slots)
+            else:
+                getattr(self.engine, "enable_" + m.flag)()
         # observation layout written by the render kernel: the reference's PyTorchObsWrapper ("cwh") and
         # GreyscaleWrapper ("grey") are fused into its epilogue instead of running as separate passes
         self.obs_format = obs_format
@@ -398,10 +401,6 @@ class BatchedMiniWorld:
         """goal_distance=True: one grid per level from its definition instance (navigation.level_grid), goal slot -1 at
         levels without a goal rule."""
         from .navigation import level_grid
-        if not self.device_reset:
-            self.engine.close()
-            raise TypeError("goal distance is built by device resets; host-reset levels build their worlds in Python "
-                            "(MiniWorldEnv.goal_distance() of the level itself)")
         grids = np.zeros(len(defs), GOAL_GRID_DTYPE)
         grids["goal_slot"] = -1
         for l, d in enumerate(defs):
@@ -590,32 +589,11 @@ class BatchedMiniWorld:
                 elif spec[0] == "entity_pos":              # TMaze: info["goal_pos"] = self.box.pos (tmaze.py:89)
                     self._info_views[key] = (int(spec[1]), [self._views()[n] for n in ("ent_x", "ent_y", "ent_z")])
             self._obs_dict = dict(self._device_obs_extra)
-            if self.dynamic_levels:
-                # the level of each env's current episode (after a terminating step still the one that just ended)
-                self._info["level"] = self.level_tensor
-            if self.episode_seeds:
-                # the seed each env's current episode started from (after a terminating step still the ended one's)
-                self._info["seed"] = self.episode_seed
-            if self.maze_layouts:
-                # the layout of each env's current episode (after a terminating step still the ended one's)
-                self._info["maze"] = self.episode_maze
-            if self.start_poses:
-                # the agent's (x, z, dir) at the start of each env's current episode (after a terminating step still
-                # the ended one's)
-                self._info["start"] = self.episode_start
-            if self.reset_draws:
-                # the outcome of every reset draw of each env's current episode (after a terminating step still the
-                # ended one's)
-                self._info["draws"] = self.episode_draws
-            if self.goal_distance:
-                # the agent's geodesic distance to the goal now, and the shortest path of each env's current episode
-                # (after a terminating step still the ended one's)
-                self._info["goal_dist"] = self.goal_dist
-                self._info["shortest"] = self.episode_shortest
-            if self.state_bank:
-                # the slot each env's current episode was loaded from, -1 for none (after a terminating step still the
-                # ended one's)
-                self._info["state"] = self.episode_state
+            # what each mode records of every env's current episode (after a terminating step still of the one that
+            # just ended: its level, seed, maze, start pose, draws, shortest path and loaded slot), and goal_dist now
+            for m in _MODES:
+                if getattr(self, m.flag):
+                    self._info.update((key, self._views()[name]) for key, name in m.info)
         return self._torch
 
     # ------------------------------------------------------------------ run-time arrays

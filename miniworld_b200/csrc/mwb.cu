@@ -1357,6 +1357,51 @@ extern "C" int mwb_set_levels(mwb_handle* h, int n_levels, const mwb_level* leve
   return MWB_OK;
 }
 
+// The run-time modes with a bit in the snapshot mark (level changes have base marks of their own, kSnapMagic...): how
+// a handle shows the mode on, and the words its enable call, mwb_state_array and snapshot_mode use for it.  Episode
+// seeds write the mode letter in lower case ("MWBs", "MWBl", "MWBw", "MWBx"), maze layouts the "B" ("MWbS", ...), start
+// poses the "W" and the state bank the "M"; reset draws set the high bit of the mode letter and goal distance that of
+// the "M" (every letter's case bit already names a mode).
+struct ModeBit {
+  uint32_t bit;
+  const char* name;      // as snapshot_mode prints it; mwb_enable_<name, '_' for ' '> turns the mode on
+  const char* subject;   // as the refusals name it, with its verb
+  bool (*on)(const DevState& S);
+};
+enum Mode { kSeeds, kMazes, kPoses, kBank, kDraws, kNav };
+static const ModeBit kModeBits[] = {
+    {0x20000000u, "episode seeds", "episode seeds are", [](const DevState& S) { return S.next_seed != nullptr; }},
+    {0x00200000u, "maze layouts", "maze layouts are", [](const DevState& S) { return S.layouts != nullptr; }},
+    {0x00002000u, "start poses", "start poses are", [](const DevState& S) { return S.poses != nullptr; }},
+    {0x00000020u, "state bank", "the state bank is", [](const DevState& S) { return S.bank != nullptr; }},
+    {0x80000000u, "reset draws", "reset draws are", [](const DevState& S) { return S.draws != nullptr; }},
+    {0x00000080u, "goal distance", "goal distance is", [](const DevState& S) { return S.nav != nullptr; }},
+};
+
+// The checks every enable call but mwb_enable_level_changes starts with, in this order: a handle, the mode off, the
+// state bank off unless the mode is goal distance (the bank's record layout depends on the other modes) and device
+// resets (`no_resets` says why the mode needs them).
+static int enable_prologue(mwb_handle* h, Mode m, const char* no_resets) {
+  if (!h) return fail(MWB_EINVAL, "null handle");
+  const ModeBit& b = kModeBits[m];
+  if (b.on(h->S)) return fail(MWB_ESTATE, std::string(b.subject) + " already on");
+  if (m != kNav && h->S.bank)
+    return fail(MWB_ESTATE,
+                std::string(b.name) + " cannot be turned on once the state bank is on (its record layout depends on it)");
+  if (!h->have_params || !h->S.ops) return fail(MWB_ESTATE, no_resets);
+  return MWB_OK;
+}
+
+// A device copy of the host record `rec` of a mode (uploaded on the handle's stream, synchronised) -> *out
+template <class T>
+static int publish_record(mwb_handle* h, const T& rec, const T** out, const char* alloc_failed) {
+  T* d = nullptr;
+  if (alloc_arr(h, &d, 1)) return fail(MWB_ECUDA, alloc_failed);
+  if (h2d(d, &rec, sizeof(T), h->stream) != 0 || sync_stream(h->stream) != 0) return fail(MWB_ECUDA, "upload failed");
+  *out = d;
+  return MWB_OK;
+}
+
 // The run-time control arrays a mode's enable call adds: with the handle drained, each of `bytes` bytes, zeros or, where
 // `minus_one`, all -1 (0xFF bytes).  `what` names the mode in the allocation error.
 struct ControlArray {
@@ -1397,12 +1442,10 @@ extern "C" int mwb_enable_level_changes(mwb_handle* h, uint64_t seed, int32_t en
 }
 
 extern "C" int mwb_enable_episode_seeds(mwb_handle* h) {
-  if (!h) return fail(MWB_EINVAL, "null handle");
-  if (h->S.next_seed) return fail(MWB_ESTATE, "episode seeds are already on");
-  if (h->S.bank) return fail(MWB_ESTATE, "episode seeds cannot be turned on once the state bank is on (its record layout depends on it)");
-  if (!h->have_params || !h->S.ops)
-    return fail(MWB_ESTATE, "episode seeds need device resets (params and a reset program: mwb_set_levels, or "
-                            "mwb_set_params and mwb_set_program); host-generated worlds keep their streams on the host");
+  if (int rc = enable_prologue(h, kSeeds, "episode seeds need device resets (params and a reset program: "
+                                          "mwb_set_levels, or mwb_set_params and mwb_set_program); host-generated "
+                                          "worlds keep their streams on the host"))
+    return rc;
   DevState& S = h->S;
   void *next, *episode;
   int rc = alloc_control_arrays(h, "episode-seed", {{&next, S.N * sizeof(int64_t), true},
@@ -1524,12 +1567,9 @@ extern "C" int mwb_set_level_maze(mwb_handle* h, int level, const mwb_maze_desc*
 }
 
 extern "C" int mwb_enable_maze_layouts(mwb_handle* h) {
-  if (!h) return fail(MWB_EINVAL, "null handle");
-  if (h->S.layouts) return fail(MWB_ESTATE, "maze layouts are already on");
-  if (h->S.bank) return fail(MWB_ESTATE, "maze layouts cannot be turned on once the state bank is on (its record layout depends on it)");
-  if (!h->have_params || !h->S.ops)
-    return fail(MWB_ESTATE, "maze layouts need device resets (mwb_set_maze or mwb_set_level_maze on a handle with a "
-                            "reset program); host-generated worlds are built on the host");
+  if (int rc = enable_prologue(h, kMazes, "maze layouts need device resets (mwb_set_maze or mwb_set_level_maze on a "
+                                          "handle with a reset program); host-generated worlds are built on the host"))
+    return rc;
   DevState& S = h->S;
   int rows = 0, cols = 0;
   std::vector<int32_t> quads(h->level_quads);
@@ -1564,20 +1604,14 @@ extern "C" int mwb_enable_maze_layouts(mwb_handle* h) {
   Y.episode = (uint8_t*)episode;
   Y.rows = rows;
   Y.cols = cols;
-  MazeLayouts* d = nullptr;
-  if (alloc_arr(h, &d, 1)) return fail(MWB_ECUDA, "maze layout state allocation failed");
-  if (h2d(d, &Y, sizeof(Y), h->stream) != 0 || sync_stream(h->stream) != 0) return fail(MWB_ECUDA, "upload failed");
-  S.layouts = d;
-  return MWB_OK;
+  return publish_record(h, Y, &S.layouts, "maze layout state allocation failed");
 }
 
 extern "C" int mwb_enable_start_poses(mwb_handle* h) {
-  if (!h) return fail(MWB_EINVAL, "null handle");
-  if (h->S.poses) return fail(MWB_ESTATE, "start poses are already on");
-  if (h->S.bank) return fail(MWB_ESTATE, "start poses cannot be turned on once the state bank is on (its record layout depends on it)");
-  if (!h->have_params || !h->S.ops)
-    return fail(MWB_ESTATE, "start poses need device resets (params and a reset program: mwb_set_levels, or "
-                            "mwb_set_params and mwb_set_program); host-generated worlds are placed on the host");
+  if (int rc = enable_prologue(h, kPoses, "start poses need device resets (params and a reset program: "
+                                          "mwb_set_levels, or mwb_set_params and mwb_set_program); host-generated "
+                                          "worlds are placed on the host"))
+    return rc;
   DevState& S = h->S;
   const size_t N = S.N, E = S.E;
   void *next, *next_agent, *pending, *episode;
@@ -1591,20 +1625,14 @@ extern "C" int mwb_enable_start_poses(mwb_handle* h) {
   P.next_agent = (double*)next_agent;
   P.pending = (uint8_t*)pending;
   P.episode = (double*)episode;
-  StartPoses* d = nullptr;
-  if (alloc_arr(h, &d, 1)) return fail(MWB_ECUDA, "start pose state allocation failed");
-  if (h2d(d, &P, sizeof(P), h->stream) != 0 || sync_stream(h->stream) != 0) return fail(MWB_ECUDA, "upload failed");
-  S.poses = d;
-  return MWB_OK;
+  return publish_record(h, P, &S.poses, "start pose state allocation failed");
 }
 
 extern "C" int mwb_enable_reset_draws(mwb_handle* h) {
-  if (!h) return fail(MWB_EINVAL, "null handle");
-  if (h->S.draws) return fail(MWB_ESTATE, "reset draws are already on");
-  if (h->S.bank) return fail(MWB_ESTATE, "reset draws cannot be turned on once the state bank is on (its record layout depends on it)");
-  if (!h->have_params || !h->S.ops)
-    return fail(MWB_ESTATE, "reset draws need device resets (params and a reset program: mwb_set_levels, or "
-                            "mwb_set_params and mwb_set_program); host-generated worlds draw on the host");
+  if (int rc = enable_prologue(h, kDraws, "reset draws need device resets (params and a reset program: "
+                                          "mwb_set_levels, or mwb_set_params and mwb_set_program); host-generated "
+                                          "worlds draw on the host"))
+    return rc;
   // D: the largest draw count over the levels, whose draws must be numbered 0, 1, ... in program order
   int D = 0;
   for (size_t l = 0; l < h->levels.size(); ++l) {
@@ -1631,11 +1659,7 @@ extern "C" int mwb_enable_reset_draws(mwb_handle* h) {
   R.episode = (double*)episode;
   R.D = D;
   R.pad_ = 0;
-  ResetDraws* d = nullptr;
-  if (alloc_arr(h, &d, 1)) return fail(MWB_ECUDA, "reset draw state allocation failed");
-  if (h2d(d, &R, sizeof(R), h->stream) != 0 || sync_stream(h->stream) != 0) return fail(MWB_ECUDA, "upload failed");
-  h->S.draws = d;
-  return MWB_OK;
+  return publish_record(h, R, &h->S.draws, "reset draw state allocation failed");
 }
 
 #ifndef MWB_HOSTSIM
@@ -1669,11 +1693,10 @@ static int launch_nav(mwb_handle* h, stream_t s) {
 }
 
 extern "C" int mwb_enable_goal_distance(mwb_handle* h, const mwb_goal_grid* grids) {
-  if (!h) return fail(MWB_EINVAL, "null handle");
-  if (h->S.nav) return fail(MWB_ESTATE, "goal distance is already on");
-  if (!h->have_params || !h->S.ops)
-    return fail(MWB_ESTATE, "goal distance needs device resets (params and a reset program: mwb_set_levels, or "
-                            "mwb_set_params and mwb_set_program); host-generated worlds arrive without a reset kernel");
+  if (int rc = enable_prologue(h, kNav, "goal distance needs device resets (params and a reset program: "
+                                        "mwb_set_levels, or mwb_set_params and mwb_set_program); host-generated "
+                                        "worlds arrive without a reset kernel"))
+    return rc;
   if (!grids) return fail(MWB_EINVAL, "null grids");
   int64_t G = 0;
   for (size_t l = 0; l < h->levels.size(); ++l) {
@@ -1699,6 +1722,7 @@ extern "C" int mwb_enable_goal_distance(mwb_handle* h, const mwb_goal_grid* grid
   if (rc) return rc;
   mwb_goal_grid* d_grids = nullptr;
   if (alloc_arr(h, &d_grids, h->levels.size())) return fail(MWB_ECUDA, "goal distance state allocation failed");
+  if (h2d(d_grids, grids, h->levels.size() * sizeof(mwb_goal_grid), h->stream) != 0) return fail(MWB_ECUDA, "upload failed");
   GoalNav& V = h->nav_h;
   V.grids = d_grids;
   V.field = (uint16_t*)field;
@@ -1709,13 +1733,7 @@ extern "C" int mwb_enable_goal_distance(mwb_handle* h, const mwb_goal_grid* grid
   V.shortest = (double*)shortest;
   V.G = (int32_t)G;
   V.pad_ = 0;
-  GoalNav* d = nullptr;
-  if (alloc_arr(h, &d, 1)) return fail(MWB_ECUDA, "goal distance state allocation failed");
-  if (h2d(d_grids, grids, h->levels.size() * sizeof(mwb_goal_grid), h->stream) != 0 || h2d(d, &V, sizeof(V), h->stream) != 0 ||
-      sync_stream(h->stream) != 0)
-    return fail(MWB_ECUDA, "upload failed");
-  h->S.nav = d;
-  return MWB_OK;
+  return publish_record(h, V, &h->S.nav, "goal distance state allocation failed");
 }
 
 // The record layout of the handle as it stands (StateBank in state.h): the scalars of one env, widest first so that
@@ -1777,11 +1795,10 @@ static void bank_layout(const mwb_handle* h, std::vector<BankCol>& cols, StateBa
 }
 
 extern "C" int mwb_enable_state_bank(mwb_handle* h, int32_t slots) {
-  if (!h) return fail(MWB_EINVAL, "null handle");
-  if (h->S.bank) return fail(MWB_ESTATE, "the state bank is already on");
-  if (!h->have_params || !h->S.ops)
-    return fail(MWB_ESTATE, "the state bank needs device resets (params and a reset program: mwb_set_levels, or "
-                            "mwb_set_params and mwb_set_program); host-generated worlds are reset on the host");
+  if (int rc = enable_prologue(h, kBank, "the state bank needs device resets (params and a reset program: "
+                                         "mwb_set_levels, or mwb_set_params and mwb_set_program); host-generated "
+                                         "worlds are reset on the host"))
+    return rc;
   if (slots < 1) return fail(MWB_EINVAL, "slots must be at least 1");
   DevState& S = h->S;
   std::vector<BankCol> cols;
@@ -1804,13 +1821,8 @@ extern "C" int mwb_enable_state_bank(mwb_handle* h, int32_t slots) {
   B.slots = slots;
   h->d_bank_pairs = (int32_t*)pairs;
   h->d_bank_winner = (int32_t*)winner;
-  StateBank* d = nullptr;
-  if (alloc_arr(h, &d, 1)) return fail(MWB_ECUDA, "state bank allocation failed");
-  if (h2d(dcols, cols.data(), cols.size() * sizeof(BankCol), h->stream) != 0 || h2d(d, &B, sizeof(B), h->stream) != 0 ||
-      sync_stream(h->stream) != 0)
-    return fail(MWB_ECUDA, "upload failed");
-  S.bank = d;
-  return MWB_OK;
+  if (h2d(dcols, cols.data(), cols.size() * sizeof(BankCol), h->stream) != 0) return fail(MWB_ECUDA, "upload failed");
+  return publish_record(h, B, &S.bank, "state bank allocation failed");
 }
 
 extern "C" int mwb_save_states(mwb_handle* h, const int32_t* env_ids, const int32_t* slots, int n, void* stream) {
@@ -2508,48 +2520,31 @@ extern "C" int mwb_visible_ents_from(mwb_handle* h, const double* poses, uint32_
 // ------------------------------------------------------------------ ABI: snapshot / restore
 // A header, then the sections of snapshot_sections in one fixed order.  The magic names the blob's mode: a handle
 // with level changes on writes (and needs) the level-change section, and a level table with Maze levels carries the
-// per-env worlds after the templates
+// per-env worlds after the templates; each mode of kModeBits that is on sets its bit
 static const uint32_t kSnapMagic = 0x5342574du;               // "MWBS"
 static const uint32_t kSnapMagicLevelChanges = 0x4c42574du;   // "MWBL"
 static const uint32_t kSnapMagicWorlds = 0x5742574du;         // "MWBW": level table with per-env worlds
 static const uint32_t kSnapMagicWorldsLevelChanges = 0x5842574du;   // "MWBX": ... and level changes on
-// a handle with episode seeds on writes the mode letter in lower case ("MWBs", "MWBl", "MWBw", "MWBx") and carries
-// next_seed and episode_seed among its arrays
-static const uint32_t kSnapMagicSeeds = 0x20000000u;
-// one with maze layouts on writes the "B" in lower case ("MWbS", "MWbs", ...) and carries the four layout arrays
-static const uint32_t kSnapMagicMazes = 0x00200000u;
-// one with start poses on writes the "W" in lower case ("MwBS", "MwbS", ...) and carries the four start pose arrays
-static const uint32_t kSnapMagicPoses = 0x00002000u;
-// one with the state bank on writes the "M" in lower case ("mWBS", "mwbs", ...) and carries the records, bank_level,
-// next_state and episode_state
-static const uint32_t kSnapMagicBank = 0x00000020u;
-// one with reset draws on sets the high bit of the mode letter (every letter's case bit already names a mode) and
-// carries next_draws, draws_pending and episode_draws
-static const uint32_t kSnapMagicDraws = 0x80000000u;
-// one with goal distance on sets the high bit of the "M" and carries episode_shortest (the fields are rebuilt)
-static const uint32_t kSnapMagicNav = 0x00000080u;
-static const uint32_t kSnapMagicModes =
-    kSnapMagicSeeds | kSnapMagicMazes | kSnapMagicPoses | kSnapMagicBank | kSnapMagicDraws | kSnapMagicNav;
+static const uint32_t kSnapMagicModes = [] {
+  uint32_t bits = 0;
+  for (const ModeBit& m : kModeBits) bits |= m.bit;
+  return bits;
+}();
 
 static uint32_t snapshot_magic(const mwb_handle* h) {
-  const uint32_t seeds = (h->S.next_seed ? kSnapMagicSeeds : 0u) | (h->S.layouts ? kSnapMagicMazes : 0u) |
-                         (h->S.poses ? kSnapMagicPoses : 0u) | (h->S.bank ? kSnapMagicBank : 0u) |
-                         (h->S.draws ? kSnapMagicDraws : 0u) | (h->S.nav ? kSnapMagicNav : 0u);
-  if (h->level_mazes) return (h->S.next_level ? kSnapMagicWorldsLevelChanges : kSnapMagicWorlds) | seeds;
-  return (h->S.next_level ? kSnapMagicLevelChanges : kSnapMagic) | seeds;
+  uint32_t modes = 0;
+  for (const ModeBit& m : kModeBits) modes |= m.on(h->S) ? m.bit : 0u;
+  if (h->level_mazes) return (h->S.next_level ? kSnapMagicWorldsLevelChanges : kSnapMagicWorlds) | modes;
+  return (h->S.next_level ? kSnapMagicLevelChanges : kSnapMagic) | modes;
 }
 static std::string snapshot_mode(uint32_t magic) {
   const uint32_t base = magic & ~kSnapMagicModes;
-  return std::string(base == kSnapMagic ? "level changes off, no per-env worlds"
-                     : base == kSnapMagicLevelChanges ? "level changes on, no per-env worlds"
-                     : base == kSnapMagicWorlds ? "level changes off, per-env worlds"
-                                                : "level changes on, per-env worlds") +
-         (magic & kSnapMagicSeeds ? ", episode seeds on" : ", episode seeds off") +
-         (magic & kSnapMagicMazes ? ", maze layouts on" : ", maze layouts off") +
-         (magic & kSnapMagicPoses ? ", start poses on" : ", start poses off") +
-         (magic & kSnapMagicBank ? ", state bank on" : ", state bank off") +
-         (magic & kSnapMagicDraws ? ", reset draws on" : ", reset draws off") +
-         (magic & kSnapMagicNav ? ", goal distance on" : ", goal distance off");
+  std::string s = base == kSnapMagic ? "level changes off, no per-env worlds"
+                  : base == kSnapMagicLevelChanges ? "level changes on, no per-env worlds"
+                  : base == kSnapMagicWorlds ? "level changes off, per-env worlds"
+                                             : "level changes on, per-env worlds";
+  for (const ModeBit& m : kModeBits) s += std::string(", ") + m.name + (magic & m.bit ? " on" : " off");
+  return s;
 }
 
 struct SnapHeader {
@@ -2777,22 +2772,17 @@ extern "C" int mwb_state_array(mwb_handle* h, int which, void** dev_ptr, int64_t
   const DevState& S = h->S;
   const MazeLayouts& Y = h->layouts_h;
   const StartPoses& P = h->poses_h;
-  const int64_t N = S.N, E = S.E;
-  // why the arrays of a mode are missing, naming the call that adds them; null while the mode is on
-  const char* levels_off = S.next_level ? nullptr : "level changes are off (mwb_enable_level_changes)";
-  const char* seeds_off = S.next_seed ? nullptr : "episode seeds are off (mwb_enable_episode_seeds)";
-  const char* mazes_off = S.layouts ? nullptr : "maze layouts are off (mwb_enable_maze_layouts)";
-  const char* poses_off = S.poses ? nullptr : "start poses are off (mwb_enable_start_poses)";
-  const char* bank_off = S.bank ? nullptr : "the state bank is off (mwb_enable_state_bank)";
-  const char* draws_off = S.draws ? nullptr : "reset draws are off (mwb_enable_reset_draws)";
   const ResetDraws& Dr = h->draws_h;
-  const char* nav_off = S.nav ? nullptr : "goal distance is off (mwb_enable_goal_distance)";
   const GoalNav& V = h->nav_h;
   const StateBank& B = h->bank_h;
+  const int64_t N = S.N, E = S.E;
+  // why an array is missing, naming the call that adds it; null while it is there
+  const char* levels_off = S.next_level ? nullptr : "level changes are off (mwb_enable_level_changes)";
   const char* params_off = h->have_params && S.ops ? nullptr
                            : "the handle has no device resets (params and a reset program: mwb_set_levels, or "
                              "mwb_set_params and mwb_set_program); host-generated worlds carry their own draws";
   const char* off = nullptr;
+  int mode = -1;   // the array's mode in kModeBits
   void* p = nullptr;
   int64_t n = N;
   switch (which) {
@@ -2805,30 +2795,35 @@ extern "C" int mwb_state_array(mwb_handle* h, int which, void** dev_ptr, int64_t
     case MWB_ARRAY_ENV_LEVEL: p = S.env_level; off = levels_off; break;                           // int32 [N]
     case MWB_ARRAY_NEXT_LEVEL: p = S.next_level; off = levels_off; break;                         // int32 [N]
     case MWB_ARRAY_LEVEL_WEIGHTS: p = (void*)S.level_weights; n = S.num_levels; off = levels_off; break;   // float32 [L]
-    case MWB_ARRAY_NEXT_SEED: p = S.next_seed; off = seeds_off; break;                            // int64 [N]
-    case MWB_ARRAY_EPISODE_SEED: p = S.episode_seed; off = seeds_off; break;                      // int64 [N]
-    case MWB_ARRAY_NEXT_MAZE: p = Y.next; n = N * Y.rows * Y.cols; off = mazes_off; break;        // uint8 [N][rows][cols]
-    case MWB_ARRAY_EPISODE_MAZE: p = Y.episode; n = N * Y.rows * Y.cols; off = mazes_off; break;  // uint8 [N][rows][cols]
-    case MWB_ARRAY_NEXT_MAZE_CELLS: p = Y.cells; n = 2 * N; off = mazes_off; break;               // int32 [N][2]
-    case MWB_ARRAY_MAZE_PENDING: p = Y.pending; off = mazes_off; break;                           // uint8 [N]
-    case MWB_ARRAY_NEXT_POSE: p = P.next; n = N * E * 3; off = poses_off; break;                  // float64 [N][E][3]
-    case MWB_ARRAY_NEXT_AGENT_POSE: p = P.next_agent; n = N * 3; off = poses_off; break;          // float64 [N][3]
-    case MWB_ARRAY_POSE_PENDING: p = P.pending; off = poses_off; break;                           // uint8 [N]
-    case MWB_ARRAY_EPISODE_START: p = P.episode; n = N * 3; off = poses_off; break;               // float64 [N][3]
-    case MWB_ARRAY_NEXT_STATE: p = B.next_state; off = bank_off; break;                           // int32 [N]
-    case MWB_ARRAY_EPISODE_STATE: p = B.episode_state; off = bank_off; break;                     // int32 [N]
-    case MWB_ARRAY_BANK_LEVEL: p = B.bank_level; n = B.slots; off = bank_off; break;              // int32 [slots]
-    case MWB_ARRAY_NEXT_DRAWS: p = Dr.next; n = N * Dr.D; off = draws_off; break;                 // float64 [N][D]
-    case MWB_ARRAY_DRAWS_PENDING: p = Dr.pending; off = draws_off; break;                         // uint8 [N]
-    case MWB_ARRAY_EPISODE_DRAWS: p = Dr.episode; n = N * Dr.D; off = draws_off; break;           // float64 [N][D]
-    case MWB_ARRAY_GOAL_DIST: p = V.goal_dist; off = nav_off; break;                              // float64 [N]
-    case MWB_ARRAY_EXPERT_ACTION: p = V.expert; off = nav_off; break;                             // int32 [N]
-    case MWB_ARRAY_EPISODE_SHORTEST: p = V.shortest; off = nav_off; break;                        // float64 [N]
-    case MWB_ARRAY_GOAL_FIELD: p = V.field; n = N * V.G; off = nav_off; break;                    // uint16 [N][G]
+    case MWB_ARRAY_NEXT_SEED: p = S.next_seed; mode = kSeeds; break;                            // int64 [N]
+    case MWB_ARRAY_EPISODE_SEED: p = S.episode_seed; mode = kSeeds; break;                      // int64 [N]
+    case MWB_ARRAY_NEXT_MAZE: p = Y.next; n = N * Y.rows * Y.cols; mode = kMazes; break;        // uint8 [N][rows][cols]
+    case MWB_ARRAY_EPISODE_MAZE: p = Y.episode; n = N * Y.rows * Y.cols; mode = kMazes; break;  // uint8 [N][rows][cols]
+    case MWB_ARRAY_NEXT_MAZE_CELLS: p = Y.cells; n = 2 * N; mode = kMazes; break;               // int32 [N][2]
+    case MWB_ARRAY_MAZE_PENDING: p = Y.pending; mode = kMazes; break;                           // uint8 [N]
+    case MWB_ARRAY_NEXT_POSE: p = P.next; n = N * E * 3; mode = kPoses; break;                  // float64 [N][E][3]
+    case MWB_ARRAY_NEXT_AGENT_POSE: p = P.next_agent; n = N * 3; mode = kPoses; break;          // float64 [N][3]
+    case MWB_ARRAY_POSE_PENDING: p = P.pending; mode = kPoses; break;                           // uint8 [N]
+    case MWB_ARRAY_EPISODE_START: p = P.episode; n = N * 3; mode = kPoses; break;               // float64 [N][3]
+    case MWB_ARRAY_NEXT_STATE: p = B.next_state; mode = kBank; break;                           // int32 [N]
+    case MWB_ARRAY_EPISODE_STATE: p = B.episode_state; mode = kBank; break;                     // int32 [N]
+    case MWB_ARRAY_BANK_LEVEL: p = B.bank_level; n = B.slots; mode = kBank; break;              // int32 [slots]
+    case MWB_ARRAY_NEXT_DRAWS: p = Dr.next; n = N * Dr.D; mode = kDraws; break;                 // float64 [N][D]
+    case MWB_ARRAY_DRAWS_PENDING: p = Dr.pending; mode = kDraws; break;                         // uint8 [N]
+    case MWB_ARRAY_EPISODE_DRAWS: p = Dr.episode; n = N * Dr.D; mode = kDraws; break;           // float64 [N][D]
+    case MWB_ARRAY_GOAL_DIST: p = V.goal_dist; mode = kNav; break;                              // float64 [N]
+    case MWB_ARRAY_EXPERT_ACTION: p = V.expert; mode = kNav; break;                             // int32 [N]
+    case MWB_ARRAY_EPISODE_SHORTEST: p = V.shortest; mode = kNav; break;                        // float64 [N]
+    case MWB_ARRAY_GOAL_FIELD: p = V.field; n = N * V.G; mode = kNav; break;                    // uint16 [N][G]
     case MWB_ARRAY_LEVEL_PARAMS: p = (void*)S.level_params; n = (int64_t)h->levels.size(); off = params_off; break;  // mwb_params [L]
     default: return fail(MWB_EINVAL, "unknown array");
   }
   if (off) return fail(MWB_ESTATE, off);
+  if (mode >= 0 && !kModeBits[mode].on(S)) {
+    std::string call = std::string("mwb_enable_") + kModeBits[mode].name;
+    std::replace(call.begin(), call.end(), ' ', '_');
+    return fail(MWB_ESTATE, std::string(kModeBits[mode].subject) + " off (" + call + ")");
+  }
   *dev_ptr = p;
   *count = n;
   return MWB_OK;
