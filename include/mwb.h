@@ -479,6 +479,42 @@ int mwb_enable_start_poses(mwb_handle* h);
  * in the header; restoring across the mode fails with MWB_ESTATE before anything else is compared. */
 int mwb_enable_reset_draws(mwb_handle* h);
 
+/* Env params (automatic domain randomisation with per-env boundary sampling, robustness sweeps over camera, lighting
+ * and dynamics): give an env's next episode DomainParams of its own.  Valid on a handle with device resets (params and
+ * a reset program), before the state bank: MWB_ESTATE when the handle resets on the host, has the mode on already or
+ * has the bank on.  A params row is MWB_ENV_PARAM_ELEMS element rows in the order of mwb_params with each vector param
+ * expanded element by element (sky_color[0..2] 0-2, light_pos 3-5, light_color 6-8, light_ambient 9-11,
+ * obj_color_bias 12-14, forward_step 15, forward_drift 16, turn_step 17, cam_pitch 18, cam_fov_y 19, cam_height 20,
+ * cam_fwd_disp 21); an element row is float64 (default, min, max).  Three arrays, read and written in place through
+ * mwb_state_array, stream-ordered, without a sync:
+ *   next_params float64 [N][22][3]     the row env i's next episode runs (all NaN at the call);
+ *   params_pending uint8 [N]           nonzero: the row waits for the env's next reset (all 0 at the call);
+ *   episode_params float64 [N][22][3]  the row of the env's running episode, all NaN when it runs its level's params.
+ * At every reset of env i (mwb_reset, and the next-step auto-reset inside mwb_step) that runs a program, at any level,
+ * after the level, seed and bank rules: with params_pending[i] set, params_pending[i] = 0 and next_params[i] is copied
+ * into episode_params[i], the rows staying as written; otherwise episode_params[i] is set to all NaN.  The episode then
+ * runs on its level's params merged with episode_params[i], element by element:
+ *   - the range is the env's (min, max) when both are finite, else the level's; the default is the env's when finite,
+ *     else the level's.  A range is lowered as lo = min and rng = max - min in float64 (numpy's uniform());
+ *   - "the level's" means the level row as it stands at the reset for the params read at resets (sky, light,
+ *     obj_color_bias, the camera params), and at every step for forward_step, forward_drift and turn_step, so that
+ *     writes to MWB_ARRAY_LEVEL_PARAMS keep reaching every entry an episode did not design, mid-episode included;
+ *   - max_forward_step (the near() threshold and the carry distance) is the env's forward_step max when that element's
+ *     range applies, else the level's at the reset; the episode keeps it.
+ * A design changes no draw count: under the level's domain_rand flag every element is still one uniform(), without it
+ * only defaults are read, so the stream advances as without a design and a seed plus a design reproduces an episode.
+ * (v, v, v) pins an element either way.  A range with min > max runs on the device only (lo + (max - min) * u with
+ * a negative span); the reference and the drop-in class draw with numpy's Generator.uniform, which refuses it.  The goal distance
+ * mode uses the merged max_forward_step for its near-goal nodes and the merged turn_step default for its expert.  A
+ * state-bank load consumes only next_state: a pending row waits for the next reset that runs a program, and
+ * episode_params is part of the record (528 B more per record).  Handles that never call this behave exactly as
+ * before it existed, and the addition changes no struct, so MWB_ABI_VERSION stays as it is.  Snapshots of a handle
+ * with the mode on carry the three arrays and are marked as such in the header; restoring across the mode fails with
+ * MWB_ESTATE before anything else is compared.  Memory: 2 x 528 + 1 B per env for the arrays, plus a 536 B per-env
+ * scratch for the merged row. */
+#define MWB_ENV_PARAM_ELEMS 22
+int mwb_enable_env_params(mwb_handle* h);
+
 /* State bank (Go-Explore, backplay and demonstration-start curricula, branching rollouts): save env states into device
  * records and start an env's next episode from one.  Valid on a handle with device resets, after the level table, any
  * Maze levels and the other modes are set up: MWB_ESTATE when the handle resets on the host or has the bank on already,
@@ -760,6 +796,10 @@ int mwb_debug_camera(mwb_handle* h, float* out /* host [num_envs][16] */);
 #define MWB_ARRAY_EXPERT_ACTION 33    /* int32 [num_envs]  action along the shortest path, -1 = none                   */
 #define MWB_ARRAY_EPISODE_SHORTEST 34 /* float64 [num_envs]  goal_dist right after the running episode's reset          */
 #define MWB_ARRAY_GOAL_FIELD 35       /* uint16 [num_envs][G]  distance field in units of h / 5, 0xFFFF = none          */
+/* with env params on (mwb_enable_env_params; MWB_ESTATE otherwise); count = elements: */
+#define MWB_ARRAY_NEXT_PARAMS 36      /* float64 [num_envs][22][3]  (default, min, max) rows of the next episode       */
+#define MWB_ARRAY_PARAMS_PENDING 37   /* uint8 [num_envs]  nonzero = next_params waits for the env's next reset        */
+#define MWB_ARRAY_EPISODE_PARAMS 38   /* float64 [num_envs][22][3]  rows of the running episode, NaN = the level's      */
 int mwb_state_array(mwb_handle* h, int which, void** dev_ptr, int64_t* count);
 /* 1 when this library keeps the handle's state arrays (mwb_state_array) in host memory -- the CPU build of the kernels
  * used by the test suite -- and 0 for libmwb.so, whose arrays are device memory. */

@@ -24,6 +24,8 @@ Per-environment semantics are exactly those of the reference's `MiniWorldEnv.res
   * with `reset_draws=True`, an env's next reset can take designed outcomes of its level's reset draws (object kinds and
     colours, box sizes, goal sides, headings) written into a device tensor (`next_draws`, `set_env_draws`), and
     `info["draws"]` holds the outcome of every draw of each running episode;
+  * with `env_params=True`, an env's next episode can run on DomainParams of its own, (default, min, max) rows written
+    into a device tensor (`next_params`, `set_env_param`), and `info["params"]` holds the rows of each running episode;
   * with `state_bank=K`, envs can be saved into K device-side records (`save_states`) and an env's next reset can load
     one (`next_state`, `set_env_state`), and `info["state"]` names the record each running episode was loaded from;
   * with `goal_distance=True`, every step and reset leaves each env's geodesic distance to its goal (`goal_dist`), an
@@ -37,7 +39,7 @@ from collections import namedtuple
 import numpy as np
 
 from . import pack
-from .engine import (Engine, GOAL_GRID_DTYPE, LEVEL_CAP, LOWERED_PARAMS, OP_PLACE, OP_PUT, PARAMS_COLUMN, PROTO_DTYPE, RULE_GOAL,
+from .engine import (ENV_PARAM_ROWS, Engine, GOAL_GRID_DTYPE, LEVEL_CAP, LOWERED_PARAMS, OP_PLACE, OP_PUT, PARAMS_COLUMN, PROTO_DTYPE, RULE_GOAL,
                      RULE_NONE, RULE_HEALTH, RULE_PICKUP, RULE_PUTNEXT, RULE_SIDEWALK, RULE_SIGN, generator_from_state,
                      rng_state_of, RNG_DTYPE)
 from .envs import LEVELS
@@ -193,6 +195,10 @@ _MODES = (
           "this batch has no reset draws: construct it with reset_draws=True",
           "reset draws are taken by device resets; host-reset levels draw in Python "
           "(reset(options={\"draws\": ...}) of the level itself)", [("draws", "episode_draws")]),
+    _Mode("env_params", ("next_params", "params_pending", "episode_params"),
+          "this batch has no env params: construct it with env_params=True",
+          "env params are taken by device resets; host-reset levels draw their params in Python "
+          "(reset(options={\"params\": ...}) of the level itself)", [("params", "episode_params")]),
     _Mode("goal_distance", ("goal_dist", "expert_action", "episode_shortest", "goal_field"),
           "this batch has no goal distance: construct it with goal_distance=True",
           "goal distance is built by device resets; host-reset levels build their worlds in Python "
@@ -304,6 +310,21 @@ class BatchedMiniWorld:
     count; after a terminating step they still name the episode that just ended.  A designed start pose still wins for
     position and dir; a state-bank load leaves pending draws for the next reset that runs a program.
 
+    `env_params=True` (one level or a table; levels that reset on the device) gives episodes DomainParams of their own,
+    for automatic domain randomisation with per-env boundary sampling and for robustness sweeps over camera, lighting
+    and dynamics.  A row is 22 element rows of float64 (default, min, max) in engine.LOWERED_PARAMS order, vector params
+    expanded element by element; `param_rows` maps each param to its row index or slice.  With `params_pending[i]` set,
+    env i's next reset at any level, the auto-reset inside `step` included, copies `next_params[i]` into
+    `episode_params[i]` and clears the flag (the rows stay as written); any other reset that runs a program sets
+    `episode_params[i]` to NaN.  The episode runs on its level's params merged element by element: the env's (min, max)
+    when both are finite, else the level's range; the env's default when finite, else the level's.  The level's entries
+    are read as they stand (forward_step, forward_drift and turn_step at every step, so `set_level_param` keeps reaching
+    every entry an episode did not design), and max_forward_step follows a designed forward_step range.  Draw counts
+    do not change (the level's `domain_rand` still decides whether draws are made), so a seed plus a row reproduces an
+    episode, and (v, v, v) pins an element.  `episode_params` / `info["params"]` (float64 [N, 22, 3]) hold each running
+    episode's row; after a terminating step they still name the episode that just ended.  A state-bank load leaves a
+    pending row for the next reset that runs a program.  Memory: 1 057 B per env plus a 536 B merge scratch.
+
     `state_bank=K` (one level or a table; levels that reset on the device) keeps K records of env states on the device,
     for Go-Explore, backplay and branching rollouts: `save_states(env_ids, slots)` copies env env_ids[t] into slot
     slots[t] (entity list, counters, health, camera, lighting, colours, textures, the RNG stream, the level, the mode
@@ -333,7 +354,8 @@ class BatchedMiniWorld:
     def __init__(self, level, num_envs, obs_width=80, obs_height=60, domain_rand=False, autoreset=True,
                  msaa_samples=8, device=0, want_depth=False, level_kwargs=None, obs_format="hwc", env_level=None,
                  dynamic_levels=False, level_seed=0, env_offset=0, per_env_worlds=False, episode_seeds=False,
-                 maze_layouts=False, start_poses=False, state_bank=None, reset_draws=False, goal_distance=False):
+                 maze_layouts=False, start_poses=False, state_bank=None, reset_draws=False, goal_distance=False,
+                 env_params=False):
         given = locals()
         self.num_envs = int(num_envs)
         self.obs_width, self.obs_height = int(obs_width), int(obs_height)
@@ -602,7 +624,7 @@ class BatchedMiniWorld:
         return self._view_map
 
     def _write_pending(self, what, ids, arrays):
-        """The part set_env_level / set_env_seed / set_env_maze / set_env_pose / set_env_draws / set_env_state share: check the env ids `ids` (1-D
+        """The part set_env_level / set_env_seed / set_env_maze / set_env_pose / set_env_draws / set_env_param / set_env_state share: check the env ids `ids` (1-D
         integers in [0, N)), then write each (array name or view, values) of `arrays` at those envs -- values one per id
         (a numpy array, or a CUDA tensor) or one for all -- an env listed more than once taking its last entry.  On the host build the write is
         numpy's; on the device it is torch ops on the current stream, without a sync."""
@@ -872,6 +894,106 @@ class BatchedMiniWorld:
         if got not in ((), ids.shape):
             raise ValueError("set_env_draws: values are one value or one per env id (%d), got shape %s" % (ids.size, got))
         self._write_pending("set_env_draws", ids, [(view[:, int(index)], vals), ("draws_pending", 1)])
+
+    # ------------------------------------------------------------------ env params (env_params=True)
+    param_rows = ENV_PARAM_ROWS
+
+    @property
+    def next_params(self):
+        """float64 [N, 22, 3] view of the (default, min, max) rows each env's next episode runs with `params_pending`
+        set (NaN: the level's); write it in place (stream-ordered, no sync).  `param_rows` names the rows."""
+        return self._views()["next_params"]
+
+    @property
+    def params_pending(self):
+        """uint8 [N] view: nonzero when next_params[i] waits for env i's next reset, which clears it."""
+        return self._views()["params_pending"]
+
+    @property
+    def episode_params(self):
+        """float64 [N, 22, 3] view of the rows of each env's running episode, all NaN when it runs its level's params."""
+        return self._views()["episode_params"]
+
+    def set_env_param(self, env_ids, name, default=None, min=None, max=None):
+        """Design param `name` (one of engine.LOWERED_PARAMS, a float param) of the listed envs' next episodes: `default`,
+        `min` and `max` are each a value of the param's shape (() or (3,)), or one per env id ([n, *shape]), as
+        floats, sequences, numpy arrays or CUDA tensors; None writes NaN, the level's.  The range applies when both
+        min and max are finite.  Envs in mid-episode finish it first; an env listed more than once takes its last entry.
+        Sets `params_pending`; the other rows written earlier stay.  Host values are checked as DomainParams.set checks
+        them (shapes, min <= default <= max where given); tensor values are not checked.  The write is numpy's on the
+        host build, torch ops on the current stream on the device; env ids given as a CUDA tensor are read back to the
+        host first (the duplicate and range checks run there), which synchronises."""
+        view = self._views()["next_params"]          # a batch without the mode raises before any input check
+        if name not in LOWERED_PARAMS:
+            raise KeyError("%r is not a param the engine reads; these are: %s" % (name, ", ".join(LOWERED_PARAMS)))
+        for level, pe in enumerate(self.proto_envs):
+            if pe.params.params[name].type != "float":
+                raise TypeError("%r of level %d is a %s param; only float params can be set"
+                                % (name, level, pe.params.params[name].type))
+        ids = np.atleast_1d(_host(env_ids))
+        rows = self.param_rows[name]
+        shape = (3,) if isinstance(rows, slice) else ()
+        vals, host = {}, {}
+        for key, v in (("default", default), ("min", min), ("max", max)):
+            if v is None:
+                vals[key] = float("nan")
+                continue
+            if hasattr(v, "is_cuda") and v.is_cuda:
+                t = v.to(self._ensure_torch().float64)
+                got = tuple(t.shape)
+            else:
+                a = np.asarray(_host(v))
+                if a.dtype == object:                # None entries of a sequence: the level's
+                    try:
+                        a = a.astype(np.float64)
+                    except (TypeError, ValueError):
+                        pass
+                if not (np.issubdtype(a.dtype, np.floating) or np.issubdtype(a.dtype, np.integer)):
+                    raise ValueError("set_env_param: %s of %r is real numbers, got %s" % (key, name, a.dtype))
+                t = host[key] = a.astype(np.float64)
+                got = t.shape
+            if got not in (shape, ids.shape + shape):
+                raise ValueError("%s of %r must have shape %s or %s, got %s" % (key, name, shape, ids.shape + shape, got))
+            vals[key] = t if got != shape else (np.broadcast_to(t, ids.shape + shape) if isinstance(t, np.ndarray)
+                                                else t.expand(ids.shape + shape))
+        for a, b in (("min", "default"), ("default", "max"), ("min", "max")):
+            if a in host and b in host:
+                lo, hi = np.broadcast_arrays(host[a], host[b])
+                if not np.all((hi >= lo) | np.isnan(lo) | np.isnan(hi)):
+                    raise ValueError("%r: %s %s is above %s %s" % (name, a, host[a], b, host[b]))
+        self._write_pending("set_env_param", ids, [(view[:, rows, k], vals[key])
+                                                   for k, key in enumerate(("default", "min", "max"))]
+                            + [("params_pending", 1)])
+
+    def set_env_params(self, env_ids, params):
+        """Design every param of `params` (a DomainParams) that the engine reads for the listed envs' next episodes, as
+        `set_env_param` does; entries the engine does not read are ignored."""
+        for name in LOWERED_PARAMS:
+            if name in params.params:
+                p = params.params[name]
+                self.set_env_param(env_ids, name, p.default, p.min, p.max)
+
+    def get_env_params(self, env):
+        """The DomainParams env `env`'s running episode runs on (synchronises with the device): its level's params as
+        they stand now (get_level_params), merged with its `episode_params` row."""
+        env = int(env)
+        if not 0 <= env < self.num_envs:
+            raise ValueError("env must lie in [0, %d), got %d" % (self.num_envs, env))
+        self._sync_level_writes()
+        row = _host(self.episode_params[env]).copy()
+        level = int(_host(self._views()["env_level"])[env]) if self.dynamic_levels else int(self._env_level[env])
+        out = self.get_level_params(level)
+        for name in LOWERED_PARAMS:
+            p, r = out.params[name], row[self.param_rows[name]]
+            r = r.reshape(-1, 3)
+            d, lo, hi = (np.array(p.default, float).reshape(-1), np.array(p.min, float).reshape(-1),
+                         np.array(p.max, float).reshape(-1))
+            rng = np.isfinite(r[:, 1]) & np.isfinite(r[:, 2])
+            d = np.where(np.isfinite(r[:, 0]), r[:, 0], d)
+            lo, hi = np.where(rng, r[:, 1], lo), np.where(rng, r[:, 2], hi)
+            vals = [v if len(v) == 3 else float(v[0]) for v in (d, lo, hi)]
+            out.params[name] = DomainParams.DomainParam(vals[0], vals[1], vals[2], "float")
+        return out
 
     # ------------------------------------------------------------------ state bank (state_bank=K)
     @property
@@ -1205,10 +1327,10 @@ class BatchedMiniWorld:
     def _torch_writes(self):
         """True when torch work may write arrays the kernels read: next_level / level_weights (level changes on),
         next_seed (episode seeds on), the pending maze layouts (maze layouts on), the designed start poses (start poses
-        on), the designed draws (reset draws on), the pending slots (state bank on) or the params table (once
-        set_level_param has written it)."""
+        on), the designed draws (reset draws on), the designed params (env params on), the pending slots (state bank on)
+        or the params table (once set_level_param has written it)."""
         return ((self.dynamic_levels or self.episode_seeds or self.maze_layouts or self.start_poses
-                 or self.reset_draws or self.state_bank or self._params_written)
+                 or self.reset_draws or self.env_params or self.state_bank or self._params_written)
                 and not self.engine.host_memory)
 
     def _level_stream(self):

@@ -126,6 +126,7 @@ struct mwb_handle {
   MazeLayouts layouts_h;              // host copy of *S.layouts (mwb_enable_maze_layouts)
   StartPoses poses_h;                 // host copy of *S.poses (mwb_enable_start_poses)
   ResetDraws draws_h;                 // host copy of *S.draws (mwb_enable_reset_draws)
+  EnvParams envparams_h;              // host copy of *S.envparams (mwb_enable_env_params)
   GoalNav nav_h;                      // host copy of *S.nav (mwb_enable_goal_distance)
   StateBank bank_h;                   // host copy of *S.bank (mwb_enable_state_bank)
   int32_t* d_bank_pairs;              // [2][slots] staging of a host mwb_save_states call (env ids, then slots)
@@ -246,6 +247,9 @@ MWB_DEV void step_one(const DevState& S, int i, const int32_t* actions, const do
     o.terminated = 0;
     o.truncated = 0;
   } else {
+    // the step ranges of this episode's level as they stand at this step, with env params on merged with the
+    // episode's own row (merge_env_params writes only the three step elements), taken first, while little is live
+    const mwb_params& P = S.envparams ? *merge_env_params(S.envparams, i, &env_params_of(S, i), 15, 18) : env_params_of(S, i);
     int action = actions[i];
     if (S.act_noise) {            // wrapper.action() runs before env.step() draws its three parameters
       NpRng r = load_rng(S, i);
@@ -255,9 +259,7 @@ MWB_DEV void step_one(const DevState& S, int i, const int32_t* actions, const do
       MWB_WARP_SYNC();
     }
     double fs, fd, ts;
-    // the level of this episode: its domain_rand, and its step ranges as they stand at this step
-    const LevelDev& L = env_level_of(S, i);
-    const mwb_params& P = env_params_of(S, i);
+    const LevelDev& L = env_level_of(S, i);   // the level of this episode: its domain_rand
     if (step_params) {
       fs = step_params[i * 3 + 0];
       fd = step_params[i * 3 + 1];
@@ -1361,21 +1363,24 @@ extern "C" int mwb_set_levels(mwb_handle* h, int n_levels, const mwb_level* leve
 // a handle shows the mode on, and the words its enable call, mwb_state_array and snapshot_mode use for it.  Episode
 // seeds write the mode letter in lower case ("MWBs", "MWBl", "MWBw", "MWBx"), maze layouts the "B" ("MWbS", ...), start
 // poses the "W" and the state bank the "M"; reset draws set the high bit of the mode letter and goal distance that of
-// the "M" (every letter's case bit already names a mode).
+// the "M" (every letter's case bit already names a mode); env params set the high bit of the "B".
 struct ModeBit {
   uint32_t bit;
   const char* name;      // as snapshot_mode prints it; mwb_enable_<name, '_' for ' '> turns the mode on
   const char* subject;   // as the refusals name it, with its verb
   bool (*on)(const DevState& S);
+  bool named_off;        // snapshot_mode names the mode when it is off too (later modes only when on, so that the
+                         // refusals of blobs without them read as before)
 };
-enum Mode { kSeeds, kMazes, kPoses, kBank, kDraws, kNav };
+enum Mode { kSeeds, kMazes, kPoses, kBank, kDraws, kNav, kEnvParams };
 static const ModeBit kModeBits[] = {
-    {0x20000000u, "episode seeds", "episode seeds are", [](const DevState& S) { return S.next_seed != nullptr; }},
-    {0x00200000u, "maze layouts", "maze layouts are", [](const DevState& S) { return S.layouts != nullptr; }},
-    {0x00002000u, "start poses", "start poses are", [](const DevState& S) { return S.poses != nullptr; }},
-    {0x00000020u, "state bank", "the state bank is", [](const DevState& S) { return S.bank != nullptr; }},
-    {0x80000000u, "reset draws", "reset draws are", [](const DevState& S) { return S.draws != nullptr; }},
-    {0x00000080u, "goal distance", "goal distance is", [](const DevState& S) { return S.nav != nullptr; }},
+    {0x20000000u, "episode seeds", "episode seeds are", [](const DevState& S) { return S.next_seed != nullptr; }, true},
+    {0x00200000u, "maze layouts", "maze layouts are", [](const DevState& S) { return S.layouts != nullptr; }, true},
+    {0x00002000u, "start poses", "start poses are", [](const DevState& S) { return S.poses != nullptr; }, true},
+    {0x00000020u, "state bank", "the state bank is", [](const DevState& S) { return S.bank != nullptr; }, true},
+    {0x80000000u, "reset draws", "reset draws are", [](const DevState& S) { return S.draws != nullptr; }, true},
+    {0x00000080u, "goal distance", "goal distance is", [](const DevState& S) { return S.nav != nullptr; }, true},
+    {0x00800000u, "env params", "env params are", [](const DevState& S) { return S.envparams != nullptr; }, false},
 };
 
 // The checks every enable call but mwb_enable_level_changes starts with, in this order: a handle, the mode off, the
@@ -1662,6 +1667,25 @@ extern "C" int mwb_enable_reset_draws(mwb_handle* h) {
   return publish_record(h, R, &h->S.draws, "reset draw state allocation failed");
 }
 
+extern "C" int mwb_enable_env_params(mwb_handle* h) {
+  if (int rc = enable_prologue(h, kEnvParams, "env params need device resets (params and a reset program: "
+                                              "mwb_set_levels, or mwb_set_params and mwb_set_program); host-generated "
+                                              "worlds draw their params on the host"))
+    return rc;
+  const size_t N = h->S.N, row = MWB_ENV_PARAM_WORDS * sizeof(double);
+  void *next, *pending, *episode, *merged;
+  // NaN rows (0xFF bytes): no design until one is written, and the level's params before the first reset
+  int rc = alloc_control_arrays(h, "env param", {{&next, N * row, true}, {&pending, N, false}, {&episode, N * row, true},
+                                                 {&merged, N * sizeof(mwb_params), false}});
+  if (rc) return rc;
+  EnvParams& V = h->envparams_h;
+  V.next = (double*)next;
+  V.pending = (uint8_t*)pending;
+  V.episode = (double*)episode;
+  V.merged = (mwb_params*)merged;
+  return publish_record(h, V, &h->S.envparams, "env param state allocation failed");
+}
+
 #ifndef MWB_HOSTSIM
 // nav_kernel's shared memory opt-in, per device: like K2's (ensure_k2_smem) an attribute of the kernel function that
 // handles with different grids share, so it is only ever raised
@@ -1763,6 +1787,7 @@ static void bank_layout(const mwb_handle* h, std::vector<BankCol>& cols, StateBa
   if (S.next_seed) add(S.episode_seed, 8, 1, false);
   if (S.poses) add(h->poses_h.episode, 8, 3, true);
   if (S.draws) add(h->draws_h.episode, 8, h->draws_h.D, true);
+  if (S.envparams) add(h->envparams_h.episode, 8, MWB_ENV_PARAM_WORDS, true);
   add(S.ent_proto, 4, E, false);
   add(S.num_slots, 4, 1, false); add(S.agent_slot, 4, 1, false); add(S.carrying, 4, 1, false);
   add(S.step_count, 4, 1, false); add(S.num_picked, 4, 1, false); add(S.ghost_slot, 4, 1, false);
@@ -2543,7 +2568,8 @@ static std::string snapshot_mode(uint32_t magic) {
                   : base == kSnapMagicLevelChanges ? "level changes on, no per-env worlds"
                   : base == kSnapMagicWorlds ? "level changes off, per-env worlds"
                                              : "level changes on, per-env worlds";
-  for (const ModeBit& m : kModeBits) s += std::string(", ") + m.name + (magic & m.bit ? " on" : " off");
+  for (const ModeBit& m : kModeBits)
+    if (m.named_off || (magic & m.bit)) s += std::string(", ") + m.name + (magic & m.bit ? " on" : " off");
   return s;
 }
 
@@ -2573,7 +2599,7 @@ struct SnapSection {
 
 // The sections of a blob after its header, in blob order: every array that changes while episodes run (entity lists,
 // counters, camera / lighting parameters, RNG streams, pending-reset flags), the geometry currently on the device and
-// the level ranges, then the episode-seed, maze-layout, start-pose and reset-draw arrays, the state bank and
+// the level ranges, then the episode-seed, maze-layout, start-pose, reset-draw and env-param arrays, the state bank and
 // episode_shortest of handles with those modes on.  A handle with level
 // changes on closes the blob with its level-change section: env_level, next_level, level_draws, level_weights and
 // `tail` (adopted on restore: the assignment is state).  A static table of several levels closes it with the host's
@@ -2607,6 +2633,11 @@ static std::vector<SnapSection> snapshot_sections(mwb_handle* h, LevelChangeTail
   if (S.draws) {
     const ResetDraws& R = h->draws_h;
     dev(R.next, N * R.D * sizeof(double)); dev(R.pending, N); dev(R.episode, N * R.D * sizeof(double));
+  }
+  if (S.envparams) {   // (the merged scratch is written before every read)
+    const EnvParams& V = h->envparams_h;
+    const size_t row = MWB_ENV_PARAM_WORDS * sizeof(double);
+    dev(V.next, N * row); dev(V.pending, N); dev(V.episode, N * row);
   }
   if (S.bank) {
     const StateBank& B = h->bank_h;
@@ -2773,6 +2804,7 @@ extern "C" int mwb_state_array(mwb_handle* h, int which, void** dev_ptr, int64_t
   const MazeLayouts& Y = h->layouts_h;
   const StartPoses& P = h->poses_h;
   const ResetDraws& Dr = h->draws_h;
+  const EnvParams& Ep = h->envparams_h;
   const GoalNav& V = h->nav_h;
   const StateBank& B = h->bank_h;
   const int64_t N = S.N, E = S.E;
@@ -2815,6 +2847,9 @@ extern "C" int mwb_state_array(mwb_handle* h, int which, void** dev_ptr, int64_t
     case MWB_ARRAY_EXPERT_ACTION: p = V.expert; mode = kNav; break;                             // int32 [N]
     case MWB_ARRAY_EPISODE_SHORTEST: p = V.shortest; mode = kNav; break;                        // float64 [N]
     case MWB_ARRAY_GOAL_FIELD: p = V.field; n = N * V.G; mode = kNav; break;                    // uint16 [N][G]
+    case MWB_ARRAY_NEXT_PARAMS: p = Ep.next; n = N * MWB_ENV_PARAM_WORDS; mode = kEnvParams; break;     // float64 [N][22][3]
+    case MWB_ARRAY_PARAMS_PENDING: p = Ep.pending; mode = kEnvParams; break;                            // uint8 [N]
+    case MWB_ARRAY_EPISODE_PARAMS: p = Ep.episode; n = N * MWB_ENV_PARAM_WORDS; mode = kEnvParams; break;  // float64 [N][22][3]
     case MWB_ARRAY_LEVEL_PARAMS: p = (void*)S.level_params; n = (int64_t)h->levels.size(); off = params_off; break;  // mwb_params [L]
     default: return fail(MWB_EINVAL, "unknown array");
   }

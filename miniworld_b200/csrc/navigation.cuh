@@ -160,7 +160,7 @@ MWB_DEV void nav_query(const DevState& S, int i, const mwb_goal_grid& gr, const 
       const double vx = d_sub(wx, ax), vz = d_sub(wz, az);
       const double vf = d_add(d_mul(vx, co), d_mul(vz, -si));   // v . dir_vec, dir_vec = (cos, 0, -sin)
       const double vv = d_add(d_mul(vx, vx), d_mul(vz, vz));
-      const double ch = mwb_libm::cos_glibc(d_mul(d_mul(0.5, env_params_of(S, i).turn_step), 0.017453292519943295));
+      const double ch = mwb_libm::cos_glibc(d_mul(d_mul(0.5, env_turn_step(S, i)), 0.017453292519943295));
       if (vf > 0.0 && d_mul(vf, vf) >= d_mul(vv, d_mul(ch, ch)))
         action = 2;                                               // move_forward
       else                                                        // turn_left (dir grows) turns dir_vec towards

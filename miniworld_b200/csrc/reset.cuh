@@ -14,7 +14,8 @@
 // with the goal box and the agent in the layout's cells.  With start poses on (mwb_enable_start_poses) a reset can take
 // designed poses for the agent and the placed entities (take_poses, designed_pose), as place_entity(pos=..., dir=...).
 // With reset draws on (mwb_enable_reset_draws) a reset can replace the outcomes of its CHOICE / UNIFORM ops with
-// designed ones inside their support, and records every outcome (take_draws, designed_draw).  With the state bank on (mwb_enable_state_bank) a reset with a pending slot can instead load a saved env state
+// designed ones inside their support, and records every outcome (take_draws, designed_draw).  With env params on
+// (mwb_enable_env_params) a reset can run on its level's params merged with a row of its own (take_env_params).  With the state bank on (mwb_enable_state_bank) a reset with a pending slot can instead load a saved env state
 // (bank_load in bank.cuh) and return before the program runs.
 #pragma once
 #include "bank.cuh"
@@ -192,6 +193,30 @@ MWB_DEV_NOINLINE double designed_draw(const ResetDraws* R, int i, const mwb_op* 
   return v;
 }
 
+// The params env i's reset at level row `lvl` runs on (mwb_enable_env_params; include/mwb.h states the rule): a pending
+// row is taken into episode[i] and the flag cleared, the rows staying as written; otherwise episode[i] becomes all NaN.
+// Returns the level row merged with episode[i] (merge_env_params).  As in take_draws, every lane computes the same
+// flag from the same load, warp barriers separate the flag's load from its store, and it is out of line and given the
+// record's address; the record row is filled by all lanes, word w by lane w % 32.
+MWB_DEV_NOINLINE const mwb_params* take_env_params(const EnvParams* V, int i, const mwb_params* lvl) {
+  MWB_WARP_SYNC();
+  const bool take = V->pending[i] != 0;
+  MWB_WARP_SYNC();
+  if (take) V->pending[i] = 0;
+  const double* nx = V->next + (size_t)i * MWB_ENV_PARAM_WORDS;
+  double* ep = V->episode + (size_t)i * MWB_ENV_PARAM_WORDS;
+  // the 66 words spread over the warp's lanes (every lane then reads them after the barrier below)
+#ifdef __CUDA_ARCH__
+  const int lane = threadIdx.x & 31, lanes = 32;
+#else
+  const int lane = 0, lanes = 1;
+#endif
+#pragma unroll 1
+  for (int w = lane; w < MWB_ENV_PARAM_WORDS; w += lanes) ep[w] = take ? nx[w] : MWB_NAN;
+  MWB_WARP_SYNC();
+  return take ? merge_env_params(V, i, lvl, 0, MWB_ENV_PARAM_ELEMS) : lvl;
+}
+
 MWB_DEV void device_reset(const DevState& S, int i) {
   const size_t N = S.N;
   // the world changes: the goal distance kernel that follows rebuilds the env's field (navigation.cuh)
@@ -202,12 +227,14 @@ MWB_DEV void device_reset(const DevState& S, int i) {
   // bit 4 of flags below: this reset takes designed draws (taken before anything below is loaded: a call while those
   // values are live costs reset_kernel registers)
   const int draw_flag = S.draws && take_draws(S.draws, i) ? 16 : 0;
-  NpRng rng = load_rng(S, i);
   const int lvl = S.next_level ? resolve_level(S, i) : S.env_level[i];
+  // the level's ranges as they stand at this reset, merged with the env's own row when it took one (env params; taken
+  // before the stream is loaded, for the reason above)
+  const mwb_params& P = S.envparams ? *take_env_params(S.envparams, i, S.level_params + lvl) : S.level_params[lvl];
+  NpRng rng = load_rng(S, i);
   // the resolved level decides everything below, its domain_rand included: a reset that switches levels draws by the
   // new level's flag (read at each use: the row's address is live anyway, a cached copy would cost step_kernel a spill)
   const LevelDev& L = S.levels[lvl];
-  const mwb_params& P = S.level_params[lvl];   // the level's ranges as they stand at this reset
   const mwb_op* ops = S.ops + L.op_first;
   const int num_ops = L.num_ops;
   // the geometry of the level this episode runs: the env's own world (regenerated below by a Maze program) or the
@@ -376,16 +403,21 @@ MWB_DEV void device_reset(const DevState& S, int i) {
     for (int k = 0; k < 3; ++k)
       S.envp[(size_t)(q * 3 + k) * N + i] = L.domain_rand ? rng_uniform(rng, los[q][k], rngs[q][k]) : defs[q][k];
 
-  // for ent in self.entities: ent.randomize(params, rand)
-  if (L.domain_rand) {
+  // for ent in self.entities: ent.randomize(params, rand).  Without randomisation a Box still adds obj_color_bias's
+  // default (params.sample(None, ...), entity.py:405-407): zero unless a level row or an env's row sets it, and adding
+  // zero changes no colour, so the loop runs only when there is something to draw or add
+  const bool bias = P.obj_color_bias[0] != 0.0 || P.obj_color_bias[1] != 0.0 || P.obj_color_bias[2] != 0.0;
+  if (L.domain_rand || bias) {
     for (int e = 0; e < slots; ++e) {
       const mwb_proto& pr = S.protos[S.ent_proto[e * N + i]];
       if (pr.kind == MWB_KIND_BOX) {
         for (int k = 0; k < 3; ++k) {
-          double c = d_add(pr.color[k], rng_uniform(rng, P.obj_color_bias_lo[k], P.obj_color_bias_rng[k]));
+          const double b = L.domain_rand ? rng_uniform(rng, P.obj_color_bias_lo[k], P.obj_color_bias_rng[k])
+                                         : P.obj_color_bias[k];
+          double c = d_add(pr.color[k], b);
           S.ent_col[((size_t)e * 3 + k) * N + i] = c < 0.0 ? 0.0 : (c > 1.0 ? 1.0 : c);
         }
-      } else if (pr.kind == MWB_KIND_AGENT) {
+      } else if (L.domain_rand && pr.kind == MWB_KIND_AGENT) {
         S.cam[0 * N + i] = rng_uniform(rng, P.cam_height_lo, P.cam_height_rng);
         S.cam[1 * N + i] = rng_uniform(rng, P.cam_fwd_disp_lo, P.cam_fwd_disp_rng);
         S.cam[2 * N + i] = rng_uniform(rng, P.cam_pitch_lo, P.cam_pitch_rng);

@@ -50,6 +50,15 @@ struct ResetDraws {
   int32_t D, pad_;
 };
 
+// The env params arrays (mwb_enable_env_params).  A row is MWB_ENV_PARAM_ELEMS element rows of (default, min, max).
+#define MWB_ENV_PARAM_WORDS (MWB_ENV_PARAM_ELEMS * 3)
+struct EnvParams {
+  double* next;                 // [N][22][3] row the env's next reset takes
+  uint8_t* pending;             // [N] 1 = next[i] waits for the env's next reset
+  double* episode;              // [N][22][3] row of the env's running episode (NaN: the level's)
+  mwb_params* merged;           // [N] scratch: the level row merged with episode[i], written before every read
+};
+
 // The goal distance arrays (mwb_enable_goal_distance); navigation.cuh builds and reads them.
 struct GoalNav {
   const mwb_goal_grid* grids;   // [levels]
@@ -209,6 +218,8 @@ struct DevState {
   const struct StateBank* bank;
   // goal distance (mwb_enable_goal_distance); null on a handle without it, one pointer for the same reason
   const struct GoalNav* nav;
+  // env params (mwb_enable_env_params); null on a handle without them, one pointer for the same reason
+  const struct EnvParams* envparams;
   int32_t autoreset;
   // StochasticActionWrapper on the device (reference wrappers.py:49-71): per step one uniform() draw from
   // the env's own stream; below act_prob the chosen action stands, else act_random (< 0: integers(0, 6))
@@ -221,6 +232,47 @@ MWB_DEV int geom_block(const DevState& S, int i, int lvl) { return S.levels[lvl]
 MWB_DEV int geom_index(const DevState& S, int i) { return geom_block(S, i, S.env_level[i]); }
 MWB_DEV const LevelDev& env_level_of(const DevState& S, int i) { return S.levels[S.env_level[i]]; }
 MWB_DEV const mwb_params& env_params_of(const DevState& S, int i) { return S.level_params[S.env_level[i]]; }
+
+// Words of element e (mwb_enable_env_params' order) in an mwb_params record viewed as doubles: its default, lo and rng.
+// A vector param is [3] defaults, [3] lows, [3] spans; a scalar one default, low, span.
+MWB_DEV int env_param_word(int e) { return e < 15 ? (e / 3) * 9 + e % 3 : 45 + (e - 15) * 3; }
+MWB_DEV int env_param_step(int e) { return e < 15 ? 3 : 1; }
+
+// The level row `lvl` merged with env i's episode row for elements [e0, e1) into V->merged[i] (include/mwb.h states the
+// rule), and max_forward_step with them when forward_step (15) is among them.  Returns the merged record, or the level
+// row when the episode row designs none of those elements.  Out of line, and given the record's address rather than its
+// fields, so that handles without the mode keep their registers.
+MWB_DEV_NOINLINE const mwb_params* merge_env_params(const EnvParams* V, int i, const mwb_params* lvl, int e0, int e1) {
+  const double* ep = V->episode + (size_t)i * MWB_ENV_PARAM_WORDS;
+  bool any = false;
+#pragma unroll 1
+  for (int e = e0; e < e1; ++e) any |= isfinite(ep[3 * e]) || (isfinite(ep[3 * e + 1]) && isfinite(ep[3 * e + 2]));
+  if (!any) return lvl;
+  const double* src = (const double*)lvl;
+  mwb_params* m = V->merged + i;
+  double* dst = (double*)m;
+#pragma unroll 1
+  for (int e = e0; e < e1; ++e) {
+    const int w = env_param_word(e), s = env_param_step(e);
+    const double d = ep[3 * e], lo = ep[3 * e + 1], hi = ep[3 * e + 2];
+    const bool range = isfinite(lo) && isfinite(hi);
+    dst[w] = isfinite(d) ? d : src[w];
+    dst[w + s] = range ? lo : src[w + s];
+    dst[w + 2 * s] = range ? d_sub(hi, lo) : src[w + 2 * s];
+    if (e == 15) m->max_forward_step = range ? hi : lvl->max_forward_step;
+  }
+  MWB_WARP_SYNC();
+  return m;
+}
+
+// turn_step's default of env i's running episode (its episode row's when finite, else its level's as it stands)
+MWB_DEV double env_turn_step(const DevState& S, int i) {
+  if (S.envparams) {
+    const double t = S.envparams->episode[(size_t)i * MWB_ENV_PARAM_WORDS + 3 * 17];
+    if (isfinite(t)) return t;
+  }
+  return env_params_of(S, i).turn_step;
+}
 
 MWB_DEV NpRng load_rng(const DevState& S, int i) {
   NpRng r;

@@ -27,8 +27,8 @@ class ShardedMiniWorld:
         `dynamic_levels=True` (and `level_seed`) the level draws of global env i are those of the single-process run.
         `episode_seeds=True` is passed on as it is: a seed belongs to an env, so this rank's `local.next_seed` /
         `local.episode_seed` are its slice of the single-process arrays, and so are the maze layout arrays of `maze_layouts=True`
-        the start pose arrays of `start_poses=True` and the draw arrays of `reset_draws=True` (`local.set_env_draws`
-        takes local env ids).  `state_bank=K` gives every rank a bank of K slots of its own:
+        the start pose arrays of `start_poses=True`, the draw arrays of `reset_draws=True` (`local.set_env_draws`
+        takes local env ids) and the params arrays of `env_params=True` (`local.set_env_param` takes local env ids).  `state_bank=K` gives every rank a bank of K slots of its own:
         `local.save_states` / `local.set_env_state` take this rank's local env ids, and records stay on their rank.
         `goal_distance=True` is passed on as it is: `local.goal_dist`, `local.expert_action` and
         `local.episode_shortest` are this rank's slice of the single-process arrays."""

@@ -48,6 +48,10 @@ class Params(C.Structure):
 
 
 LOWERED_PARAMS = _VEC_PARAMS + _SCALAR_PARAMS     # the DomainParams entries the engine reads
+# element rows of an env params row (mwb_enable_env_params): param name -> its row index, or a slice of three rows
+ENV_PARAM_ROWS = dict([(n, slice(3 * k, 3 * k + 3)) for k, n in enumerate(_VEC_PARAMS)] +
+                      [(n, 15 + k) for k, n in enumerate(_SCALAR_PARAMS)])
+ENV_PARAM_ELEMS = 22
 PARAMS_DOUBLES = C.sizeof(Params) // 8
 # field of mwb_params -> its column in a float64 view of the params table
 PARAMS_COLUMN = {name: getattr(Params, name).offset // 8 for name, _ in Params._fields_}
@@ -142,6 +146,7 @@ EXPORTS = (
     "mwb_set_levels", "mwb_enable_level_changes", "mwb_state_in_host_memory", "mwb_set_level_maze",
     "mwb_enable_episode_seeds", "mwb_enable_maze_layouts", "mwb_enable_start_poses", "mwb_enable_state_bank",
     "mwb_save_states", "mwb_enable_reset_draws", "mwb_enable_goal_distance", "mwb_render_views", "mwb_visible_ents_from",
+    "mwb_enable_env_params",
 )
 OBS_FORMATS = {"hwc": 0, "cwh": 1, "grey": 2}
 
@@ -186,6 +191,7 @@ def load_library():
     lib.mwb_enable_state_bank.argtypes = [vp, C.c_int32]
     lib.mwb_enable_reset_draws.argtypes = [vp]
     lib.mwb_enable_goal_distance.argtypes = [vp, vp]
+    lib.mwb_enable_env_params.argtypes = [vp]
     lib.mwb_save_states.argtypes = [vp, vp, vp, C.c_int, vp]
     lib.mwb_state_in_host_memory.argtypes = []
     lib.mwb_seed.argtypes = [vp, vp, C.c_int, vp]
@@ -514,6 +520,12 @@ class Engine:
         needs device resets and a level with a draw, before the state bank."""
         self._check(self.lib.mwb_enable_reset_draws(self.h))
 
+    def enable_env_params(self):
+        """Resets with "params_pending" set run on their level's params merged with the (default, min, max) rows of
+        "next_params", and every reset records its rows in "episode_params" from now on (mwb_enable_env_params); needs
+        device resets, before the state bank."""
+        self._check(self.lib.mwb_enable_env_params(self.h))
+
     def enable_goal_distance(self, grids):
         """`grids` (GOAL_GRID_DTYPE [n_levels]): the goal distance kernel follows every step and reset from now on and
         fills "goal_dist", "expert_action", "episode_shortest" and "goal_field" (mwb_enable_goal_distance); needs
@@ -624,7 +636,7 @@ class Engine:
     # name -> (mwb_state_array id, element type, shape): "env" = [N], "ents" = [max_ents, N], "level" = [count]
     # ([n_levels], or [slots] for bank_level),
     # "params" = [n_levels, PARAMS_DOUBLES] (mwb_params records as float64 words), "env_rows" = [N, count / N],
-    # "env_slots" = [N, max_ents, 3]
+    # "env_slots" = [N, count / (3 N), 3] ([N, max_ents, 3], or [N, 22, 3] for the env params rows)
     ARRAYS = {"counter": (0, "<i4", "env"), "step_count": (1, "<i4", "env"), "ent_x": (2, "<f8", "ents"),
               "ent_y": (3, "<f8", "ents"), "ent_z": (4, "<f8", "ents"), "ent_dir": (5, "<f8", "ents"),
               "env_level": (6, "<i4", "env"), "next_level": (7, "<i4", "env"), "level_weights": (8, "<f4", "level"),
@@ -638,6 +650,11 @@ class Engine:
               "episode_draws": (31, "<f8", "env_rows"), "goal_dist": (32, "<f8", "env"),
               "expert_action": (33, "<i4", "env"), "episode_shortest": (34, "<f8", "env"),
               "goal_field": (35, "<u2", "env_rows")}
+    # ARRAYS holds the arrays of the modes up to goal distance; its key set is what pinned refusal texts walk, so
+    # later modes list theirs in a table of their own (state_array reads ARRAYS, then those tables).  A later mode adds
+    # a table here, or the tables are merged together with those texts.
+    ENV_PARAM_ARRAYS = {"next_params": (36, "<f8", "env_slots"), "params_pending": (37, "|u1", "env"),
+                        "episode_params": (38, "<f8", "env_slots")}
 
     def state_array(self, name, shape=None):
         """Zero-copy view of a state array (mwb_state_array) as an object with __cuda_array_interface__:
@@ -650,11 +667,11 @@ class Engine:
         uint8 [N]; with the state bank on, "next_state" / "episode_state" int32 [N] and "bank_level" int32 [slots];
         with reset draws on, "next_draws" / "episode_draws" float64 [N, D] and "draws_pending" uint8 [N]; with goal
         distance on, "goal_dist" / "episode_shortest" float64 [N], "expert_action" int32 [N] and "goal_field" uint16
-        [N, G].
+        [N, G]; with env params on, "next_params" / "episode_params" float64 [N, 22, 3] and "params_pending" uint8 [N].
         `shape` gives the view
         another shape of the same size (the maze layouts as [N, rows, cols]).  On the host build of the kernels the
         arrays live in host memory, and the view is a numpy array over the same memory instead."""
-        which, typestr, axis = self.ARRAYS[name]
+        which, typestr, axis = self.ARRAYS[name] if name in self.ARRAYS else self.ENV_PARAM_ARRAYS[name]
         ptr, count = C.c_void_p(), C.c_int64()
         self._check(self.lib.mwb_state_array(self.h, which, C.byref(ptr), C.byref(count)))
         n = count.value

@@ -97,3 +97,23 @@ def _defaults():
 
 
 DEFAULT_PARAMS = _defaults()
+
+
+def overlay_params(params, design):
+    """A copy of `params` overlaid by `design` {name: (default, min, max)}, element by element as an env params row of
+    the batched engine overlays its level's: a finite default replaces the param's, a finite (min, max) pair its range;
+    None or NaN entries keep the param's.  The result is built without DomainParams.set's checks, so a range may lie
+    outside its default or have min > max (numpy's uniform() takes both)."""
+    out = params.copy()
+    for name, row in design.items():
+        p = out.params[name]
+        if p.type != "float":
+            raise TypeError("%r is a %s param; only float params can be designed" % (name, p.type))
+        shape = np.shape(p.default)
+        d, lo, hi = (np.full(shape, np.nan) if v is None else np.broadcast_to(np.asarray(v, np.float64), shape)
+                     for v in row)
+        rng = np.isfinite(lo) & np.isfinite(hi)
+        vals = [np.where(np.isfinite(d), d, p.default), np.where(rng, lo, p.min), np.where(rng, hi, p.max)]
+        vals = [np.array(v, np.float64) if shape else float(v) for v in vals]
+        out.params[name] = DomainParam(vals[0], vals[1], vals[2], p.type)
+    return out

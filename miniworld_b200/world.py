@@ -26,7 +26,7 @@ from ._gym import gym, spaces
 from .assets import Texture
 from .entity import Agent, Entity
 from .math import Y_VEC, intersect_circle_segs
-from .params import DEFAULT_PARAMS
+from .params import DEFAULT_PARAMS, overlay_params
 
 DEFAULT_WALL_HEIGHT = 2.74
 TEX_DENSITY = 512   # texels per metre
@@ -249,8 +249,19 @@ class MiniWorldEnv(gym.Env):
         "agent_pose" (x, z, dir) for place_agent (see place_entity); Maze levels also read a designed layout.  "draws"
         {d: v} designs the level's reset draws, the choice / integers / uniform calls _gen_world() makes itself, numbered
         0, 1, ... in call order: each is made as usual, then replaced by v when v lies in its support (_DesignedDraws);
-        `episode_draws` then lists every outcome.  Placement and texture draws are not reset draws."""
+        `episode_draws` then lists every outcome.  Placement and texture draws are not reset draws.  "params"
+        {name: (default, min, max)} runs the episode on a copy of the level's params overlaid element by element as
+        BatchedMiniWorld(env_params=True) overlays them: a finite default replaces the level's, a finite (min, max)
+        pair its range; None or NaN entries keep the level's.  The next reset without the option runs on the level's
+        params again."""
         super().reset(seed=seed)
+        overlay = getattr(self, "_params_overlay", None)
+        if overlay is not None and self.params is overlay[1]:
+            self.params = overlay[0]            # the level's params again
+        self._params_overlay = None
+        if options and "params" in options:
+            self._params_overlay = (self.params, overlay_params(self.params, options["params"]))
+            self.params = self._params_overlay[1]
         self.step_count = 0
         self.agent = Agent()
         self.entities = []
