@@ -683,6 +683,27 @@ int mwb_render_views(mwb_handle* h, const double* poses, int views, int render_a
  * device) as mwb_render_views defines it; a skipped row leaves mask[i] as it is. */
 int mwb_visible_ents_from(mwb_handle* h, const double* poses, uint32_t* mask, void* stream);
 
+/* ---- designed cameras with their own intrinsics, frame size and sample count --------------------------
+ * mwb_render_views with rows of row_width 3 or 7 columns, rendered at width x height with `samples` samples per
+ * pixel (1, 4, 8 or 16).  A 7-column row is (x, z, dir, cam_height, cam_fwd_disp, cam_pitch, cam_fov_y): the view
+ * of env i is what the reference's render_obs(FrameBuffer(width, height, samples)) / render_depth(...) return after
+ * agent.pos = (x, agent.pos[1], z), agent.dir = dir and each camera attribute set to the row's value, nothing else
+ * changed.  NaN in columns 3-6 means the running episode's value (the one its reset drew, or the merged env params
+ * value): an all-NaN 7-column row renders the same bytes as its 3-column row.  Besides the 3-column skip rule, a
+ * 7-column row is skipped when an intrinsic column is +-inf, a given cam_fov_y lies outside (0, 180) or a given
+ * |cam_pitch| >= 90 (gluLookAt's basis is undefined at 90).  Frames come back in the observation format at
+ * width x height: obs [views][N] frames of that size, depth float32[views][N][height][width].  Host destinations
+ * use the handle's staging, which grows on the first call at a larger size and is never shrunk.
+ * mwb_render_views(h, poses, views, ...) is mwb_render_views_at(h, poses, 3, views, obs_width, obs_height,
+ * msaa_samples, ...). */
+int mwb_render_views_at(mwb_handle* h, const double* rows, int row_width, int views, int width, int height, int samples,
+                        int render_agent, uint8_t* obs, float* depth, void* stream);
+
+/* mwb_visible_ents_from with rows float64[N][row_width], row_width 3 or 7, as mwb_render_views_at defines them.  The
+ * reference's get_visible_ents always renders into obs_fb, so the query uses the row's camera attributes but the
+ * handle's own frame size and sample count. */
+int mwb_visible_ents_from_at(mwb_handle* h, const double* rows, int row_width, uint32_t* mask, void* stream);
+
 /* ---- state exchange (env.agent.pos, env.entities[i].pos ... views; checkpointing) ------ */
 int mwb_get_state(mwb_handle* h, const mwb_state_view* out);
 

@@ -1373,9 +1373,11 @@ class BatchedMiniWorld:
 
     def visible_ents(self, out=None, poses=None):
         """uint32 [N]: bit e set iff entity-list slot e of that env passes the reference's occlusion query
-        (get_visible_ents, miniworld.py:1238-1333).  With `poses` (float64 [N, 3] rows (x, z, dir), a CUDA tensor or
-        numpy array) the query runs from each env's designed camera as `render_views` defines it; a row that
-        `render_views` skips leaves that env's entry of `out` as it is."""
+        (get_visible_ents, miniworld.py:1238-1333).  With `poses` (float64 [N, 3] or [N, 7] rows as `render_views`
+        takes them, a CUDA tensor or numpy array) the query runs from each env's designed camera as `render_views`
+        defines it; a row that `render_views` skips leaves that env's entry of `out` as it is.  The reference's
+        get_visible_ents always renders into obs_fb, so the query uses a 7-column row's camera attributes but the
+        batch's own frame size and sample count."""
         if poses is not None:
             poses = self._view_rows("visible_ents", poses, single=True)
         if out is None:
@@ -1385,11 +1387,11 @@ class BatchedMiniWorld:
                 torch = self._ensure_torch()
                 out = torch.zeros(self.num_envs, dtype=torch.int32, device=torch.device("cuda", self.device))
         stream = None if (self.engine.host_memory or poses is None) else _torch_stream(self._ensure_torch(), self.device)
-        self.engine.visible_ents(out, stream=stream, poses=poses)
+        self.engine.visible_ents(out, stream=stream, poses=poses, row_width=3 if poses is None else poses.shape[-1])
         return out
 
     def _view_rows(self, what, poses, single=False):
-        """Checked pose rows: a contiguous float64 CUDA tensor or numpy array [V, N, 3] (or [N, 3])."""
+        """Checked pose rows: a contiguous float64 CUDA tensor or numpy array [V, N, 3|7] (or [N, 3|7])."""
         if hasattr(poses, "is_cuda"):
             if poses.dtype != self._ensure_torch().float64:
                 raise ValueError("%s: poses must be float64, not %s" % (what, poses.dtype))
@@ -1402,29 +1404,48 @@ class BatchedMiniWorld:
                 raise ValueError("%s: poses must be float64, not %s" % (what, np.asarray(poses).dtype))
             poses = np.ascontiguousarray(poses)
         shape = tuple(poses.shape)
-        ok = shape == (self.num_envs, 3) if single else (len(shape) in (2, 3) and shape[-2:] == (self.num_envs, 3))
+        ok = len(shape) == (2 if single else len(shape)) and len(shape) in (2, 3) and shape[-2] == self.num_envs and \
+            shape[-1] in (3, 7)
         if not ok or (len(shape) == 3 and shape[0] <= 0):
             raise ValueError("%s: poses must have shape %s, not %s" % (
-                what, "[N, 3]" if single else "[V, N, 3] or [N, 3] with N = %d" % self.num_envs, shape))
+                what, "[N, 3] or [N, 7]" if single else "[V, N, 3|7] or [N, 3|7] with N = %d" % self.num_envs, shape))
         return poses
 
-    def render_views(self, poses, render_agent=False, out=None, depth=None):
-        """Render every env from designed cameras (mwb_render_views).  `poses`: float64 [V, N, 3] or [N, 3] rows
-        (x, z, dir), a CUDA tensor or numpy array; the view of env i from (x, z, dir) is what the reference's
+    def render_views(self, poses, render_agent=False, out=None, depth=None, size=None, samples=None):
+        """Render every env from designed cameras (mwb_render_views_at).  `poses`: float64 [V, N, 3|7] or [N, 3|7]
+        rows, a CUDA tensor or numpy array.  The view of env i from (x, z, dir) is what the reference's
         render_obs() / render_depth() return after agent.pos = (x, agent.pos[1], z), agent.dir = dir, nothing else
-        changed (same entities, textures, light and the episode's camera parameters).  `render_agent=True` also draws
-        the agent's marker triangle at its real pose: a third-person view.  A row with a non-finite entry, or with
-        |dir| >= 105414350 (beyond the range the glibc-exact sin / cos are validated for), is skipped: its frame (and
-        depth) in that view is left as it is in `out` / `depth`.  No env state changes.
-        Returns frames [V, N, *frame] (or [N, *frame]) in the batch's observation layout -- `out` filled in place or a
-        fresh zero tensor -- and, when `depth` is True or an array / tensor float32 [V, N, H, W, 1] (or [N, H, W, 1])
-        to fill, (frames, depth).  With CUDA tensors throughout the call runs on torch's current stream without a
-        host sync."""
+        changed (same entities, textures, light and the episode's camera parameters).  A 7-column row
+        (x, z, dir, cam_height, cam_fwd_disp, cam_pitch, cam_fov_y) also sets those camera attributes; NaN in columns
+        3-6 keeps the running episode's value, so an all-NaN 7-column row renders what its 3-column row does.
+        `render_agent=True` also draws the agent's marker triangle at its real pose: a third-person view.
+        A row is skipped when x, z or dir is not finite or |dir| >= 105414350 (beyond the range the glibc-exact sin /
+        cos are validated for), and a 7-column row also when an intrinsic column is +-inf, a given cam_fov_y lies
+        outside (0, 180) or a given |cam_pitch| >= 90.  A skipped row's frame (and depth) in that view is left as it is
+        in `out` / `depth`.  No env state changes.
+        `size` = (W, H) and `samples` (1, 4, 8 or 16) render as the reference does into FrameBuffer(W, H, samples);
+        they default to the batch's observation size and sample count.
+        Returns frames [V, N, *frame] (or [N, *frame]) in the batch's observation layout at that size -- `out` filled
+        in place or a fresh zero tensor -- and, when `depth` is True or an array / tensor float32 [V, N, H, W, 1] (or
+        [N, H, W, 1]) to fill, (frames, depth).  With CUDA tensors throughout the call runs on torch's current stream
+        without a host sync."""
         poses = self._view_rows("render_views", poses)
         one = poses.ndim == 2 if isinstance(poses, np.ndarray) else poses.dim() == 2
         V = 1 if one else int(poses.shape[0])
         lead = () if one else (V,)
-        H, W = self.obs_height, self.obs_width
+        if size is None:
+            W, H = self.obs_width, self.obs_height
+        else:
+            if len(size) != 2 or not all(isinstance(v, (int, np.integer)) and not isinstance(v, bool) and v > 0
+                                         for v in size):
+                raise ValueError("render_views: size must be (width, height), two positive ints, not %r" % (size,))
+            W, H = int(size[0]), int(size[1])
+        if samples is None:
+            samples = self.engine.cfg.msaa_samples
+        elif isinstance(samples, bool) or samples not in (1, 4, 8, 16):
+            raise ValueError("render_views: samples must be 1, 4, 8 or 16, not %r" % (samples,))
+        N = self.num_envs
+        obs_shape = {"hwc": (N, H, W, 3), "cwh": (N, 3, W, H), "grey": (N, H, W, 1)}[self.obs_format]
         host = self.engine.host_memory
         if out is None or depth is True:
             torch = None if host else self._ensure_torch()
@@ -1433,10 +1454,10 @@ class BatchedMiniWorld:
                 (lambda shape, dt: torch.zeros(shape, dtype={np.uint8: torch.uint8, np.float64: torch.float64,
                                                              np.float32: torch.float32}[dt], device=dev))
             if out is None:
-                out = zeros(lead + self.obs_shape, self.obs_dtype)
+                out = zeros(lead + obs_shape, self.obs_dtype)
             if depth is True:
                 depth = zeros(lead + (self.num_envs, H, W, 1), np.float32)
-        for name, arr, shape, dt in (("out", out, lead + self.obs_shape, np.dtype(self.obs_dtype)),
+        for name, arr, shape, dt in (("out", out, lead + obs_shape, np.dtype(self.obs_dtype)),
                                      ("depth", depth, lead + (self.num_envs, H, W, 1), np.dtype(np.float32))):
             if arr is None or arr is False:
                 continue
@@ -1448,7 +1469,8 @@ class BatchedMiniWorld:
         if depth is False:
             depth = None
         stream = None if host else _torch_stream(self._ensure_torch(), self.device)
-        self.engine.render_views(poses, V, obs=out, depth=depth, render_agent=render_agent, stream=stream)
+        self.engine.render_views(poses, V, obs=out, depth=depth, render_agent=render_agent, stream=stream,
+                                 row_width=poses.shape[-1], size=(W, H), samples=int(samples))
         return out if depth is None else (out, depth)
 
     # ------------------------------------------------------------------ state views

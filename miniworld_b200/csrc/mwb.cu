@@ -113,6 +113,7 @@ struct mwb_handle {
   size_t obs_px_bytes;            // bytes per pixel of that layout (3, or 8 for float64 greyscale)
   size_t d_obs_bytes;             // capacity of the d_obs staging buffer
   float* d_depth;
+  size_t d_depth_px;              // capacity of the d_depth staging buffer, in pixels
   int32_t* d_ids;
   int* d_overflow;
   WorldUpload* d_upload;
@@ -148,9 +149,10 @@ struct mwb_handle {
   bool obs_is_peer;               // this launch's observation buffer lives on another GPU (K2 stages whole frames)
   int k2_static_smem;             // static shared memory of the K2 instantiation in use (cudaFuncGetAttributes)
   TriRec* vis_tris;              // scratch of mwb_visible_ents, allocated on first use
-  double* d_view_rows;           // [N][3] staging of host rows for mwb_render_views / mwb_visible_ents_from, on first use
+  double* d_view_rows;           // [N][7] staging of host rows for mwb_render_views_at / mwb_visible_ents_from_at, on first use
   ViewSpec view;                 // what the next render launch draws (agent camera unless mwb_render_top_view)
   int k2_parts;                   // blocks per env frame (1 at 80x60, 4 at 160x120)
+  int sms;                        // the device's multiprocessors (K2's parts per frame depend on them)
 #ifndef MWB_HOSTSIM
   cudaStream_t copy_stream;
   cudaEvent_t chunk_done[MWB_D2H_CHUNKS], copies_done;
@@ -420,9 +422,10 @@ template <int MSAA>
 static void hostsim_render_t(const DevState& S, const RenderAssets& A, const ViewSpec& view, uint8_t* obs, float* depth) {
   const int W = S.obs_w, H = S.obs_h;
   for (int i = 0; i < S.N; ++i) {
-    if (view.mode == 2 && view_row_skipped(view.rows + (size_t)i * 3)) continue;   // like K2: the frame is left as it is
+    const double* row = view.mode == 2 ? view.rows + (size_t)i * view.row_width : nullptr;
+    if (row && view_row_skipped(row, view.row_width)) continue;   // like K2: the frame is left as it is
     Camera cam = view.mode == 1 ? make_top_camera(S, i, view)
-               : view.mode == 2 ? make_row_camera(S, i, view.rows + (size_t)i * 3) : make_camera(S, i);
+               : row ? make_row_camera(S, i, row, view.row_width) : make_camera(S, i);
     FrameMap fm = build_frame_map(S, i, view.mode != 0 && view.render_agent != 0);
     std::vector<TriRec> tris;
     TriRec rec;
@@ -543,7 +546,7 @@ static void hostsim_render(const DevState& S, const RenderAssets& A, const ViewS
   if (obs_out && fmt != MWB_OBS_HWC_U8) {
     const int W = S.obs_w, H = S.obs_h;
     for (int i = 0; i < S.N; ++i)
-      for (int y = 0; y < H && !(view.mode == 2 && view_row_skipped(view.rows + (size_t)i * 3)); ++y)
+      for (int y = 0; y < H && !(view.mode == 2 && view_row_skipped(view.rows + (size_t)i * view.row_width, view.row_width)); ++y)
         for (int x = 0; x < W; ++x) {
           const uint8_t* c = obs + (((size_t)i * H + y) * W + x) * 3;
           if (fmt == MWB_OBS_CWH_U8) {
@@ -561,26 +564,30 @@ static void hostsim_render(const DevState& S, const RenderAssets& A, const ViewS
 // The frame stage holds one env's whole RGB frame (80x60: 14.4 KB) so that it leaves the SM as full 16-byte
 // row-contiguous stores -- what makes the peer-memory observation path efficient over NVLink (8-byte
 // scattered segments reach ~190 GB/s into one GPU, 128-byte lines several times that).
-static int k2_list_bytes(const mwb_handle* h) {
-  const K2Layout L = k2_layout(h->smem_recs, h->tri_cap, h->stage_bytes, k2_halves_per_part(h->S.obs_w, h->S.obs_h, h->k2_parts), 0);
+// A frame's plan depends on its size W x H and on `parts`, the blocks per env frame (k2_parts_for); the handle supplies
+// the triangle capacities and the observation format.
+static int k2_list_bytes(const mwb_handle* h, int W, int H, int parts) {
+  const K2Layout L = k2_layout(h->smem_recs, h->tri_cap, h->stage_bytes, k2_halves_per_part(W, H, parts), 0);
   return (int)L.stage_off;
 }
-static int k2_frame_stage_bytes(const mwb_handle* h) {
-  const int W = h->S.obs_w, H = h->S.obs_h, tiles_x = (W + 7) >> 3;
+static int k2_frame_stage_bytes(const mwb_handle* h, int W, int H, int parts) {
+  const int tiles_x = (W + 7) >> 3;
   // bytes one block stages: the whole frame, or (frames cut into several blocks) its band of whole half-tile rows
-  const size_t rows = h->k2_parts == 1 ? (size_t)H : (size_t)(k2_halves_per_part(W, H, h->k2_parts) / tiles_x) * 4;
+  const size_t rows = parts == 1 ? (size_t)H : (size_t)(k2_halves_per_part(W, H, parts) / tiles_x) * 4;
   const size_t bytes = rows * W * 3;
   if (h->obs_format == MWB_OBS_GREY_F64 || bytes > 16384 || (bytes & 15) != 0 || (W & 7) != 0) return 0;
-  if (h->k2_parts != 1 && (h->obs_format != MWB_OBS_HWC_U8 || (H & 3) != 0)) return 0;
+  if (parts != 1 && (h->obs_format != MWB_OBS_HWC_U8 || (H & 3) != 0)) return 0;
   // Staging pays only when the stores leave the GPU (peer memory of rank 0: full 16-byte address-ordered stores
   // instead of 8-byte row segments, 52 % -> 89 % weak-scaling efficiency on 8 GPUs); for local HBM it costs 6 %.
   if (!h->obs_is_peer) return 0;
   // not at the price of a resident block: three blocks per SM (+ 1 KB each for the system) must still fit in 227 KB
-  const size_t per_block = (size_t)k2_list_bytes(h) + bytes + (size_t)h->k2_static_smem + 1024;
+  const size_t per_block = (size_t)k2_list_bytes(h, W, H, parts) + bytes + (size_t)h->k2_static_smem + 1024;
   if (3 * per_block > 232448) return 0;
   return (int)bytes;      // a multiple of 16: every band starts 16-byte aligned
 }
-static int k2_smem_bytes(const mwb_handle* h) { return k2_list_bytes(h) + k2_frame_stage_bytes(h); }
+static int k2_smem_bytes(const mwb_handle* h, int W, int H, int parts) {
+  return k2_list_bytes(h, W, H, parts) + k2_frame_stage_bytes(h, W, H, parts);
+}
 
 // K2's instantiations, one per block shape x MSAA count x camera kind (the agent's / the top view's, or designed
 // cameras: mwb_render_views); they share one signature.  Block shape on H100 (DESIGN.md
@@ -594,23 +601,36 @@ static const K2Kernel k2_kernels[16] = {
     render_kernel<1, 256, 3, true>, render_kernel<4, 256, 3, true>, render_kernel<8, 256, 3, true>,
     render_kernel<16, 256, 3, true>, render_kernel<1, 320, 3, true>, render_kernel<4, 320, 3, true>,
     render_kernel<8, 320, 3, true>, render_kernel<16, 320, 3, true>};
-static int k2_threads(const mwb_handle* h) { return h->k2_parts == 1 ? 256 : 320; }
-static int k2_index(const mwb_handle* h) {
-  const int m = h->S.msaa;
-  return (h->view.mode == 2 ? 8 : 0) + (h->k2_parts == 1 ? 0 : 4) + (m == 1 ? 0 : m == 4 ? 1 : m == 8 ? 2 : 3);
+static int k2_threads(int parts) { return parts == 1 ? 256 : 320; }
+static int k2_index(int msaa, int parts, bool views) {
+  return (views ? 8 : 0) + (parts == 1 ? 0 : 4) + (msaa == 1 ? 0 : msaa == 4 ? 1 : msaa == 8 ? 2 : 3);
 }
 
 // The opt-in for large dynamic shared memory is an attribute of the kernel FUNCTION (per device), not of a
 // handle: several handles with different triangle capacities share it, so it is only ever raised.
 static int g_k2_smem[16][16] = {};
-static int ensure_k2_smem(mwb_handle* h, int smem) {
-  int& granted = g_k2_smem[h->cfg.device & 15][k2_index(h)];
+static int ensure_k2_smem(mwb_handle* h, int index, int smem) {
+  int& granted = g_k2_smem[h->cfg.device & 15][index];
   if (smem <= granted) return 0;
-  if (cudaFuncSetAttribute(k2_kernels[k2_index(h)], cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) return -1;
+  if (cudaFuncSetAttribute(k2_kernels[index], cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) return -1;
   granted = smem;
   return 0;
 }
 #endif
+
+// Blocks per env frame of a W x H frame for N envs on `sms` multiprocessors: at least one per 150 half-tiles (80x60
+// -> 1, 160x120 -> 4), and more when few envs are resident so that the grid still covers ~4 waves of the SMs x 3 block
+// slots (each part redoes the cheap geometry phase); never fewer than 30 half-tiles per part
+static int k2_parts_for(int W, int H, int N, int sms) {
+  const int slots = 4 * 3 * sms;
+  const int halves = ((W + 7) / 8) * ((H + 3) / 4);
+  const int base = (halves + 149) / 150, want = (slots + N - 1) / N;
+  const int maxp = halves / 30 > 1 ? halves / 30 : 1;
+  int parts = base > want ? base : want;
+  if (parts > maxp) parts = maxp;
+  if (parts < 1) parts = 1;
+  return parts;
+}
 
 // K2's triangle-list residence and quad staging.  Every room quad and box face can yield two set-up triangles; lists
 // of up to MWB_SMEM_TRI_CAP records live in shared memory, larger ones in HBM (S.room_tris), and a level's static
@@ -646,11 +666,12 @@ static void plan_k2(mwb_handle* h) {
   }
 }
 
-// HBM triangle lists for every env (level changes can move any env into a level that needs them)
-static int ensure_room_tris(mwb_handle* h) {
+// HBM triangle lists for every env (level changes can move any env into a level that needs them), for frames cut
+// into `parts` blocks; they only ever grow
+static int ensure_room_tris(mwb_handle* h, int parts) {
   bool any = false;
   for (const LevelDev& D : h->levels) any = any || D.tris_hbm;
-  const size_t recs = (size_t)h->S.N * h->k2_parts * h->tri_cap;
+  const size_t recs = (size_t)h->S.N * parts * h->tri_cap;
   if (!any || recs <= h->room_tris_recs) return MWB_OK;
   auto it = std::find(h->allocs.begin(), h->allocs.end(), (void*)h->S.room_tris);
   if (h->S.room_tris && it != h->allocs.end()) {
@@ -671,8 +692,9 @@ static void k2_report(mwb_handle* h) {
 #ifndef MWB_HOSTSIM
   if (!getenv("MWB_DEBUG")) return;
   int nb = 0;
-  const int launch_smem = k2_smem_bytes(h);
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k2_kernels[k2_index(h)], k2_threads(h), launch_smem);
+  const int launch_smem = k2_smem_bytes(h, h->S.obs_w, h->S.obs_h, h->k2_parts);
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k2_kernels[k2_index(h->S.msaa, h->k2_parts, false)], k2_threads(h->k2_parts),
+                                                launch_smem);
   std::string levels;
   if (h->level_mazes) {
     levels = ", shared-memory records " + std::to_string(h->smem_recs) + ", HBM lists: levels";
@@ -685,7 +707,7 @@ static void k2_report(mwb_handle* h) {
     if (none) levels += " none";
   }
   fprintf(stderr, "[mwb] K2 %d threads, %dx MSAA: dynamic smem %d B (local destination), parts %d, resident blocks/SM %d%s\n",
-          k2_threads(h), h->S.msaa, launch_smem, h->k2_parts, nb, levels.c_str());
+          k2_threads(h->k2_parts), h->S.msaa, launch_smem, h->k2_parts, nb, levels.c_str());
 #else
   (void)h;
 #endif
@@ -810,6 +832,7 @@ extern "C" int mwb_create(const mwb_config* cfg, mwb_handle** out) {
   if (!rc) rc = alloc_arr(h, &h->d_obs, N * (size_t)S.obs_w * S.obs_h * 3);
   h->d_obs_bytes = N * (size_t)S.obs_w * S.obs_h * 3;
   if (!rc) rc = alloc_arr(h, &h->d_depth, N * (size_t)S.obs_w * S.obs_h);
+  h->d_depth_px = N * (size_t)S.obs_w * S.obs_h;
   if (!rc) rc = alloc_arr(h, &h->d_ids, N);
   if (!rc) rc = alloc_arr(h, &h->d_overflow, 1);
   S.fault = h->d_overflow;
@@ -836,42 +859,32 @@ extern "C" int mwb_create(const mwb_config* cfg, mwb_handle** out) {
   dev_memset(S.carrying, 0xFF, N * sizeof(int32_t));
   // every room quad and box face can yield two set-up triangles.  Up to 512 of them live in
   // shared memory; larger levels (Maze) keep the per-env lists in HBM instead.
-  {
-    // blocks per env frame: at least one per 150 half-tiles (80x60 -> 1, 160x120 -> 4), and more
-    // when few envs are resident so that the grid still covers ~4 waves of the SMs x 3 block
-    // slots (each part redoes the cheap geometry phase); never fewer than 30 half-tiles per part
-    int sms = 132;                   // H100 SXM
+  h->sms = 132;                      // H100 SXM
 #ifndef MWB_HOSTSIM
-    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, cfg->device) != cudaSuccess) {
-      cudaGetLastError();
-      sms = 132;
-    }
-#endif
-    const int slots = 4 * 3 * sms;
-    const int halves = ((cfg->obs_width + 7) / 8) * ((cfg->obs_height + 3) / 4);
-    const int base = (halves + 149) / 150, want = (slots + cfg->num_envs - 1) / cfg->num_envs;
-    const int maxp = halves / 30 > 1 ? halves / 30 : 1;
-    h->k2_parts = base > want ? base : want;
-    if (h->k2_parts > maxp) h->k2_parts = maxp;
-    if (h->k2_parts < 1) h->k2_parts = 1;
+  if (cudaDeviceGetAttribute(&h->sms, cudaDevAttrMultiProcessorCount, cfg->device) != cudaSuccess) {
+    cudaGetLastError();
+    h->sms = 132;
   }
+#endif
+  h->k2_parts = k2_parts_for(cfg->obs_width, cfg->obs_height, cfg->num_envs, h->sms);
   plan_k2(h);
-  if (ensure_room_tris(h) || upload_levels(h)) {
+  if (ensure_room_tris(h, h->k2_parts) || upload_levels(h)) {
     mwb_destroy(h);
     return MWB_ECUDA;
   }
 #ifndef MWB_HOSTSIM
   {
     cudaFuncAttributes fa;
-    if (cudaFuncGetAttributes(&fa, k2_kernels[k2_index(h)]) == cudaSuccess) {
+    if (cudaFuncGetAttributes(&fa, k2_kernels[k2_index(h->S.msaa, h->k2_parts, false)]) == cudaSuccess) {
       h->k2_static_smem = (int)fa.sharedSizeBytes;
     } else {
       cudaGetLastError();
       h->k2_static_smem = 19456;
     }
   }
-  const int smem = k2_smem_bytes(h) + 16384;     // room for a frame stage whatever observation layout is chosen later
-  if (ensure_k2_smem(h, smem)) {
+  // room for a frame stage whatever observation layout is chosen later
+  const int smem = k2_smem_bytes(h, h->S.obs_w, h->S.obs_h, h->k2_parts) + 16384;
+  if (ensure_k2_smem(h, k2_index(h->S.msaa, h->k2_parts, false), smem)) {
     mwb_destroy(h);
     return fail(MWB_ECUDA, "cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed");
   }
@@ -1566,7 +1579,7 @@ extern "C" int mwb_set_level_maze(mwb_handle* h, int level, const mwb_maze_desc*
   h->levels[level].env_worlds = 1;
   h->level_quads[level] = 8 * cells - 2;
   plan_k2(h);
-  if ((rc = ensure_room_tris(h)) != 0 || (rc = put_maze(h, level, mz)) != 0) return rc;
+  if ((rc = ensure_room_tris(h, h->k2_parts)) != 0 || (rc = put_maze(h, level, mz)) != 0) return rc;
   k2_report(h);
   return MWB_OK;
 }
@@ -1599,7 +1612,7 @@ extern "C" int mwb_enable_maze_layouts(mwb_handle* h) {
   if (h->level_mazes) {   // K2's per-level capacity and the HBM lists from the all-open bound
     h->level_quads = quads;
     plan_k2(h);
-    if ((rc = ensure_room_tris(h)) != 0 || (rc = upload_levels(h)) != 0) return rc;
+    if ((rc = ensure_room_tris(h, h->k2_parts)) != 0 || (rc = upload_levels(h)) != 0) return rc;
     k2_report(h);
   }
   MazeLayouts& Y = h->layouts_h;
@@ -2217,8 +2230,9 @@ extern "C" int mwb_profile_read(mwb_handle* h, double* k1_ms, double* k2_ms, int
 }
 
 // ------------------------------------------------------------------ ABI: the hot path
-// Launch K2 for envs [env0, env0 + count) (obs / depth point at env 0 of the full buffers).
-static int launch_k2(mwb_handle* h, uint8_t* obs, float* depth, int env0, int count, stream_t s) {
+// Launch K2 for envs [env0, env0 + count) (obs / depth point at env 0 of the full buffers) of state S (the handle's,
+// or a copy with another frame size and sample count), frames cut into `parts` blocks.
+static int launch_k2(mwb_handle* h, const DevState& S, int parts, uint8_t* obs, float* depth, int env0, int count, stream_t s) {
 #ifndef MWB_HOSTSIM
   if (obs != h->peer_checked) {         // the observation destination rarely changes: query its home device once
     cudaPointerAttributes pa;
@@ -2228,13 +2242,13 @@ static int launch_k2(mwb_handle* h, uint8_t* obs, float* depth, int env0, int co
     cudaGetLastError();
   }
   h->obs_is_peer = h->obs_peer_hint >= 0 ? h->obs_peer_hint != 0 : h->peer_result;
-  const int smem = k2_smem_bytes(h), fstage = k2_frame_stage_bytes(h);
-  const K2Layout lay = k2_layout(h->smem_recs, h->tri_cap, h->stage_bytes, k2_halves_per_part(h->S.obs_w, h->S.obs_h, h->k2_parts), fstage);
-  if (ensure_k2_smem(h, smem)) return fail(MWB_ECUDA, "cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed");
+  const int W = S.obs_w, H = S.obs_h, index = k2_index(S.msaa, parts, h->view.mode == 2);
+  const int smem = k2_smem_bytes(h, W, H, parts), fstage = k2_frame_stage_bytes(h, W, H, parts);
+  const K2Layout lay = k2_layout(h->smem_recs, h->tri_cap, h->stage_bytes, k2_halves_per_part(W, H, parts), fstage);
+  if (ensure_k2_smem(h, index, smem)) return fail(MWB_ECUDA, "cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed");
   prof_mark(h, h->ev_k2, s);
-  k2_kernels[k2_index(h)]<<<count * h->k2_parts, k2_threads(h), smem, s>>>(h->S, h->A, h->view, h->obs_format, obs, depth, env0,
-                                                                          h->k2_parts, h->tri_cap, h->stage_bytes, fstage, lay,
-                                                                          h->d_overflow);
+  k2_kernels[index]<<<count * parts, k2_threads(parts), smem, s>>>(S, h->A, h->view, h->obs_format, obs, depth, env0, parts,
+                                                                   h->tri_cap, h->stage_bytes, fstage, lay, h->d_overflow);
   prof_mark(h, h->ev_k2, s);
   h->launches++;
   CK(cudaGetLastError());
@@ -2245,31 +2259,32 @@ static int launch_k2(mwb_handle* h, uint8_t* obs, float* depth, int env0, int co
 // Render all envs.  With host destinations the frame batch is cut into chunks: chunk c is
 // copied device->host on a second stream while chunk c + 1 is being rasterised, so the PCIe
 // transfer of the observations overlaps the render instead of following it.
-static int launch_render(mwb_handle* h, uint8_t* obs, float* depth, stream_t s, uint8_t* host_obs = nullptr,
-                         float* host_depth = nullptr) {
+// S and parts as launch_k2 takes them.
+static int launch_render(mwb_handle* h, const DevState& S, int parts, uint8_t* obs, float* depth, stream_t s,
+                         uint8_t* host_obs = nullptr, float* host_depth = nullptr) {
   if (!h->A.tex) return fail(MWB_ESTATE, "textures not uploaded");
 #ifndef MWB_HOSTSIM
   {
-    const long long threads = (long long)h->S.N * (6 + 2 * h->S.E);
-    if (h->view.mode == 2) frame_trig_kernel<true><<<(unsigned)((threads + 127) / 128), 128, 0, s>>>(h->S, h->view);
-    else frame_trig_kernel<false><<<(unsigned)((threads + 127) / 128), 128, 0, s>>>(h->S, h->view);
+    const long long threads = (long long)S.N * (6 + 2 * S.E);
+    if (h->view.mode == 2) frame_trig_kernel<true><<<(unsigned)((threads + 127) / 128), 128, 0, s>>>(S, h->view);
+    else frame_trig_kernel<false><<<(unsigned)((threads + 127) / 128), 128, 0, s>>>(S, h->view);
     h->launches++;
     CK(cudaGetLastError());
   }
-  if (h->S.mesh_cap > 0) {
-    if (h->view.mode == 2) mesh_setup_kernel<true><<<dim3(h->S.N, h->S.E), 256, 0, s>>>(h->S, h->A, h->view);
-    else mesh_setup_kernel<false><<<dim3(h->S.N, h->S.E), 256, 0, s>>>(h->S, h->A, h->view);
+  if (S.mesh_cap > 0) {
+    if (h->view.mode == 2) mesh_setup_kernel<true><<<dim3(S.N, S.E), 256, 0, s>>>(S, h->A, h->view);
+    else mesh_setup_kernel<false><<<dim3(S.N, S.E), 256, 0, s>>>(S, h->A, h->view);
     h->launches++;
     CK(cudaGetLastError());
   }
-  const int N = h->S.N;
-  const size_t px = (size_t)h->S.obs_w * h->S.obs_h;
+  const int N = S.N;
+  const size_t px = (size_t)S.obs_w * S.obs_h;
   const bool pipelined = (host_obs || host_depth) && N >= 256;
   int chunks = pipelined ? MWB_D2H_CHUNKS : 1;
   while (chunks > 1 && N / chunks < 256) --chunks;   // keep every launch a few hundred blocks wide
   for (int c = 0; c < chunks; ++c) {
     const int e0 = (int)((long long)N * c / chunks), e1 = (int)((long long)N * (c + 1) / chunks);
-    int rc = launch_k2(h, obs, depth, e0, e1 - e0, s);
+    int rc = launch_k2(h, S, parts, obs, depth, e0, e1 - e0, s);
     if (rc) return rc;
     if (pipelined) {
       CK(cudaEventRecord(h->chunk_done[c], s));
@@ -2289,7 +2304,8 @@ static int launch_render(mwb_handle* h, uint8_t* obs, float* depth, stream_t s, 
     CK(cudaStreamWaitEvent(s, h->copies_done, 0));   // later work on s (and its sync) sees the copies
   }
 #else
-  hostsim_render(h->S, h->A, h->view, h->obs_format, obs, depth);
+  (void)parts;
+  hostsim_render(S, h->A, h->view, h->obs_format, obs, depth);
 #endif
   return MWB_OK;
 }
@@ -2349,8 +2365,9 @@ extern "C" int mwb_step(mwb_handle* h, const int32_t* actions, const double* ste
   if (h->S.nav && launch_nav(h, s)) return MWB_ECUDA;
   const bool obs_host = obs && !is_device_ptr(obs), depth_host = depth && !is_device_ptr(depth);
   if (obs || depth) {
-    int rc = launch_render(h, obs ? (obs_host ? h->d_obs : obs) : nullptr, depth ? (depth_host ? h->d_depth : depth) : nullptr, s,
-                           obs_host ? obs : nullptr, depth_host ? depth : nullptr);
+    int rc = launch_render(h, h->S, h->k2_parts, obs ? (obs_host ? h->d_obs : obs) : nullptr,
+                           depth ? (depth_host ? h->d_depth : depth) : nullptr, s, obs_host ? obs : nullptr,
+                           depth_host ? depth : nullptr);
     if (rc) return rc;
   }
   return finish_outputs(h, obs, obs_host, depth, depth_host, reward, terminated, truncated, s, stream != nullptr);
@@ -2361,8 +2378,9 @@ extern "C" int mwb_render_obs(mwb_handle* h, uint8_t* obs, float* depth, void* s
   stream_t s = stream ? (stream_t)stream : h->stream;
   if (stream_enter(h, s)) return MWB_ECUDA;
   const bool obs_host = obs && !is_device_ptr(obs), depth_host = depth && !is_device_ptr(depth);
-  int rc = launch_render(h, obs ? (obs_host ? h->d_obs : obs) : nullptr, depth ? (depth_host ? h->d_depth : depth) : nullptr, s,
-                         obs_host ? obs : nullptr, depth_host ? depth : nullptr);
+  int rc = launch_render(h, h->S, h->k2_parts, obs ? (obs_host ? h->d_obs : obs) : nullptr,
+                         depth ? (depth_host ? h->d_depth : depth) : nullptr, s, obs_host ? obs : nullptr,
+                         depth_host ? depth : nullptr);
   if (rc) return rc;
   return finish_outputs(h, obs, obs_host, depth, depth_host, nullptr, nullptr, nullptr, s, stream != nullptr);
 }
@@ -2412,35 +2430,71 @@ extern "C" int mwb_render_top_view(mwb_handle* h, const double extents[4], int r
   h->view.r = extents[1];
   h->view.b = -extents[3];
   h->view.t = -extents[2];
-  int rc = launch_render(h, obs_host ? h->d_obs : obs, nullptr, s, obs_host ? obs : nullptr, nullptr);
+  int rc = launch_render(h, h->S, h->k2_parts, obs_host ? h->d_obs : obs, nullptr, s, obs_host ? obs : nullptr, nullptr);
   memset(&h->view, 0, sizeof(ViewSpec));
   if (rc) return rc;
   return finish_outputs(h, obs, obs_host, nullptr, false, nullptr, nullptr, nullptr, s, stream != nullptr);
 }
 
-// Device rows of a designed view: `poses` itself, or its [N][3] block uploaded to the handle's staging (host rows).
-static const double* device_rows(mwb_handle* h, const double* poses, stream_t s) {
+// Device rows of a designed view: `poses` itself, or its [N][width] block uploaded to the handle's staging (host rows).
+static const double* device_rows(mwb_handle* h, const double* poses, int width, stream_t s) {
   if (is_device_ptr(poses)) return poses;
-  if (!h->d_view_rows && alloc_arr(h, &h->d_view_rows, (size_t)h->S.N * 3)) return nullptr;
-  if (h2d(h->d_view_rows, poses, (size_t)h->S.N * 3 * sizeof(double), s) != 0) return nullptr;
+  if (!h->d_view_rows && alloc_arr(h, &h->d_view_rows, (size_t)h->S.N * 7)) return nullptr;
+  if (h2d(h->d_view_rows, poses, (size_t)h->S.N * width * sizeof(double), s) != 0) return nullptr;
   return h->d_view_rows;
+}
+
+// Replace a staging buffer by one of at least `need` elements (contents not kept); buffers only ever grow.
+template <typename T>
+static int grow_staging(mwb_handle* h, T** buf, size_t* cap, size_t need) {
+  if (need <= *cap) return 0;
+  auto it = std::find(h->allocs.begin(), h->allocs.end(), (void*)*buf);
+  if (*buf && it != h->allocs.end()) {
+    dev_free(*buf);
+    h->allocs.erase(it);
+  }
+  *buf = nullptr;
+  *cap = 0;
+  if (alloc_arr(h, buf, need)) return -1;
+  *cap = need;
+  return 0;
 }
 
 extern "C" int mwb_render_views(mwb_handle* h, const double* poses, int views, int render_agent, uint8_t* obs, float* depth,
                                 void* stream) {
-  if (!h || !poses || (!obs && !depth)) return fail(MWB_EINVAL, "null argument");
+  if (!h) return fail(MWB_EINVAL, "null argument");
+  return mwb_render_views_at(h, poses, 3, views, h->S.obs_w, h->S.obs_h, h->S.msaa, render_agent, obs, depth, stream);
+}
+
+extern "C" int mwb_render_views_at(mwb_handle* h, const double* rows, int row_width, int views, int width, int height,
+                                   int samples, int render_agent, uint8_t* obs, float* depth, void* stream) {
+  if (!h || !rows || (!obs && !depth)) return fail(MWB_EINVAL, "null argument");
   if (views <= 0) return fail(MWB_EINVAL, "views must be positive");
+  if (row_width != 3 && row_width != 7) return fail(MWB_EINVAL, "row_width must be 3 or 7");
+  if (width <= 0 || height <= 0) return fail(MWB_EINVAL, "width and height must be positive");
+  if (samples != 1 && samples != 4 && samples != 8 && samples != 16) return fail(MWB_EINVAL, "samples must be 1, 4, 8 or 16");
   stream_t s = stream ? (stream_t)stream : h->stream;
   if (stream_enter(h, s)) return MWB_ECUDA;
-  const size_t N = h->S.N, px = (size_t)h->S.obs_w * h->S.obs_h;
+  const size_t N = h->S.N, px = (size_t)width * height;
   const size_t frame_bytes = N * px * h->obs_px_bytes, depth_bytes = N * px * sizeof(float);
   const bool obs_host = obs && !is_device_ptr(obs), depth_host = depth && !is_device_ptr(depth);
+  // frames of another size or sample count: the call runs on a copy of the state with those, and the frames are cut
+  // into the blocks K2 would use for a batch of that size (the handle's own plan when both are the batch's)
+  const int parts = k2_parts_for(width, height, (int)N, h->sms);
+  if (ensure_room_tris(h, parts)) return MWB_ECUDA;
+  if ((obs_host && grow_staging(h, &h->d_obs, &h->d_obs_bytes, frame_bytes)) ||
+      (depth_host && grow_staging(h, &h->d_depth, &h->d_depth_px, N * px)))
+    return fail(MWB_ECUDA, "staging allocation failed");
+  DevState S = h->S;
+  S.obs_w = width;
+  S.obs_h = height;
+  S.msaa = samples;
   int rc = MWB_OK;
   for (int v = 0; v < views && rc == MWB_OK; ++v) {
     uint8_t* obs_v = obs ? obs + (size_t)v * frame_bytes : nullptr;
     float* depth_v = depth ? depth + (size_t)v * N * px : nullptr;
-    const double* rows = device_rows(h, poses + (size_t)v * N * 3, s);
-    if (!rows) { rc = fail(MWB_ECUDA, "row upload failed"); break; }
+    const double* dev_rows = device_rows(h, rows + (size_t)v * N * row_width, row_width, s);
+    if (!dev_rows) { rc = fail(MWB_ECUDA, "row upload failed"); break; }
     // host destinations: the staging starts as the caller's frames, so that skipped rows come back unchanged
     if ((obs_host && h2d(h->d_obs, obs_v, frame_bytes, s) != 0) || (depth_host && h2d(h->d_depth, depth_v, depth_bytes, s) != 0)) {
       rc = fail(MWB_ECUDA, "staging upload failed");
@@ -2448,9 +2502,11 @@ extern "C" int mwb_render_views(mwb_handle* h, const double* poses, int views, i
     }
     h->view.mode = 2;
     h->view.render_agent = render_agent != 0;
-    h->view.rows = rows;
-    rc = launch_render(h, obs ? (obs_host ? h->d_obs : obs_v) : nullptr, depth ? (depth_host ? h->d_depth : depth_v) : nullptr, s,
-                       obs_host ? obs_v : nullptr, depth_host ? depth_v : nullptr);
+    h->view.rows = dev_rows;
+    h->view.row_width = row_width;
+    rc = launch_render(h, S, parts, obs ? (obs_host ? h->d_obs : obs_v) : nullptr,
+                       depth ? (depth_host ? h->d_depth : depth_v) : nullptr, s, obs_host ? obs_v : nullptr,
+                       depth_host ? depth_v : nullptr);
     memset(&h->view, 0, sizeof(ViewSpec));
     if (rc == MWB_OK && !h->frames_copied) {
       if ((obs_host && d2h(obs_v, h->d_obs, frame_bytes, s) != 0) || (depth_host && d2h(depth_v, h->d_depth, depth_bytes, s) != 0))
@@ -2465,8 +2521,14 @@ extern "C" int mwb_render_views(mwb_handle* h, const double* poses, int views, i
   return MWB_OK;
 }
 
-// get_visible_ents from the agent's camera (rows null) or from designed cameras ([N][3] rows, device or host)
-static int visible_ents_impl(mwb_handle* h, const double* poses, uint32_t* mask, void* stream) {
+// get_visible_ents from the agent's camera (rows null) or from designed cameras ([N][row_width] rows, device or host)
+#ifndef MWB_HOSTSIM
+typedef decltype(&visible_ents_kernel<1, 3>) VisKernel;
+static const VisKernel vis_kernels[2][4] = {
+    {visible_ents_kernel<1, 3>, visible_ents_kernel<4, 3>, visible_ents_kernel<8, 3>, visible_ents_kernel<16, 3>},
+    {visible_ents_kernel<1, 7>, visible_ents_kernel<4, 7>, visible_ents_kernel<8, 7>, visible_ents_kernel<16, 7>}};
+#endif
+static int visible_ents_impl(mwb_handle* h, const double* poses, int row_width, uint32_t* mask, void* stream) {
   if (!h || !mask) return fail(MWB_EINVAL, "null argument");
   if (!h->have_protos) return fail(MWB_ESTATE, "protos not set");
   stream_t s = stream ? (stream_t)stream : h->stream;
@@ -2477,26 +2539,25 @@ static int visible_ents_impl(mwb_handle* h, const double* poses, uint32_t* mask,
   uint32_t* d_mask = host ? reinterpret_cast<uint32_t*>(h->d_ids) : mask;   // d_ids: N x int32 staging, free between calls
   const double* rows = nullptr;
   if (poses) {
-    rows = device_rows(h, poses, s);
+    rows = device_rows(h, poses, row_width, s);
     if (!rows) return fail(MWB_ECUDA, "row upload failed");
     // skipped rows leave their entries: the staging starts as the caller's mask
     if (host && h2d(d_mask, mask, (size_t)N * sizeof(uint32_t), s) != 0) return fail(MWB_ECUDA, "staging upload failed");
   }
 #ifndef MWB_HOSTSIM
-  switch (h->S.msaa) {
-    case 1: visible_ents_kernel<1><<<N, 256, 0, s>>>(h->S, h->A, h->vis_tris, cap, box0, d_mask, rows); break;
-    case 4: visible_ents_kernel<4><<<N, 256, 0, s>>>(h->S, h->A, h->vis_tris, cap, box0, d_mask, rows); break;
-    case 16: visible_ents_kernel<16><<<N, 256, 0, s>>>(h->S, h->A, h->vis_tris, cap, box0, d_mask, rows); break;
-    default: visible_ents_kernel<8><<<N, 256, 0, s>>>(h->S, h->A, h->vis_tris, cap, box0, d_mask, rows); break;
+  {
+    const int m = h->S.msaa, mi = m == 1 ? 0 : m == 4 ? 1 : m == 16 ? 3 : 2;
+    vis_kernels[row_width == 7 ? 1 : 0][mi]<<<N, 256, 0, s>>>(h->S, h->A, h->vis_tris, cap, box0, d_mask, rows);
   }
   h->launches++;
   CK(cudaGetLastError());
 #else
   const int W = h->S.obs_w, H = h->S.obs_h, M = h->S.msaa;
   for (int i = 0; i < N; ++i) {
-    if (rows && view_row_skipped(rows + (size_t)i * 3)) continue;
+    const double* row = rows ? rows + (size_t)i * row_width : nullptr;
+    if (row && view_row_skipped(row, row_width)) continue;
     TriRec* tris = h->vis_tris + (size_t)i * cap;
-    const Camera cam = rows ? make_row_camera(h->S, i, rows + (size_t)i * 3) : make_camera(h->S, i);
+    const Camera cam = row ? make_row_camera(h->S, i, row, row_width) : make_camera(h->S, i);
     int ent_slot[32];
     const int n_query = queried_entities(h->S, i, ent_slot);
     int n_room = 0;
@@ -2535,11 +2596,17 @@ static int visible_ents_impl(mwb_handle* h, const double* poses, uint32_t* mask,
   return MWB_OK;
 }
 
-extern "C" int mwb_visible_ents(mwb_handle* h, uint32_t* mask, void* stream) { return visible_ents_impl(h, nullptr, mask, stream); }
+extern "C" int mwb_visible_ents(mwb_handle* h, uint32_t* mask, void* stream) { return visible_ents_impl(h, nullptr, 3, mask, stream); }
 
 extern "C" int mwb_visible_ents_from(mwb_handle* h, const double* poses, uint32_t* mask, void* stream) {
   if (!poses) return fail(MWB_EINVAL, "null argument");
-  return visible_ents_impl(h, poses, mask, stream);
+  return visible_ents_impl(h, poses, 3, mask, stream);
+}
+
+extern "C" int mwb_visible_ents_from_at(mwb_handle* h, const double* rows, int row_width, uint32_t* mask, void* stream) {
+  if (!rows) return fail(MWB_EINVAL, "null argument");
+  if (row_width != 3 && row_width != 7) return fail(MWB_EINVAL, "row_width must be 3 or 7");
+  return visible_ents_impl(h, rows, row_width, mask, stream);
 }
 
 // ------------------------------------------------------------------ ABI: snapshot / restore

@@ -103,8 +103,9 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 
 // ---- per-frame trigonometry: thread (env i, k): k < 6 the camera's cos / sin, else entity slot (k - 6) / 2 -----------
-// (VIEWS: the launch draws designed cameras, view.mode 2, and the heading comes from env i's row.  The designed-camera
-// path is a separate instantiation of this kernel, the mesh pre-pass and K2, so the agent-camera code is unchanged.)
+// (VIEWS: the launch draws designed cameras, view.mode 2, and the heading -- with 7-column rows also the pitch and field
+// of view where given -- comes from env i's row.  The designed-camera path is a separate instantiation of this kernel,
+// the mesh pre-pass and K2, so the agent-camera code is unchanged.)
 template <bool VIEWS>
 __global__ void frame_trig_kernel(DevState S, ViewSpec view) {
   const int per = 6 + 2 * S.E;
@@ -116,8 +117,9 @@ __global__ void frame_trig_kernel(DevState S, ViewSpec view) {
     double ang[3];
     camera_angles(S, i, ang);
     if (VIEWS) {
-      if (view_row_skipped(view.rows + (size_t)i * 3)) return;      // no camera for a skipped row
-      ang[0] = view.rows[(size_t)i * 3 + 2];
+      const double* row = view.rows + (size_t)i * view.row_width;
+      if (view_row_skipped(row, view.row_width)) return;      // no camera for a skipped row
+      view_row_angles(row, view.row_width, ang);
     }
     S.cam_trig[(size_t)k * N + i] = (k & 1) ? mwb_libm::sin_glibc(ang[k >> 1]) : mwb_libm::cos_glibc(ang[k >> 1]);
     return;
@@ -141,7 +143,7 @@ __global__ void __launch_bounds__(256) mesh_setup_kernel(DevState S, RenderAsset
   __shared__ int box[4];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   MeshSegInfo* info = S.mesh_seg + (size_t)i * S.E + e;
-  if (VIEWS && view_row_skipped(view.rows + (size_t)i * 3)) return;   // K2 skips this env's frame too
+  if (VIEWS && view_row_skipped(view.rows + (size_t)i * view.row_width, view.row_width)) return;   // K2 skips this env's frame too
   const int p = e == S.ghost_slot[i] ? S.ghost_proto[i] : (e < S.num_slots[i] ? S.ent_proto[e * N + i] : -1);
   if (p < 0 || S.protos[p].kind != MWB_KIND_MESH) {
     if (tid == 0) info->count = 0;
@@ -304,7 +306,7 @@ render_kernel(DevState S, RenderAssets A, ViewSpec view, int fmt, uint8_t* __res
   // rasterises its share of the half-tiles), which evens out the load when few envs are resident
   const int i = env0 + (int)blockIdx.x / parts, part = (int)blockIdx.x % parts;
   // a skipped row of a designed view: the whole block leaves before any barrier (the condition is the block's env's)
-  if (VIEWS && view_row_skipped(view.rows + (size_t)i * 3)) return;
+  if (VIEWS && view_row_skipped(view.rows + (size_t)i * view.row_width, view.row_width)) return;
   // set-up triangles of rooms + boxes: shared memory, or this env's HBM block for big levels (per level: the
   // env's own capacity bounds its list; tri_cap, the largest level's, is the stride of the HBM blocks)
   const LevelDev& lv = env_level_of(S, i);

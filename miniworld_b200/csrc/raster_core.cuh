@@ -110,13 +110,17 @@ struct Camera {
 // Which view a render launch draws: the agent's camera (render_obs, miniworld.py:1177-1221), the
 // orthographic map of render_top_view (miniworld.py:1088-1175): glOrtho(l, r, b, t, -100, 100) under
 // the model-view that maps world (x, y, z) to eye (x, -z, y), plus the agent's marker triangle, or a
-// designed camera (mwb_render_views): render_obs with the agent moved to env i's row (x, z, dir) of `rows`.
+// designed camera (mwb_render_views_at): render_obs with the agent moved to env i's row (x, z, dir) of `rows`, and
+// with a 7-column row also the row's (cam_height, cam_fwd_disp, cam_pitch, cam_fov_y) where given (not NaN).
 struct ViewSpec {
   int mode;                      // 0 = agent camera, 1 = top view, 2 = designed camera
   int render_agent;              // top view / designed camera: draw Agent.render()'s triangle (entity.py:518-539)
   union {
     struct { double l, r, b, t; };   // glOrtho extents (top view)
-    const double* rows;              // designed camera: [N][3] rows (x, z, dir) of the current view
+    struct {                         // designed camera: [N][row_width] rows of the current view, row_width 3 or 7
+      const double* rows;
+      int row_width;
+    };
   };
 };
 
@@ -124,11 +128,34 @@ struct ViewSpec {
 // (libm_sincos.cuh); beyond it their table index is meaningless.
 #define MWB_VIEW_MAX_DIR 105414350.0
 
-// designed camera: a row with a non-finite entry or |dir| >= MWB_VIEW_MAX_DIR is skipped (its frame is left as it
-// is; no trig is evaluated for it).  x * 0 + z * 0 is +-0 when both are finite and NaN otherwise, so |dir| plus it is
-// |dir| exactly or NaN, and one comparison (false for NaN) covers the row: K2's default path keeps its spill count.
-MWB_DEV bool view_row_skipped(const double* row) {
-  return !(fabs(row[2]) + (row[0] * 0.0 + row[1] * 0.0) < MWB_VIEW_MAX_DIR);
+// designed camera: a row with a non-finite x, z or dir or with |dir| >= MWB_VIEW_MAX_DIR is skipped (its frame is left
+// as it is; no trig is evaluated for it).  x * 0 + z * 0 is +-0 when both are finite and NaN otherwise, so |dir| plus
+// it is |dir| exactly or NaN, and one comparison (false for NaN) covers a 3-column row: K2's default path keeps its
+// spill count.  A 7-column row is also skipped when an intrinsic column is +-inf, a given cam_pitch has |pitch| >= 90
+// (gluLookAt's view direction would be parallel to its up vector) or a given cam_fov_y lies outside (0, 180).
+MWB_DEV bool view_row_skipped(const double* row, int width = 3) {
+  if (!(fabs(row[2]) + (row[0] * 0.0 + row[1] * 0.0) < MWB_VIEW_MAX_DIR)) return true;
+  if (width == 3) return false;
+  const double h = row[3], fd = row[4], pitch = row[5], fov = row[6];
+  if (fabs(h) > 1.7976931348623157e308 || fabs(fd) > 1.7976931348623157e308) return true;
+  if (pitch == pitch && !(fabs(pitch) < 90.0)) return true;
+  return fov == fov && !(fov > 0.0 && fov < 180.0);
+}
+
+// Camera parameter k (0 cam_height, 1 cam_fwd_disp, 2 cam_pitch, 3 cam_fov_y) of env i under a designed-camera row:
+// a 7-column row's value where given, else the running episode's.
+MWB_DEV double view_row_cam(const DevState& S, int i, const double* row, int width, int k) {
+  if (width == 7 && row[3 + k] == row[3 + k]) return row[3 + k];
+  return S.cam[(size_t)k * S.N + i];
+}
+
+// The camera angles of a designed-camera row, over those of env i's camera (camera_angles): the heading, and with a
+// 7-column row the pitch and half the field of view where given, through the same float64 steps.
+MWB_DEV void view_row_angles(const double* row, int width, double ang[3]) {
+  ang[0] = row[2];
+  if (width != 7) return;
+  if (row[5] == row[5]) ang[1] = d_div(d_mul(row[5], 3.141592653589793), 180.0);
+  if (row[6] == row[6]) ang[2] = d_div(d_mul(row[6], 3.141592653589793), 360.0);
 }
 
 // The three camera angles of env i (heading, pitch, half the vertical field of view), float64.
@@ -163,10 +190,9 @@ MWB_DEV void camera_common(const DevState& S, int i, Camera& c) {
 // sin / cos so that the oracle, fed the same (pos, dir, cam_*) doubles on the host, derives the
 // identical float32 basis.  (The six evaluations are independent: the kernel spreads them over
 // six threads.)
-// The agent at (px, py, pz); every camera parameter is env i's.
-MWB_DEV Camera make_camera_at(const DevState& S, int i, double px, double py, double pz, const double trig[6]) {
-  const size_t N = S.N;
-  double h = S.cam[0 * N + i], fd = S.cam[1 * N + i];
+// The agent at (px, py, pz), the camera h above it and fd ahead of it; every other camera parameter is env i's.
+MWB_DEV Camera make_camera_at(const DevState& S, int i, double px, double py, double pz, double h, double fd,
+                              const double trig[6]) {
   const double ct = trig[0], st = trig[1], cp = trig[2], sp = trig[3];
   Camera c;
   c.ex = (float)d_add(px, d_mul(fd, ct));
@@ -196,7 +222,7 @@ MWB_DEV Camera make_camera(const DevState& S, int i, const double trig[6]) {
   const size_t N = S.N;
   const int as = S.agent_slot[i];
   const double px = S.ent_px[as * N + i], py = S.ent_py[as * N + i], pz = S.ent_pz[as * N + i];
-  return make_camera_at(S, i, px, py, pz, trig);
+  return make_camera_at(S, i, px, py, pz, S.cam[0 * N + i], S.cam[1 * N + i], trig);
 }
 
 // The perspective camera of a render launch (view.mode 0 or 2) from the trig frame_trig_kernel evaluated: the
@@ -204,15 +230,20 @@ MWB_DEV Camera make_camera(const DevState& S, int i, const double trig[6]) {
 MWB_DEV Camera make_view_camera(const DevState& S, int i, const ViewSpec& view, const double trig[6]) {
   const size_t N = S.N;
   const int as = S.agent_slot[i];
-  double px, pz;
+  double px, pz, h, fd;
   if (view.mode == 2) {
-    px = view.rows[(size_t)i * 3];
-    pz = view.rows[(size_t)i * 3 + 1];
+    const double* row = view.rows + (size_t)i * view.row_width;
+    px = row[0];
+    pz = row[1];
+    h = view_row_cam(S, i, row, view.row_width, 0);
+    fd = view_row_cam(S, i, row, view.row_width, 1);
   } else {
     px = S.ent_px[as * N + i];
     pz = S.ent_pz[as * N + i];
+    h = S.cam[0 * N + i];
+    fd = S.cam[1 * N + i];
   }
-  return make_camera_at(S, i, px, S.ent_py[as * N + i], pz, trig);
+  return make_camera_at(S, i, px, S.ent_py[as * N + i], pz, h, fd, trig);
 }
 
 // render_top_view's camera: the projection matrix entries are formed in float64 and rounded once, as
@@ -241,18 +272,20 @@ MWB_DEV Camera make_camera(const DevState& S, int i) {
   return make_camera(S, i, trig);
 }
 
-// The designed camera of env i, `row` = (x, z, dir): the agent's camera after agent.pos = (x, agent.pos[1], z),
-// agent.dir = dir -- the same float64 steps, so a row equal to the agent's pose gives the identical basis.
-MWB_DEV Camera make_row_camera(const DevState& S, int i, const double* row) {
+// The designed camera of env i, `row` = (x, z, dir[, cam_height, cam_fwd_disp, cam_pitch, cam_fov_y]): the agent's
+// camera after agent.pos = (x, agent.pos[1], z), agent.dir = dir and the given camera attributes set -- the same
+// float64 steps, so a row equal to the agent's pose and camera gives the identical basis.
+MWB_DEV Camera make_row_camera(const DevState& S, int i, const double* row, int width = 3) {
   double ang[3], trig[6];
   camera_angles(S, i, ang);
-  ang[0] = row[2];
+  view_row_angles(row, width, ang);
   for (int k = 0; k < 3; ++k) {
     trig[2 * k] = mwb_libm::cos_glibc(ang[k]);
     trig[2 * k + 1] = mwb_libm::sin_glibc(ang[k]);
   }
   const int as = S.agent_slot[i];
-  return make_camera_at(S, i, row[0], S.ent_py[as * (size_t)S.N + i], row[1], trig);
+  return make_camera_at(S, i, row[0], S.ent_py[as * (size_t)S.N + i], row[1], view_row_cam(S, i, row, width, 0),
+                        view_row_cam(S, i, row, width, 1), trig);
 }
 
 // vertex after the exact part of the pipeline: window-homogeneous position + z numerator

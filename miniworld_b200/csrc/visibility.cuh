@@ -88,20 +88,22 @@ MWB_DEV void empty_bbox(TriRec& r) {
 }
 
 #ifdef __CUDACC__
-// rows: null = the agent's camera; else [N][3] designed cameras (x, z, dir), a skipped row leaves mask[i] as it is
-template <int MSAA>
+// rows: null = the agent's camera; else [N][ROW_WIDTH] designed cameras (x, z, dir[, cam_height, cam_fwd_disp,
+// cam_pitch, cam_fov_y]), a skipped row leaves mask[i] as it is.  ROW_WIDTH is a template parameter so that the
+// instances for the agent's camera and 3-column rows are the code they were before 7-column rows existed.
+template <int MSAA, int ROW_WIDTH>
 __global__ void __launch_bounds__(256) visible_ents_kernel(DevState S, RenderAssets A, TriRec* __restrict__ scratch, int cap,
                                                            int box0, uint32_t* __restrict__ mask, const double* __restrict__ rows) {
   const int i = blockIdx.x, tid = threadIdx.x;
   const int W = S.obs_w, H = S.obs_h;
-  if (rows && view_row_skipped(rows + (size_t)i * 3)) return;     // uniform across the block
+  if (rows && view_row_skipped(rows + (size_t)i * ROW_WIDTH, ROW_WIDTH)) return;     // uniform across the block
   __shared__ Camera cam;
   __shared__ int ent_slot[32];
   __shared__ int n_query, n_room;
   __shared__ uint32_t vis_all;
   TriRec* tris = scratch + (size_t)i * cap;
   if (tid == 0) {
-    cam = rows ? make_row_camera(S, i, rows + (size_t)i * 3) : make_camera(S, i);
+    cam = rows ? make_row_camera(S, i, rows + (size_t)i * ROW_WIDTH, ROW_WIDTH) : make_camera(S, i);
     n_query = queried_entities(S, i, ent_slot);
     n_room = 0;
     vis_all = 0;

@@ -190,10 +190,11 @@ class ShardedMiniWorld:
         check(lib.mwb_flag_write(stream, self._done_ptr[self.rank], t))
         return None
 
-    def render_views(self, poses, render_agent=False, out=None, depth=None):
-        """BatchedMiniWorld.render_views on this rank's envs: `poses` holds rows for the local envs ([V, count, 3] or
-        [count, 3]), the rank's slice of the single-process rows, and the frames are that slice of its frames."""
-        return self.local.render_views(poses, render_agent=render_agent, out=out, depth=depth)
+    def render_views(self, poses, render_agent=False, out=None, depth=None, size=None, samples=None):
+        """BatchedMiniWorld.render_views on this rank's envs: `poses` holds rows for the local envs ([V, count, 3|7] or
+        [count, 3|7]), the rank's slice of the single-process rows, and the frames are that slice of its frames."""
+        return self.local.render_views(poses, render_agent=render_agent, out=out, depth=depth, size=size,
+                                       samples=samples)
 
     def step(self, local_actions):
         """Local K1 + K2, then the gather of obs / reward / flags to rank 0."""

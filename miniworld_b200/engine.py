@@ -146,6 +146,7 @@ EXPORTS = (
     "mwb_set_levels", "mwb_enable_level_changes", "mwb_state_in_host_memory", "mwb_set_level_maze",
     "mwb_enable_episode_seeds", "mwb_enable_maze_layouts", "mwb_enable_start_poses", "mwb_enable_state_bank",
     "mwb_save_states", "mwb_enable_reset_draws", "mwb_enable_goal_distance", "mwb_render_views", "mwb_visible_ents_from",
+    "mwb_render_views_at", "mwb_visible_ents_from_at",
     "mwb_enable_env_params",
 )
 OBS_FORMATS = {"hwc": 0, "cwh": 1, "grey": 2}
@@ -203,6 +204,8 @@ def load_library():
     lib.mwb_visible_ents.argtypes = [vp, vp, vp]
     lib.mwb_render_views.argtypes = [vp, vp, C.c_int, C.c_int, vp, vp, vp]
     lib.mwb_visible_ents_from.argtypes = [vp, vp, vp, vp]
+    lib.mwb_render_views_at.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp]
+    lib.mwb_visible_ents_from_at.argtypes = [vp, vp, C.c_int, vp, vp]
     lib.mwb_set_action_noise.argtypes = [vp, C.c_int, C.c_double, C.c_int]
     lib.mwb_set_obs_format.argtypes = [vp, C.c_int]
     lib.mwb_snapshot_size.argtypes = [vp, C.POINTER(C.c_size_t)]
@@ -617,21 +620,29 @@ class Engine:
         ext = (C.c_double * 4)(*[float(v) for v in extents])
         self._check(self.lib.mwb_render_top_view(self.h, ext, int(bool(render_agent)), _dev_or_host_ptr(obs), stream))
 
-    def visible_ents(self, mask, stream=None, poses=None):
+    def visible_ents(self, mask, stream=None, poses=None, row_width=3):
         """uint32[N] (numpy or CUDA tensor): bit e = entity slot e passes the reference's occlusion query -- from the
-        agent's camera, or with `poses` (float64 [N, 3] rows (x, z, dir)) from each env's designed camera
-        (mwb_visible_ents_from; a row with a non-finite entry leaves its entry as it is)."""
+        agent's camera, or with `poses` (float64 [N, row_width] rows (x, z, dir[, cam_height, cam_fwd_disp, cam_pitch,
+        cam_fov_y]), row_width 3 or 7) from each env's designed camera (mwb_visible_ents_from_at; a skipped row leaves
+        its entry as it is)."""
         if poses is None:
             self._check(self.lib.mwb_visible_ents(self.h, _dev_or_host_ptr(mask), stream))
         else:
-            self._check(self.lib.mwb_visible_ents_from(self.h, _dev_or_host_ptr(poses), _dev_or_host_ptr(mask), stream))
+            self._check(self.lib.mwb_visible_ents_from_at(self.h, _dev_or_host_ptr(poses), int(row_width),
+                                                          _dev_or_host_ptr(mask), stream))
 
-    def render_views(self, poses, views, obs=None, depth=None, render_agent=False, stream=None):
-        """Views of every env from designed cameras (mwb_render_views): poses float64 [views, N, 3] rows (x, z, dir),
-        obs [views, N, frame] in the observation format and / or depth float32 [views, N, H, W, 1] (numpy or CUDA
-        tensors, contiguous); frames of rows with a non-finite entry are left as they are."""
-        self._check(self.lib.mwb_render_views(self.h, _dev_or_host_ptr(poses), int(views), int(bool(render_agent)),
-                                              _dev_or_host_ptr(obs), _dev_or_host_ptr(depth), stream))
+    def render_views(self, poses, views, obs=None, depth=None, render_agent=False, stream=None, row_width=3, size=None,
+                     samples=None):
+        """Views of every env from designed cameras (mwb_render_views_at): poses float64 [views, N, row_width] rows
+        (x, z, dir[, cam_height, cam_fwd_disp, cam_pitch, cam_fov_y]), obs [views, N, frame] in the observation format
+        and / or depth float32 [views, N, H, W, 1] (numpy or CUDA tensors, contiguous) at size (W, H) (default: the
+        observation size) with `samples` samples per pixel (default: the handle's); frames of skipped rows are left as
+        they are."""
+        W, H = (self.W, self.H) if size is None else (int(size[0]), int(size[1]))
+        S = self.cfg.msaa_samples if samples is None else int(samples)
+        self._check(self.lib.mwb_render_views_at(self.h, _dev_or_host_ptr(poses), int(row_width), int(views), W, H, S,
+                                                 int(bool(render_agent)), _dev_or_host_ptr(obs), _dev_or_host_ptr(depth),
+                                                 stream))
 
     # name -> (mwb_state_array id, element type, shape): "env" = [N], "ents" = [max_ents, N], "level" = [count]
     # ([n_levels], or [slots] for bank_level),
@@ -804,8 +815,9 @@ class SingleEnvEngine:
         return {ent for slot, ent in enumerate(self._slots) if (int(mask[0]) >> slot) & 1}
 
     def render_view(self, pose, render_agent):
+        """pose: a 3- or 7-column row, rendered at this engine's own frame size and sample count"""
+        pose = np.asarray(pose, np.float64).reshape(1, 1, -1)
         obs = np.zeros((self.H, self.W, 3), np.uint8)
         depth = np.zeros((self.H, self.W, 1), np.float32)
-        self.engine.render_views(np.asarray(pose, np.float64).reshape(1, 1, 3), 1, obs=obs, depth=depth,
-                                 render_agent=render_agent)
+        self.engine.render_views(pose, 1, obs=obs, depth=depth, render_agent=render_agent, row_width=pose.shape[-1])
         return obs, depth

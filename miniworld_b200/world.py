@@ -239,6 +239,7 @@ class MiniWorldEnv(gym.Env):
         self.device = device
         self._engine = None
         self._vis_engine = None
+        self._view_engines = {}         # render_view at another (width, height, samples): one engine each
         self.reset()
 
     # ------------------------------------------------------------------ episode control
@@ -601,15 +602,41 @@ class MiniWorldEnv(gym.Env):
         self._push_world()
         return {e for e in eng.visible_ents() if any(e is x for x in self.entities)}
 
-    def render_view(self, x, z, dir, render_agent=False):
+    def render_view(self, x, z, dir, render_agent=False, cam_height=None, cam_fwd_disp=None, cam_pitch=None,
+                    cam_fov_y=None, size=None, samples=None):
         """(rgb uint8[H, W, 3], depth float32[H, W, 1]) from a designed camera: what render_obs() / render_depth()
-        return after agent.pos = (x, agent.pos[1], z), agent.dir = dir, without changing the agent.
-        `render_agent=True` also draws the agent's marker triangle at its real pose (a third-person view)."""
-        if not (math.isfinite(x) and math.isfinite(z) and abs(dir) < 105414350.0):
-            raise ValueError("render_view needs a finite x, z and |dir| < 105414350, got (%r, %r, %r)" % (x, z, dir))
-        eng = self._require_engine()
-        self._push_world()
-        return eng.render_view((float(x), float(z), float(dir)), render_agent)
+        return after agent.pos = (x, agent.pos[1], z), agent.dir = dir and each given camera attribute set, without
+        changing the agent.  `size` = (W, H) and `samples` render as into FrameBuffer(W, H, samples); they default to
+        the observation size and sample count.  `render_agent=True` also draws the agent's marker triangle at its real
+        pose (a third-person view).  Raises ValueError on a row BatchedMiniWorld.render_views would skip."""
+        intr = (cam_height, cam_fwd_disp, cam_pitch, cam_fov_y)
+        given = [v for v in intr if v is not None]
+        if not (math.isfinite(x) and math.isfinite(z) and abs(dir) < 105414350.0) or \
+                any(math.isinf(v) for v in given) or \
+                (cam_pitch is not None and not abs(cam_pitch) < 90) or \
+                (cam_fov_y is not None and not 0 < cam_fov_y < 180):
+            raise ValueError("render_view needs a finite x, z and |dir| < 105414350, finite camera attributes, "
+                             "|cam_pitch| < 90 and 0 < cam_fov_y < 180, got (%r, %r, %r, %r, %r, %r, %r)" % (
+                                 (x, z, dir) + intr))
+        W, H = (self.obs_width, self.obs_height) if size is None else (int(size[0]), int(size[1]))
+        S = self.msaa_samples if samples is None else int(samples)
+        if W <= 0 or H <= 0 or S not in (1, 4, 8, 16):
+            raise ValueError("render_view: size must be positive and samples 1, 4, 8 or 16, got %r, %r" % (size, samples))
+        if (W, H, S) == (self.obs_width, self.obs_height, self.msaa_samples):
+            eng = self._require_engine()
+            self._push_world()
+        else:
+            # one cached engine per (size, samples), whose own frame is that size, as for the human view
+            from .engine import SingleEnvEngine
+            self._require_engine()          # refuses device=None
+            eng = self._view_engines.get((W, H, S))
+            if eng is None:
+                eng = self._view_engines[(W, H, S)] = SingleEnvEngine(W, H, S, self.device)
+            eng.push(self, full=True)
+        row = (float(x), float(z), float(dir))
+        if given:
+            row += tuple(math.nan if v is None else float(v) for v in intr)
+        return eng.render_view(row, render_agent)
 
     def _require_vis_engine(self):
         if self.device is None:
@@ -638,3 +665,6 @@ class MiniWorldEnv(gym.Env):
             if getattr(self, name, None) is not None:
                 getattr(self, name).close()
                 setattr(self, name, None)
+        for eng in self._view_engines.values():
+            eng.close()
+        self._view_engines = {}
