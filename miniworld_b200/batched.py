@@ -547,7 +547,9 @@ class BatchedMiniWorld:
             max_ents = max([2] + [d.num_placed for d in defs])
         else:
             caps = [int(1.25 * len(g)) + 4 for g in d0.geometry]
-            max_ents = 8
+            # room for the definition instance's entity list (CollectHealth: 18 kits and the agent) and a carried
+            # object outside it
+            max_ents = max(8, len(d0.pe.entities) + 1)
         self.engine = eng = Engine(self.num_envs, self.obs_width, self.obs_height, msaa_samples,
                                    shared_geometry=self.device_reset and self.maze_template is None,
                                    max_rooms=caps[0], max_quads=caps[1], max_segs=caps[2], max_ents=max_ents,
